@@ -12,12 +12,15 @@ data-path collective (worlds are independent; SURVEY.md §8(e)).
   e2e          same metric through the host-buffer C-ABI call rlca_env_step_host (pinned host buffers in and out,
                PCIe traffic and a stream sync inside every call) — the reference-facing call
   roofline     algorithmic bytes (4*B+96 per agent-step, SURVEY.md §8(d)) / measured per-tick time vs the measured
-               HBM copy peak (MEASURED_PEAKS.json, else the 6650 GB/s fallback); traffic = DRAM bytes per launch
-               from the committed ncu capture of >= 130 consecutive ring launches (profiles/)
+               HBM copy peak (MEASURED_PEAKS.json, else the H100 SXM data-sheet 3350 GB/s); traffic = DRAM bytes per
+               launch from a committed capture under profiles/ when there is one
   cpu_baseline the CPU oracle (port of the reference semantics) on the host cores, bounded sample
   sections     (N = 1, outside the timed region, each with its own CPU-oracle figure) the other BASELINE configs:
                stage-2 tick, circle tick, raycast sweep, full PPO training, and the reference learner (stock PyTorch
                fp32) beside ours;  learner_dp (N > 1): the data-parallel minibatch step and its all-reduce share
+
+`--dump-outputs DIR` writes what the last timed tick handed its caller (scan, reward, flags, goal/speed, pose) as
+DIR/<name>.npy in float32; actions and seeds are fixed, so two builds can be compared output for output.
 
 `--impl reference` times the reference's CPU path.  The literal Stage+ROS+mpi4py stack cannot run here
 (BASELINE.md §4), so this is the oracle port with all host threads; it builds and loads the oracle only.
@@ -54,6 +57,14 @@ def random_actions(rng, n):
     return np.stack([rng.uniform(0.0, 1.0, n), rng.uniform(-1.0, 1.0, n)], 1).astype(np.float32)
 
 
+def dump_outputs(d, tensors):
+    """tensors -> d/<name>.npy as float32 (9 MB at the headline size)."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in tensors.items():
+        np.save(os.path.join(d, name + '.npy'), t.detach().cpu().numpy().astype(np.float32))
+
+
 def measured_peak():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
@@ -62,7 +73,7 @@ def measured_peak():
                 return float(json.load(f)['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'fallback (H100 SXM data sheet, 3.35 TB/s)'
 
 
 class ClockSampler:
@@ -245,7 +256,7 @@ def time_learner(dev, n_agents):
     pol = CNNPolicy(device=str(dev), max_batch=max(n_agents, 1024), seed=0)
     opt = Adam(pol.parameters(), lr=5e-5)
     lib = pol.lib
-    out = {'tensor_cores': 'tcgen05 3xTF32: conv tower forward/backward + fc1 forward/dW/dX'}
+    out = {'tensor_cores': 'wgmma 3xTF32: conv tower forward/backward + fc1 forward/dW/dX'}
     for nb, key in ((n_agents, 'policy_forward_us'), (1024, 'ppo_minibatch_step_us')):
         obs = torch.rand(nb, 1536, device=dev) - 0.5
         gs = torch.rand(nb, 4, device=dev)
@@ -592,6 +603,7 @@ def main():
     ap.add_argument('--no-cpu', action='store_true')
     ap.add_argument('--no-graph', action='store_true', help='launch every tick from Python instead of replaying a CUDA graph')
     ap.add_argument('--no-sections', action='store_true', help='skip the extra sections (stage2 / circle / sweep / train / learner)')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the outputs of the last timed tick to DIR/<name>.npy')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -641,7 +653,7 @@ def main():
     N = env.N
     rng = np.random.default_rng(1000 + rank)
     acts = [torch.from_numpy(random_actions(rng, N)).to(dev) for _ in range(64)]
-    # rollout-style obs ring: 128 slots x N x 512 f32 = 1.08 GB > 126 MB L2, so consecutive
+    # rollout-style obs ring: 128 slots x N x 512 f32 = 1.08 GB > 50 MB L2, so consecutive
     # ticks never re-hit obs lines in L2 (the 0.26 MB simulator state is L2-resident by design)
     ring = torch.empty(128, N, BEAMS, device=dev)
 
@@ -692,6 +704,10 @@ def main():
     sync()
     ms = e0.elapsed_time(e1)
     launches = (args.steps // G) * launches_per_graph if graph is not None else env.launch_count - l0
+    if args.dump_outputs and rank == 0:
+        last = (G if graph is not None else args.steps) - 1           # tick index that wrote the last timed scan
+        dump_outputs(args.dump_outputs, {'obs': ring[last % 128], 'reward': env.reward, 'flags': env.flags,
+                                         'goal_speed': env.gs, 'pose': env.state['pose']})
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
     if world_size > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -762,7 +778,7 @@ def main():
             'config': {'workload': WORKLOAD, 'seed': 0,
                        'agents_per_gpu': N, 'beams': BEAMS, 'parallelism': f'worlds sharded over {world_size} GPU(s), '
                        'no data-path collective',
-                       'l2': 'obs written round-robin into a 128-slot rollout ring (1.08 GB > 126 MB L2)',
+                       'l2': 'obs written round-robin into a 128-slot rollout ring (1.08 GB > 50 MB L2)',
                        'launch': (f'CUDA graph of {G} consecutive ticks replayed {args.steps // G}x ({launches_per_graph // max(G, 1)} kernels per tick: physics, lidar)'
                                   if graph is not None else 'one rlca_env_step call per tick from Python'),
                        'ctas_per_world': args.ctas_per_world or 'auto'},

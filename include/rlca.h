@@ -1,10 +1,10 @@
 /*
- * rlca.h — C ABI of the B200-native collision-avoidance hot path (librlca.so).
+ * rlca.h — C ABI of the H100-native collision-avoidance hot path (librlca.so).
  *
  * Drop-in boundary for the path BASELINE.json's north_star names.  The
  * reference has no FFI of its own (its seam is duck-typed Python over ROS
  * topics, SURVEY.md §8(b)); each entry point below states the reference
- * interface it replaces (file:line under /root/reference).
+ * interface it replaces (file:line in the reference).
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -253,7 +253,7 @@ int rlca_adam_step_allreduce(const uint64_t *grad_ptrs, const uint64_t *param_pt
                              const uint64_t *v_ptrs, uint64_t mc_grad, uint64_t mc_param, uint64_t mc_m, uint64_t mc_v,
                              int32_t rank, int32_t world, int64_t n, float lr, float beta1, float beta2, float eps,
                              int32_t step, float grad_scale, int32_t replicate_moments, void *stream);
-/* Conv tower + fc1 forward/backward GEMMs on the tcgen05 tensor cores with 3xTF32 error compensation
+/* Conv tower + fc1 forward/backward GEMMs on the Hopper tensor cores (wgmma) with 3xTF32 error compensation
  * (enable = 1, the default); 2 = fc1 GEMMs only; 0 selects the plain fp32 CUDA-core kernels (kept as the
  * cross-check for the tensor-core path). */
 int rlca_policy_set_tensor_cores(rlca_policy *pol, int32_t enable);

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Stage-1 trainer on the B200-native stack (drop-in for /root/reference/ppo_stage1.py).
+"""Stage-1 trainer on the H100-native stack (drop-in for the reference's ppo_stage1.py).
 
 Same hyper-parameters, log files and checkpoint names; `mpiexec -np 24` is replaced by one process per GPU:
     python ppo_stage1.py --num-worlds 43                       # 1 GPU, 43 x 24 = 1032 robots

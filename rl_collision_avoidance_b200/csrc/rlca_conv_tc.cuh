@@ -1,4 +1,4 @@
-// rlca_conv_tc.cuh — internal interface of the tcgen05 conv tower (rlca_conv_tc.cu).
+// rlca_conv_tc.cuh — internal interface of the wgmma conv tower (rlca_conv_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>

@@ -1,4 +1,4 @@
-// rlca_dp.cu — data-parallel optimizer step fused with its collective, over NVLink peer memory (sm_100a).
+// rlca_dp.cu — data-parallel optimizer step fused with its collective, over NVLink peer memory (sm_90a).
 //
 // The reference takes an Adam step per minibatch (model/ppo.py:186-188), so under data parallelism the gradient
 // all-reduce sits on the critical path of every step.  Instead of NCCL all-reduce (8.69 MB) followed by the Adam

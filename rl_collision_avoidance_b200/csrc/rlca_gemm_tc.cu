@@ -1,4 +1,4 @@
-// rlca_gemm_tc.cu — fp32-accurate tensor-core GEMM for the fc1 layer (sm_100a: tcgen05 + TMEM + TMA).
+// rlca_gemm_tc.cu — fp32-accurate tensor-core GEMM for the fc1 layer (sm_90a: wgmma + TMA + mbarriers).
 //
 //   C[M,N] = A[M,K] . B[N,K]^T          (both operands K-major, fp32 in HBM)
 //
@@ -6,14 +6,15 @@
 // north-star budget (losses within 1e-4 of the fp32 reference) rules out plain TF32/BF16 over K = 4096, so
 // the kernel runs "3xTF32": every operand is split on the fly into hi = tf32(x) and lo = x - hi (both exactly
 // representable), and D += A_hi B_hi + A_lo B_hi + A_hi B_lo on the tensor cores with fp32 accumulation in
-// TMEM; the dropped lo*lo term is ~2^-22 relative.
+// registers; the dropped lo*lo term is ~2^-22 relative.
 //
-// Structure (one CTA per 128 x BLOCK_N output tile and K split; 6 warps):
-//   warp 0   TMA producer: 4 tiles per k-block (A_hi, A_lo, B_hi, B_lo; 128B-swizzled, 32 fp32 per row)
-//            through a 3-stage full/empty mbarrier ring
-//   warp 1   TMEM allocator + MMA issuer: one elected thread issues 12 tcgen05.mma.kind::tf32 (M128,N128,K8)
-//            per k-block; tcgen05.commit releases the smem stage / signals the epilogue
-//   warps 2-5 epilogue: tcgen05.ld 32x32b -> registers -> (optional mask) -> global
+// Structure (one CTA per 128 x BLOCK_N output tile and K split; 3 warpgroups):
+//   warpgroup 0     TMA producer (one thread): 4 tiles per k-block (A_hi, A_lo, B_hi, B_lo; 128B-swizzled,
+//                   32 fp32 per row) through a 3-stage full/empty mbarrier ring
+//   warpgroups 1-2  consumers, rows 0..63 / 64..127 of the tile: 12 wgmma.m64n128k8 tf32 per k-block, one
+//                   commit group in flight; a stage is released once the group that read it has retired.
+//                   Epilogue: registers -> the warp's 16-row slab of the idle pipeline smem -> (optional mask)
+//                   -> row-wise coalesced global stores
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -32,13 +33,15 @@ namespace {
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_N = 128;
 constexpr int BLOCK_K = 32;            // 32 fp32 = 128 bytes = one swizzle-128B row
-constexpr int UMMA_K = 8;              // tf32: 32 bytes per MMA
+constexpr int MMA_K = 8;               // tf32: 32 bytes per MMA
 constexpr int STAGES = 3;
 constexpr int TILE_BYTES = BLOCK_M * BLOCK_K * 4;           // 16 KB (A and B tiles have the same shape)
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;                 // A_hi, A_lo, B_hi, B_lo
-constexpr int TMEM_COLS = 128;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 384;
+constexpr int EP = BLOCK_N + 8;        // epilogue slab pitch: the fragment's float2 stores are conflict free
 constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+static_assert(8 * 16 * EP * 4 <= STAGES * STAGE_BYTES, "epilogue slabs exceed the pipeline smem");
+static_assert(SMEM_BYTES <= 227 * 1024, "tc gemm exceeds the 227 KB shared-memory limit");
 
 struct TcArgs {
     float *C[2];               // per problem (tower)
@@ -59,8 +62,6 @@ tf32x3_gemm_kernel(const __grid_constant__ CUtensorMap mAh0, const __grid_consta
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + (size_t)STAGES * STAGE_BYTES);
     uint64_t *empty_bar = full_bar + STAGES;
-    uint64_t *tmem_full_bar = empty_bar + STAGES;
-    uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(tmem_full_bar + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int prob = blockIdx.z / args.k_splits;
@@ -75,24 +76,14 @@ tf32x3_gemm_kernel(const __grid_constant__ CUtensorMap mAh0, const __grid_consta
     const CUtensorMap *mBh = prob ? &mBh1 : &mBh0, *mBl = prob ? &mBl1 : &mBl0;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full_bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+        mbar_fence_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(tmem_ptr_smem)),
-                     "r"((uint32_t)TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ===== TMA producer =====
-        if (lane == 0) {
+        if (threadIdx.x == 0) {
             for (int i = 0; i < nkb; ++i) {
                 const int s = i % STAGES;
                 const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
@@ -106,86 +97,67 @@ tf32x3_gemm_kernel(const __grid_constant__ CUtensorMap mAh0, const __grid_consta
                 tma_load_2d(st + 3 * TILE_BYTES, mBl, &full_bar[s], k, n0);
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_tf32(BLOCK_M, BLOCK_N);
-            for (int i = 0; i < nkb; ++i) {
-                const int s = i % STAGES;
-                const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
-                mbar_wait(&full_bar[s], ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t sbase = smem_addr(smem + (size_t)s * STAGE_BYTES);
-#pragma unroll
-                for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                    const uint32_t koff = (uint32_t)k * UMMA_K * 4;     // bytes inside the 128B swizzle row
-                    const uint64_t ah = umma_desc_sw128(sbase + 0 * TILE_BYTES + koff);
-                    const uint64_t al = umma_desc_sw128(sbase + 1 * TILE_BYTES + koff);
-                    const uint64_t bh = umma_desc_sw128(sbase + 2 * TILE_BYTES + koff);
-                    const uint64_t bl = umma_desc_sw128(sbase + 3 * TILE_BYTES + koff);
-                    umma_tf32(tmem_base, al, bh, idesc, (i | k) ? 1u : 0u);   // small terms first
-                    umma_tf32(tmem_base, ah, bl, idesc, 1u);
-                    umma_tf32(tmem_base, ah, bh, idesc, 1u);
-                }
-                umma_commit(&empty_bar[s]);          // frees the smem stage when the MMAs above retire
-            }
-            umma_commit(tmem_full_bar);              // accumulator complete
-        }
-    } else {
-        // ===== epilogue: warps 2..5, TMEM lane quadrant = warp % 4 =====
-        // TMEM -> registers (lane = row) -> this warp's 32 x 128 slab of the idle pipeline smem (pitch 132: the
-        // row-per-lane float4 stores are conflict free) -> row-wise, fully coalesced 512-byte global stores (and
-        // mask loads): a lane-per-row store would touch 32 cache lines per instruction.
-        const int q = warp & 3;
-        mbar_wait(tmem_full_bar, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        constexpr int EP = BLOCK_N + 4;
-        float *slab = reinterpret_cast<float *>(smem) + (size_t)q * 32 * EP;
-#pragma unroll 1
-        for (int c = 0; c < BLOCK_N / 32; ++c) {
-            uint32_t r[32];
-            if (nkb > 0) {
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
-                tmem_ld_wait();
-            } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) r[j] = 0u;
-            }
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-                *reinterpret_cast<float4 *>(slab + lane * EP + c * 32 + j) = make_float4(
-                    __uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-        }
-        __syncwarp();
-        float *Cp = (prob ? args.C[1] : args.C[0]) + (size_t)split * args.split_stride;
-        const float *Mp = prob ? args.mask[1] : args.mask[0];
-        const int n = n0 + lane * 4;
-#pragma unroll 8
-        for (int i = 0; i < 32; ++i) {
-            const int m = m0 + q * 32 + i;
-            if (m >= args.M) break;
-            float4 v = *reinterpret_cast<const float4 *>(slab + i * EP + lane * 4);
-            float *dst = Cp + (size_t)m * args.ldc + n;
-            if (n + 4 <= args.N) {
-                if (Mp) {
-                    const float4 mk = *reinterpret_cast<const float4 *>(Mp + (size_t)m * args.ldc + n);
-                    v.x = mk.x > 0.f ? v.x : 0.f; v.y = mk.y > 0.f ? v.y : 0.f;
-                    v.z = mk.z > 0.f ? v.z : 0.f; v.w = mk.w > 0.f ? v.w : 0.f;
-                }
-                *reinterpret_cast<float4 *>(dst) = v;
-            } else {
-                const float vv[4] = {v.x, v.y, v.z, v.w};
-                for (int j = 0; j < 4 && n + j < args.N; ++j)
-                    dst[j] = (Mp && !(Mp[(size_t)m * args.ldc + n + j] > 0.f)) ? 0.f : vv[j];
-            }
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS)
-                     : "memory");
+    // ===== consumers: warpgroup c = rows 64c .. 64c+63 of the tile =====
+    const int c = (warp >> 2) - 1, w = warp & 3;
+    float acc[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc[j] = 0.0f;
+    for (int i = 0; i < nkb; ++i) {
+        const int s = i % STAGES;
+        const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t sbase = smem_addr(smem + (size_t)s * STAGE_BYTES);
+        const uint32_t a_base = sbase + (uint32_t)c * 64 * 128;      // 64 rows of 128 bytes
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+            const uint32_t koff = (uint32_t)k * MMA_K * 4;           // bytes inside the 128B swizzle row
+            const uint64_t ah = wgmma_desc_sw128(a_base + 0 * TILE_BYTES + koff);
+            const uint64_t al = wgmma_desc_sw128(a_base + 1 * TILE_BYTES + koff);
+            const uint64_t bh = wgmma_desc_sw128(sbase + 2 * TILE_BYTES + koff);
+            const uint64_t bl = wgmma_desc_sw128(sbase + 3 * TILE_BYTES + koff);
+            wgmma_tf32_n128(acc, al, bh);                            // small terms first
+            wgmma_tf32_n128(acc, ah, bl);
+            wgmma_tf32_n128(acc, ah, bh);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                             // the previous k-block's group has retired
+        if (i > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    // both consumer warpgroups are done with the pipeline smem before it becomes the epilogue slabs
+    named_bar_sync(1, 256);
+    // registers -> this warp's 16 x 128 slab (pitch EP) -> row-wise, fully coalesced 512-byte global stores (and mask
+    // loads): storing the fragment directly would touch 8 rows per instruction
+    float *slab = reinterpret_cast<float *>(smem) + (size_t)(c * 4 + w) * 16 * EP;
+#pragma unroll
+    for (int j = 0; j < 64; j += 2)
+        *reinterpret_cast<float2 *>(slab + (frag_row(0, lane, j)) * EP + frag_col(lane, j)) = make_float2(acc[j], acc[j + 1]);
+    __syncwarp();
+    float *Cp = (prob ? args.C[1] : args.C[0]) + (size_t)split * args.split_stride;
+    const float *Mp = prob ? args.mask[1] : args.mask[0];
+    const int n = n0 + lane * 4;
+#pragma unroll 4
+    for (int i = 0; i < 16; ++i) {
+        const int m = m0 + c * 64 + w * 16 + i;
+        if (m >= args.M) break;
+        float4 v = *reinterpret_cast<const float4 *>(slab + i * EP + lane * 4);
+        float *dst = Cp + (size_t)m * args.ldc + n;
+        if (n + 4 <= args.N) {
+            if (Mp) {
+                const float4 mk = *reinterpret_cast<const float4 *>(Mp + (size_t)m * args.ldc + n);
+                v.x = mk.x > 0.f ? v.x : 0.f; v.y = mk.y > 0.f ? v.y : 0.f;
+                v.z = mk.z > 0.f ? v.z : 0.f; v.w = mk.w > 0.f ? v.w : 0.f;
+            }
+            *reinterpret_cast<float4 *>(dst) = v;
+        } else {
+            const float vv[4] = {v.x, v.y, v.z, v.w};
+            for (int j = 0; j < 4 && n + j < args.N; ++j)
+                dst[j] = (Mp && !(Mp[(size_t)m * args.ldc + n + j] > 0.f)) ? 0.f : vv[j];
+        }
     }
 }
 

@@ -1,4 +1,4 @@
-// rlca_gemm_tc.cuh — internal interface of the tcgen05 3xTF32 GEMM (rlca_gemm_tc.cu).
+// rlca_gemm_tc.cuh — internal interface of the wgmma 3xTF32 GEMM (rlca_gemm_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 

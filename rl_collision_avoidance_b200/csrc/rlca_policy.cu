@@ -1,8 +1,8 @@
-// rlca_policy.cu — CNNPolicy forward/backward, PPO loss, GAE, Adam for sm_100a (C ABI in include/rlca.h).
+// rlca_policy.cu — CNNPolicy forward/backward, PPO loss, GAE, Adam for sm_90a (C ABI in include/rlca.h).
 //
 // Round-1 layout of the learner: every op is a hand-written CUDA kernel (no cuDNN/cuBLAS/ATen):
 //   conv tower   fused conv1+ReLU+conv2+ReLU per (sample, tower), activations in shared memory
-//   fc1 / fc2    tiled fp32 GEMM with fused bias / ReLU / mask epilogues (fc1 has a tcgen05 path in
+//   fc1 / fc2    tiled fp32 GEMM with fused bias / ReLU / mask epilogues (fc1 has a wgmma path in
 //                rlca_gemm_tc.cu when enabled)
 //   heads, sampling, PPO loss (+ its gradient), GAE (float64 recurrence), Adam: fused elementwise/reduction kernels
 // Parameters, gradients and Adam moments are flat fp32 buffers in state_dict order (tensor starts
@@ -104,7 +104,7 @@ struct rlca_policy {
     float *dZTs;     // [2][hi,lo][256][bpad]
     float *FTs;      // [2][hi,lo][4096][bpad]
     float *P;        // split-K partials [splits<=8][2][B][256]
-    int use_tc_conv; // conv tower on tcgen05 (rlca_conv_tc.cu); needs use_tc (it feeds the fc1 GEMM's hi/lo split)
+    int use_tc_conv; // conv tower on wgmma (rlca_conv_tc.cu); needs use_tc (it feeds the fc1 GEMM's hi/lo split)
     int num_sms;
     float *Wimg;     // pre-swizzled tf32 hi/lo image of the conv weights for the tensor-core conv tower
     float *WimgB;    // same for the backward kernel (per tower: conv1 weights | conv2 weights regrouped by tap)
@@ -130,8 +130,8 @@ struct rlca_policy {
 // split the same way (xe/xo) for conv1's stride-2 reads, and h1o is skewed by 16 floats so that the conv1 stores of
 // one warp (alternating even/odd s) spread over all 32 banks.
 // Weights come from a pre-transposed block Wc[tower] = w1t[15][32] | b1[32] | w2t[96][32] | b2[32] built by
-// conv_prep_weights_kernel, so staging them is a conflict-free linear copy (the in-kernel transpose used to cost
-// 39 % of this kernel's shared-memory wavefronts, profiles/README_r1.md).
+// conv_prep_weights_kernel, so staging them is a conflict-free linear copy (an in-kernel transpose would cause
+// shared-memory bank conflicts).
 #define CONV_WBLK 3616          // floats per tower in the prepared weight block
 #define CONV_SPC 4              // samples per CTA: amortises the 29 KB weight staging
 struct ConvSmem {
@@ -904,7 +904,7 @@ __global__ void adam_kernel(float *__restrict__ p, const float *__restrict__ g, 
 
 // The optimizer step of a policy workspace: Adam over the whole flat buffer AND the tf32 hi / lo split of the two fc1
 // weight matrices (97 % of the parameters) with their transposes, which the next forward / backward GEMMs read - the
-// split used to be a pass of its own at the head of every forward after a step (10 us at the critical path's start).
+// split would otherwise be a pass of its own at the head of every forward after a step, on the critical path.
 // Blocks below tile_blocks take a 32 x 32 tile of fc1w[tower] (coalesced rows in, coalesced rows out, the transposed
 // copies through a padded shared tile, as split_both_kernel); the others take the parameters outside those ranges
 // element-wise.  The arithmetic is adam_kernel's, expression for expression.
@@ -1256,8 +1256,8 @@ extern "C" int rlca_policy_set_grad_event(rlca_policy *pol, void *event)
     if (!pol) return rlca_set_err(RLCA_ERR_INVALID, "NULL workspace");
     pol->fc_grads_event = (cudaEvent_t)event;
     // The conv tower backward is a persistent kernel whose CTAs fill every SM's shared memory: an NCCL kernel launched
-    // meanwhile would only start when it ends.  While a gradient event is set it runs on 16 SMs fewer (measured at
-    // N = 2: the 46 us all-reduce then hides under the 147 us of dF GEMM + conv backward instead of following them).
+    // meanwhile would only start when it ends.  While a gradient event is set it runs on 16 SMs fewer, so that the
+    // all-reduce can run under the dF GEMM + conv backward instead of following them.
     pol->reserved_sms = event ? 16 : 0;
     if (event) { const char *e = getenv("RLCA_RESERVED_SMS"); if (e) pol->reserved_sms = atoi(e); }     // experiment knob
     return RLCA_OK;
@@ -1457,7 +1457,7 @@ extern "C" int rlca_policy_backward(rlca_policy *pol, const float *params, const
         pol->launches += 1;
     }
     if (pol->use_tc && side)
-        for (int t = 0; t < 2; ++t)      // (one launch per tower measured faster than the fused two-tower launch: 88 vs 124 us at 4104)
+        for (int t = 0; t < 2; ++t)      // one launch per tower (rather than one fused two-tower launch)
             rlca_tc_transpose_split(fsrc[t], nb, FEAT, FEAT, fth[t], ftl[t], (int)BP, s0);
     const int chunks = (nb + HEAD_CHUNK - 1) / HEAD_CHUNK;
     heads_bwd_kernel<<<chunks, 128, 0, s>>>(pol->H2, pol->dOut, params + tensor_offset(T_A1W),

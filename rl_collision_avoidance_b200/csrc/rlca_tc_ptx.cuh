@@ -1,5 +1,5 @@
-// rlca_tc_ptx.cuh — sm_100a PTX wrappers shared by the tensor-core kernels (rlca_gemm_tc.cu, rlca_conv_tc.cu):
-// mbarriers, TMA, tcgen05 (UMMA) descriptors / issue / commit, TMEM alloc + load.
+// rlca_tc_ptx.cuh — sm_90a PTX wrappers shared by the tensor-core kernels (rlca_gemm_tc.cu, rlca_conv_tc.cu):
+// mbarriers, TMA / bulk copies, wgmma (warpgroup MMA) shared-memory descriptors, issue, commit and wait.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -47,70 +47,84 @@ __device__ __forceinline__ void tma_bulk_g2s(void *dst, const void *src, uint32_
                  ::"r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar))
                  : "memory");
 }
-// generic-proxy shared-memory writes -> visible to the async proxy (tcgen05.mma operand reads, TMA)
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads, TMA)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads)
 {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 // K-major, 128B-swizzled operand tile: rows of 128 bytes, 8-row groups 1024 bytes apart (SBO), LBO unused (=1),
-// descriptor version 1 (Blackwell), layout type 2 = SWIZZLE_128B.  (cute::UMMA::SmemDescriptor.)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr)
+// layout type 1 = SWIZZLE_128B in the sm_90 encoding (bits 62-63).  A K step inside the 128-byte row is a plain
+// byte offset of the start address (the swizzle is applied to the final address bits).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr)
 {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// cute::UMMA::InstrDescriptor: c_format F32 (1) @4, a/b_format TF32 (2) @7/@10, K-major both, N>>3 @17, M>>4 @24
-__device__ __forceinline__ uint32_t umma_idesc_tf32(int m, int n)
+
+// wgmma.mma_async m64nNk8, tf32 x tf32 -> f32, both operands K-major from shared memory, D += A.B^T.  Issued by a
+// whole warpgroup (128 threads).  Accumulator fragment of thread t (warp w = (t / 32) % 4, lane l), register j:
+//   row = 16 w + l / 4 + 8 ((j / 2) % 2),   column = 8 (j / 4) + 2 (l % 4) + j % 2
+__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t a, uint64_t b)
 {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(a), "l"(b), "r"(1));
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc)
+// (d0 = columns 0..31, d1 = columns 32..63)
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d0)[16], float (&d1)[16], uint64_t a, uint64_t b)
 {
-    asm volatile("{\n\t.reg .pred p;\n\t"
-                 "setp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-                 : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_addr(bar))
-                 : "memory");
-}
-// whole-warp (sync.aligned) TMEM allocation of `cols` columns (power of two >= 32); base address lands in *dst_smem
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t cols)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(dst_smem)), "r"(cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t base, uint32_t cols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(cols) : "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread i of the warp gets lane (base lane + i), registers = consecutive columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
                  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-                   "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-                   "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-                   "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+                 : "+f"(d0[0]), "+f"(d0[1]), "+f"(d0[2]), "+f"(d0[3]), "+f"(d0[4]), "+f"(d0[5]), "+f"(d0[6]), "+f"(d0[7]),
+                   "+f"(d0[8]), "+f"(d0[9]), "+f"(d0[10]), "+f"(d0[11]), "+f"(d0[12]), "+f"(d0[13]), "+f"(d0[14]), "+f"(d0[15]),
+                   "+f"(d1[0]), "+f"(d1[1]), "+f"(d1[2]), "+f"(d1[3]), "+f"(d1[4]), "+f"(d1[5]), "+f"(d1[6]), "+f"(d1[7]),
+                   "+f"(d1[8]), "+f"(d1[9]), "+f"(d1[10]), "+f"(d1[11]), "+f"(d1[12]), "+f"(d1[13]), "+f"(d1[14]), "+f"(d1[15])
+                 : "l"(a), "l"(b), "r"(1));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t a, uint64_t b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a), "l"(b), "r"(1));
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching accumulator registers across wgmma issue / wait
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R])
+{
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// fragment coordinates of register j for lane l of warp w (see above)
+__device__ __forceinline__ int frag_row(int w, int l, int j) { return 16 * w + (l >> 2) + 8 * ((j >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int l, int j) { return 8 * (j >> 2) + 2 * (l & 3) + (j & 1); }
 
 // exact tf32 head of x (low 13 mantissa bits cleared); x - tf32_hi(x) is exact in fp32
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }

@@ -152,7 +152,7 @@ class CNNPolicy:
         return self._ws
 
     def set_tensor_cores(self, enable=True):
-        """Conv tower + fc1 GEMMs on tcgen05 with 3xTF32 compensation (True, default), fc1 GEMMs only (2),
+        """Conv tower + fc1 GEMMs on wgmma with 3xTF32 compensation (True, default), fc1 GEMMs only (2),
         or everything on the fp32 CUDA-core kernels (False)."""
         self.tensor_cores = 2 if enable == 2 and enable is not True else bool(enable)
         if self._ws is not None:

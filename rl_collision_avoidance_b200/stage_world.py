@@ -21,7 +21,7 @@ Result codes: 0 none, 1 'Reach Goal', 2 'Crashed', 3 'Time out'.
 
 ROS topics, the stageros bridge and mpi4py gather/scatter are gone: the batch is
 already "gathered" on the device.  All compute is in librlca.so (hand-written
-sm_100a CUDA behind the C ABI of include/rlca.h); torch only owns the memory.
+sm_90a CUDA behind the C ABI of include/rlca.h); torch only owns the memory.
 """
 from __future__ import annotations
 

@@ -45,10 +45,13 @@ def test_fill_config_derived_fields():
     assert cfg.robots_per_world * cfg.num_worlds == 4104
 
 
-@pytest.mark.skipif(not os.path.exists('/root/reference/worlds/stage1.world'), reason='reference not mounted')
+WORLDS = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'worlds')
+
+
 def test_assets_reproduce_from_reference_worlds():
+    """The packaged maps equal what the reference's own world files (kept as fixtures with their bitmaps) parse to."""
     from rl_collision_avoidance_b200.worldfile import load_world
     for name in ('stage1', 'stage2'):
-        m = load_world(f'/root/reference/worlds/{name}.world')
+        m = load_world(os.path.join(WORLDS, f'{name}.world'))
         a = make_scenario(name).map
         assert np.array_equal(m.cells, a.cells) and (m.origin_cx, m.origin_cy) == (a.origin_cx, a.origin_cy)

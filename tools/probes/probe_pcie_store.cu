@@ -1,7 +1,7 @@
 // probe_pcie_store.cu — how fast can SM stores push a scan-sized buffer into mapped pinned host memory, and does the
 // store width matter?  (Background: rlca_env_step_host mirrors 8.4 MB of scans per call with 4-byte-per-lane stores,
 // i.e. 128 B per warp instruction, and the kernel then drains at ~46 GB/s; the DMA engine reaches ~57 GB/s.)
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o probe_pcie_store probe_pcie_store.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o probe_pcie_store probe_pcie_store.cu
 #include <cuda_runtime.h>
 #include <stdio.h>
 
