@@ -402,7 +402,8 @@ def test_env_surface_leftovers(built, scenario):
 
 
 def test_config_limits_are_rejected(built):
-    """range_cells >= 2048 would overflow the 12-bit fields of the lidar walk key: loud error, not wrong ranges."""
+    """range_cells >= 2048 would overflow the 12-bit fields of the lidar walk key, and max_reject < 1 leaves a spawn
+    without a try to take: loud errors, not wrong ranges or poses."""
     import ctypes as C
     from rl_collision_avoidance_b200 import _lib
     from rl_collision_avoidance_b200.scenarios import fill_config, make_scenario
@@ -413,6 +414,11 @@ def test_config_limits_are_rejected(built):
     h = C.c_void_p()
     assert lib.rlca_env_create(C.byref(cfg), C.byref(h)) != 0
     assert b'range_cells' in lib.rlca_last_error()
+    # a spawn takes at least one rejection-sampling try
+    cfg = fill_config(_lib.EnvConfig(), sc, num_worlds=1, beams=512)
+    cfg.max_reject = 0
+    assert lib.rlca_env_create(C.byref(cfg), C.byref(h)) != 0
+    assert b'max_reject' in lib.rlca_last_error()
 
 
 def test_circle_launch_shape_invariance(built):
