@@ -162,18 +162,7 @@ tf32x3_gemm_kernel(const __grid_constant__ CUtensorMap mAh0, const __grid_consta
 }
 
 // ---------------------------------------------------------------------------------------------- helpers
-// hi = x with the low 13 mantissa bits cleared (exact tf32), lo = x - hi (exact).  Optional transposed output.
-__global__ void split_kernel(const float *__restrict__ src, int rows, int cols, int ld, float *__restrict__ hi,
-                             float *__restrict__ lo, int ld_out)
-{
-    const int c = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
-    if (c >= cols || r >= rows) return;
-    const float x = src[(size_t)r * ld + c];
-    const float h = __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
-    hi[(size_t)r * ld_out + c] = h;
-    lo[(size_t)r * ld_out + c] = x - h;
-}
-
+// split(x): hi = x with the low 13 mantissa bits cleared (exact tf32), lo = x - hi (exact).
 // dst_{hi,lo}[c][r] = split(src[r][c]); 32x32 tiles through shared memory; dst rows padded to ld_out (zeros beyond rows)
 __global__ void transpose_split_kernel(const float *__restrict__ src, int rows, int cols, int ld, float *__restrict__ hi,
                                        float *__restrict__ lo, int ld_out)
@@ -236,13 +225,17 @@ __global__ void split_both_kernel(const SplitBothArgs a)
 }
 
 // X[t][m][n] = relu(sum_s P[s][t][m][n] + bias[t][n])   (fc1 epilogue after a split-K GEMM)
+// One thread per 4 columns of a row; rows and column groups are flattened over grid x (grid y is limited to 65535,
+// and a forward may have more rows than that).  N is a multiple of 4.
 __global__ void splitk_bias_relu_kernel(const float *__restrict__ P, int splits, long long split_stride,
                                         long long tower_stride, const float *__restrict__ bias0,
                                         const float *__restrict__ bias1, int M, int N, float *__restrict__ X0,
                                         float *__restrict__ X1, int ldx)
 {
-    const int n4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4, m = blockIdx.y, t = blockIdx.z;
-    if (n4 >= N || m >= M) return;
+    const int q = N / 4, t = blockIdx.z;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)M * q) return;
+    const int m = (int)(idx / q), n4 = (int)(idx - (long long)m * q) * 4;
     const float *p = P + (size_t)t * tower_stride + (size_t)m * N + n4;
     float4 acc = *reinterpret_cast<const float4 *>(p);
     for (int s = 1; s < splits; ++s) {
@@ -320,12 +313,6 @@ int rlca_tc_gemm(const RlcaTcProblem *pr, int nprob, int M, int N, int K, int ld
     return RLCA_OK;
 }
 
-void rlca_tc_split(const float *src, int rows, int cols, int ld, float *hi, float *lo, int ld_out, cudaStream_t s)
-{
-    dim3 grid((cols + 255) / 256, rows);
-    split_kernel<<<grid, 256, 0, s>>>(src, rows, cols, ld, hi, lo, ld_out);
-}
-
 void rlca_tc_transpose_split(const float *src, int rows, int cols, int ld, float *hi, float *lo, int ld_out, cudaStream_t s)
 {
     dim3 grid((cols + 31) / 32, (ld_out + 31) / 32);
@@ -347,6 +334,7 @@ void rlca_tc_splitk_bias_relu(const float *P, int splits, long long split_stride
                               const float *bias0, const float *bias1, int M, int N, float *X0, float *X1, int ldx,
                               cudaStream_t s)
 {
-    dim3 grid((N / 4 + 63) / 64, M, 2);
-    splitk_bias_relu_kernel<<<grid, 64, 0, s>>>(P, splits, split_stride, tower_stride, bias0, bias1, M, N, X0, X1, ldx);
+    const long long items = (long long)M * (N / 4);
+    dim3 grid((unsigned)((items + 255) / 256), 1, 2);
+    splitk_bias_relu_kernel<<<grid, 256, 0, s>>>(P, splits, split_stride, tower_stride, bias0, bias1, M, N, X0, X1, ldx);
 }

@@ -14,7 +14,6 @@ int rlca_tc_init();
 // C = A . B^T for 1 or 2 independent problems (the two towers) in one launch; K split into k_splits partial outputs.
 int rlca_tc_gemm(const RlcaTcProblem *pr, int nprob, int M, int N, int K, int ldc, int k_splits, long long split_stride,
                  cudaStream_t s);
-void rlca_tc_split(const float *src, int rows, int cols, int ld, float *hi, float *lo, int ld_out, cudaStream_t s);
 void rlca_tc_transpose_split(const float *src, int rows, int cols, int ld, float *hi, float *lo, int ld_out, cudaStream_t s);
 // both towers in one launch: hi/lo split in the source layout (pitch ldo; hi = lo = NULL skips it) and transposed
 // ([cols, rows], pitch ldt, zero-filled beyond `rows`)

@@ -96,6 +96,7 @@ struct rlca_policy {
     // ---- tensor-core (3xTF32) path for fc1: hi/lo splits of the operands, all K-major
     int use_tc;
     int weights_dirty;   // W1 hi/lo/transposed copies must be rebuilt at the next forward
+    int wimg_dirty;      // Wimg must be rebuilt before the tensor-core conv tower forward runs next
     int bpad;        // max_batch rounded up to 32 (row pitch of the transposed operands)
     float *Fs;       // [2 towers][hi,lo][B][4096]
     float *W1s;      // [2][hi,lo][256][4096]
@@ -1213,6 +1214,7 @@ extern "C" int rlca_policy_create(int32_t max_batch, rlca_policy **out)
         if (rc) return rc;
         p->use_tc = 1;
         p->weights_dirty = 1;
+        p->wimg_dirty = 1;
         p->wc_dirty = 1;
         rc = rlca_conv_tc_init();
         if (rc) return rc;
@@ -1267,6 +1269,7 @@ extern "C" int rlca_policy_weights_changed(rlca_policy *p)
 {
     if (!p) return rlca_set_err(RLCA_ERR_INVALID, "policy is NULL");
     p->weights_dirty = 1;
+    p->wimg_dirty = 1;
     p->conv_bwd_dirty = 1;
     p->wc_dirty = 1;
     p->w1_split_valid = 0;
@@ -1279,6 +1282,7 @@ extern "C" int rlca_policy_set_tensor_cores(rlca_policy *p, int32_t enable)
     p->use_tc = enable ? 1 : 0;
     p->use_tc_conv = enable == 1 ? 1 : 0;      // 2 = fc1 GEMMs only (conv tower on the CUDA cores)
     p->weights_dirty = 1;
+    p->wimg_dirty = 1;
     p->conv_bwd_dirty = 1;
     p->wc_dirty = 1;
     p->w1_split_valid = 0;
@@ -1303,11 +1307,13 @@ extern "C" int rlca_policy_forward(rlca_policy *pol, const float *params, const 
     cudaStream_t s = (cudaStream_t)stream;
     const TowerPtrs ta = tower_ptrs(params, 0), tc = tower_ptrs(params, 1);
     // the tensor-core conv tower stages the scan with 16-byte bulk copies; oddly aligned inputs take the CUDA-core kernel
+    // (which leaves Wimg as it is: its own dirty flag keeps it stale until the next forward that reads it)
     if (pol->use_tc && pol->use_tc_conv && ((uintptr_t)obs & 15) == 0) {
-        if (pol->weights_dirty) {
+        if (pol->wimg_dirty) {
             const float *w1[2] = {ta.cv1w, tc.cv1w}, *b1[2] = {ta.cv1b, tc.cv1b};
             const float *w2[2] = {ta.cv2w, tc.cv2w}, *b2[2] = {ta.cv2b, tc.cv2b};
             rlca_conv_tc_prep(w1, b1, w2, b2, pol->Wimg, s);
+            pol->wimg_dirty = 0;
             pol->launches += 1;
         }
         int rc = rlca_conv_tc_forward(obs, pol->Wimg, pol->F, pol->Fs, nb, pol->num_sms, s);
@@ -1603,6 +1609,7 @@ extern "C" int rlca_policy_adam_step(rlca_policy *pol, float *params, const floa
     }
     RLCA_CUDA_TRY(cudaGetLastError());
     pol->weights_dirty = 1;                       // the conv weight images are still rebuilt at the next forward / backward
+    pol->wimg_dirty = 1;
     pol->conv_bwd_dirty = 1;
     pol->wc_dirty = 1;
     pol->w1_split_valid = pol->use_tc ? 1 : 0;
