@@ -354,6 +354,54 @@ int rlca_gather_minibatch(const float *const *src_dev, const int32_t *row_floats
 int rlca_obs_stack_push(const float *stack_in_dev, const float *obs_dev, const uint8_t *flags_dev, int32_t n,
                         int32_t beams, float *stack_out_dev, void *stream);
 
+/* =====================================================================================
+ * Evaluation (csrc/rlca_eval.cu, DESIGN.md §9c): per-episode records and the metrics of the paper this reference
+ * accompanies - success rate, extra time, extra distance, average speed.
+ * ===================================================================================== */
+
+/* Per-agent tracking state, N = robots_per_world * num_worlds rows; the caller zeroes path / count / open and sets
+ * closed to -1 before the first tick it tracks.
+ *   path     length of the running episode's path so far, metres
+ *   count    episodes that ended so far; only the first `episodes` of them are recorded
+ *   closed   episode index (state meta.y) of the last ended episode, -1 = none: nothing is tracked until the agent
+ *            starts a new episode (auto_reset 0: the caller resets it; 2: its group re-spawns)
+ *   open     1 = the agent is in an episode that has not ended (written by every rlca_eval_track)
+ *   records  (N, episodes, 4) result code (1 Reach Goal, 2 Crashed, 3 Time out), ticks, path length, straight-line
+ *            start -> goal distance (init and goal of the eplog row) */
+typedef struct rlca_eval_state {
+    double *path_dev;
+    int32_t *count_dev;
+    int32_t *closed_dev;
+    int32_t *open_dev;
+    float *records_dev;
+    int32_t episodes;
+} rlca_eval_state;
+
+/* One launch after each rlca_env_step, with the same cfg, state buffers and io: reads the action, flags, eplog, the
+ * poses of state_in / state_out and the episode indices, and appends a record for every agent whose episode ended. */
+int rlca_eval_track(const rlca_env_config *cfg, const rlca_env_state *state_in, const rlca_env_state *state_out,
+                    const rlca_step_io *io, const rlca_eval_state *ev, void *stream);
+
+/* Per-world float64 partials of the records of worlds [world_begin, world_begin + world_count) of the shard, in a
+ * fixed order without atomics: partials_dev (world_count, RLCA_EVAL_NPARTIALS).  With T = ticks * dt and
+ * L = max(distance - goal_radius, 0), over the episodes that reached the goal: travel time T, extra time T - L / v_max,
+ * extra distance path - L, average speed path / T.  Totals are the partials summed in global world order. */
+#define RLCA_EVAL_REACHED 0          /* episodes with result 1 */
+#define RLCA_EVAL_CRASHED 1          /* result 2 */
+#define RLCA_EVAL_TIMED_OUT 2        /* result 3 */
+#define RLCA_EVAL_UNFINISHED 3       /* agents with fewer than `episodes` records that are in an episode */
+#define RLCA_EVAL_SUM_TIME 4         /* sum, sum of squares of travel time (4, 5), extra time (6, 7), */
+                                     /*   extra distance (8, 9), average speed (10, 11) */
+#define RLCA_EVAL_SUM_STRAIGHT 12    /* sum of the straight-line start -> goal distance */
+#define RLCA_EVAL_SUM_PATH 13        /* sum of the path length */
+#define RLCA_EVAL_NPARTIALS 14
+int rlca_eval_reduce(const rlca_env_config *cfg, const rlca_eval_state *ev, int32_t world_begin, int32_t world_count,
+                     double *partials_dev, void *stream);
+/* The same reduction from HOST buffers (no device needed; the code rlca_eval_reduce runs). */
+int rlca_eval_reduce_host(const rlca_env_config *cfg, const float *records_host, const int32_t *count_host,
+                          const int32_t *open_host, int32_t episodes, int32_t world_begin, int32_t world_count,
+                          double *partials_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

@@ -51,6 +51,18 @@ class StepIO(C.Structure):
                 ('eplog_dev', C.c_void_p), ('stack_in_dev', C.c_void_p), ('stack_out_dev', C.c_void_p)]
 
 
+class EvalState(C.Structure):
+    """Mirror of rlca_eval_state (include/rlca.h)."""
+    _fields_ = [('path_dev', C.c_void_p), ('count_dev', C.c_void_p), ('closed_dev', C.c_void_p),
+                ('open_dev', C.c_void_p), ('records_dev', C.c_void_p), ('episodes', C.c_int32)]
+
+
+# rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
+EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
+                 'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
+                 'sum_straight', 'sum_path')
+
+
 # every symbol include/rlca.h declares: (name, restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -98,6 +110,10 @@ SYMBOLS = {
     'rlca_gather_rows': (C.c_int, [_P, _P, C.c_int32, C.c_int32, _P, _P]),
     'rlca_gather_minibatch': (C.c_int, [_P, _P, C.c_int32, _P, C.c_int32, _P, _P]),
     'rlca_obs_stack_push': (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P]),
+    'rlca_eval_track': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), C.POINTER(EnvState), C.POINTER(StepIO),
+                                  C.POINTER(EvalState), _P]),
+    'rlca_eval_reduce': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EvalState), C.c_int32, C.c_int32, _P, _P]),
+    'rlca_eval_reduce_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

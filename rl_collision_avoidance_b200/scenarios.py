@@ -45,7 +45,74 @@ def _tables():
         return json.load(f)
 
 
-def make_scenario(name: str, map_: WorldMap | None = None, robots_per_world: int | None = None) -> Scenario:
+def _footprint_cells(sc_map: WorldMap, x, y, th):
+    """(K, P) cell rows, cols covering the footprint rectangles at poses (x, y, th): points every half cell over the
+    rectangle, edges included, in the kernels' cell convention cell = floor(coord * ppm) + origin."""
+    hl, hw = COMMON['half_len'], COMMON['half_wid']
+    step = 0.5 * sc_map.resolution
+    u = np.linspace(-hl, hl, int(math.ceil(2 * hl / step)) + 1)
+    v = np.linspace(-hw, hw, int(math.ceil(2 * hw / step)) + 1)
+    uu, vv = (a.ravel() for a in np.meshgrid(u, v))
+    c, s = np.cos(th)[:, None], np.sin(th)[:, None]
+    px = x[:, None] + c * uu - s * vv
+    py = y[:, None] + s * uu + c * vv
+    ppm = 1.0 / sc_map.resolution
+    return np.floor(py * ppm).astype(np.int64) + sc_map.origin_cy, np.floor(px * ppm).astype(np.int64) + sc_map.origin_cx
+
+
+def _rects_overlap(p, q):
+    """Separating-axis test of two footprint rectangles given as (x, y, theta); touching counts as overlapping."""
+    hl, hw = COMMON['half_len'], COMMON['half_wid']
+    corners = []
+    for x, y, th in (p, q):
+        c, s = math.cos(th), math.sin(th)
+        corners.append([(x + c * a - s * b, y + s * a + c * b) for a, b in ((hl, hw), (-hl, hw), (-hl, -hw), (hl, -hw))])
+    for th in (p[2], q[2]):
+        for ax in ((math.cos(th), math.sin(th)), (-math.sin(th), math.cos(th))):
+            pa = [cx * ax[0] + cy * ax[1] for cx, cy in corners[0]]
+            pb = [cx * ax[0] + cy * ax[1] for cx, cy in corners[1]]
+            if max(pa) < min(pb) or max(pb) < min(pa):
+                return False
+    return True
+
+
+def circle_layout(m: WorldMap, robots: int, radius: float):
+    """(init_tab, goal_tab) of `robots` robots on a circle of `radius` metres: robot i at r (cos 2 pi i/K, sin 2 pi i/K)
+    facing the centre (heading pi + 2 pi i/K wrapped to (-pi, pi]), its goal the antipode.  ValueError when K is
+    outside 2..RLCA_MAX_ROBOTS_PER_WORLD, a start footprint covers a non-free or off-map cell, or neighbouring start
+    footprints overlap."""
+    K = int(robots)
+    if not 2 <= K <= 64:
+        raise ValueError(f'circle: robots_per_world must be in 2..64, got {robots}')
+    r = float(radius)
+    if not r > 0:
+        raise ValueError(f'circle: radius must be > 0, got {radius}')
+    a = 2.0 * np.pi * np.arange(K) / K
+    x, y = r * np.cos(a), r * np.sin(a)
+    th = np.remainder(np.pi + a + np.pi, 2.0 * np.pi) - np.pi
+    th = np.where(th <= -np.pi, th + 2.0 * np.pi, th)
+    rows, cols = _footprint_cells(m, x, y, th)
+    inside = (rows >= 0) & (rows < m.grid_h) & (cols >= 0) & (cols < m.grid_w)
+    free = inside.copy()
+    free[inside] = m.cells[rows[inside], cols[inside]] == 0
+    bad = np.nonzero(~free.all(1))[0]
+    if len(bad):
+        raise ValueError(f'circle: the start footprint of robot {bad[0]} (K={K}, r={r}) is not in free cells')
+    for i in range(K):
+        j = (i + 1) % K
+        if i != j and _rects_overlap((x[i], y[i], th[i]), (x[j], y[j], th[j])):
+            raise ValueError(f'circle: start footprints of robots {i} and {j} overlap (K={K}, r={r})')
+    init = np.zeros((K, 4), np.float32)
+    init[:, 0], init[:, 1], init[:, 2] = x, y, th
+    goal = np.zeros((K, 4), np.float32)
+    goal[:, 0], goal[:, 1] = -x, -y
+    return init, goal
+
+
+def make_scenario(name: str, map_: WorldMap | None = None, robots_per_world: int | None = None,
+                  radius: float | None = None) -> Scenario:
+    """`robots_per_world` and `radius` shape the circle scenario (see circle_layout); both None, or 50 robots with no
+    radius, keep the shipped 50-row table of the reference's circle.world."""
     name = name.lower()
     if name == 'stage1':
         m = map_ or load_map(os.path.join(ASSETS, 'stage1_map.npz'))
@@ -72,12 +139,17 @@ def make_scenario(name: str, map_: WorldMap | None = None, robots_per_world: int
         return Scenario('stage2', 1, R, 200, 1.05, 1, m, init, goal, groups=tuple(t['groups']))
     if name == 'circle':
         m = map_ or load_map(os.path.join(ASSETS, 'circle_map.npz'))
-        t = _tables()['circle']
-        R = 50
-        init = np.zeros((R, 4), np.float32)
-        init[:, :3] = np.asarray(t['init_pose'], np.float64)
-        goal = np.zeros((R, 4), np.float32)
-        goal[:, :2] = np.asarray(t['goal_point'], np.float64)
+        if radius is None and robots_per_world in (None, 50):
+            t = _tables()['circle']
+            R = 50
+            init = np.zeros((R, 4), np.float32)
+            init[:, :3] = np.asarray(t['init_pose'], np.float64)
+            goal = np.zeros((R, 4), np.float32)
+            goal[:, :2] = np.asarray(t['goal_point'], np.float64)
+        else:
+            init, goal = circle_layout(m, 50 if robots_per_world is None else robots_per_world,
+                                       25.0 if radius is None else radius)
+            R = len(init)
         return Scenario('circle', 2, R, 10000, 0.7, 1, m, init, goal)
     raise ValueError(f'unknown scenario {name!r}')
 
