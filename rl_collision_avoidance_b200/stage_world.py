@@ -43,7 +43,8 @@ def _ptr(t):
 
 class StageWorld:
     def __init__(self, beam_num, index=0, num_env=None, *, scenario='stage1', num_worlds=1, device='cuda:0',
-                 seed=0, auto_reset=False, world_offset=0, raw_beams=None, map=None, ctas_per_world=0):
+                 seed=0, auto_reset=False, world_offset=0, raw_beams=None, map=None, ctas_per_world=0,
+                 max_reject=4096):
         if not torch.cuda.is_available():
             raise _lib.RlcaError('StageWorld needs a CUDA device: the simulator has no CPU path')
         self.lib = _lib.load()
@@ -57,7 +58,8 @@ class StageWorld:
         self.beam_mum = int(beam_num)           # (sic) the reference's attribute name, stage_world1.py:23
         self.N = self.num_env * self.num_worlds
         self.cfg = fill_config(_lib.EnvConfig(), self.sc, num_worlds=self.num_worlds, beams=self.beam_mum,
-                               raw_beams=raw_beams, auto_reset=auto_reset, seed=seed, world_offset=world_offset)
+                               raw_beams=raw_beams, auto_reset=auto_reset, seed=seed, world_offset=world_offset,
+                               max_reject=max_reject)
         torch.cuda.set_device(self.device)
         h = C.c_void_p()
         _lib.check(self.lib.rlca_env_create(C.byref(self.cfg), C.byref(h)))

@@ -6,16 +6,19 @@ from rl_collision_avoidance_b200.scenarios import fill_config, make_scenario
 
 
 def make_pair(scenario='stage1', num_worlds=3, beams=512, auto_reset=True, seed=0, ctas_per_world=0,
-              world_offset=0, raw_beams=None, gpu=True):
-    sc = make_scenario(scenario)
+              world_offset=0, raw_beams=None, gpu=True, robots_per_world=None, radius=None, max_reject=4096):
+    """`robots_per_world` and `radius` reshape stage 1 / circle (make_scenario); `max_reject` is the spawn sampler's
+    try budget."""
+    sc = make_scenario(scenario, robots_per_world=robots_per_world, radius=radius)
     ocfg = fill_config(OrcConfig(), sc, num_worlds=num_worlds, beams=beams, raw_beams=raw_beams,
-                       auto_reset=auto_reset, seed=seed, world_offset=world_offset)
+                       auto_reset=auto_reset, seed=seed, world_offset=world_offset, max_reject=max_reject)
     orc = OracleWorld(ocfg, sc.map.cells, sc.init_tab, sc.goal_tab)
     env = None
     if gpu:
         from rl_collision_avoidance_b200.stage_world import StageWorld
         env = StageWorld(beams, index=0, scenario=sc, num_worlds=num_worlds, seed=seed, auto_reset=auto_reset,
-                         ctas_per_world=ctas_per_world, world_offset=world_offset, raw_beams=raw_beams)
+                         ctas_per_world=ctas_per_world, world_offset=world_offset, raw_beams=raw_beams,
+                         max_reject=max_reject)
     return sc, env, orc
 
 
