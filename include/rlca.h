@@ -130,6 +130,16 @@ typedef struct rlca_step_io {
 int rlca_walk_tables_host(float range_cells, int32_t *kr, int32_t *nslots, int32_t *nentries, int16_t *slot_keys,
                           uint16_t *keyslot, uint32_t *inv_off, uint32_t *inv_ent);
 
+/* The same inverse lists as the small-map lidar reads them when the range has at most 255 slots (RLCA_ERR_UNSUPPORTED
+ * otherwise).  Call with NULL buffers for the sizes, then with
+ *   records   [4 * nrecords] uint32, one 16-byte record per relative cell (nrecords = (2 kr + 1)^2):
+ *             word 0 = list length (bits 0-7) | offset of the list's 7th entry in `overflow` (bits 8-31),
+ *             words 1-3 = entries 0-5, two per word (the even entry in the low half)
+ *   overflow  [noverflow] uint16, entries 6, 7, ... of every list, lists in relative-cell order
+ * An entry is slot | dominant-axis distance << 8; the order of a list is that of inv_ent. */
+int rlca_inv_records_host(float range_cells, int32_t *nrecords, int32_t *noverflow, uint32_t *records,
+                          uint16_t *overflow);
+
 typedef struct rlca_env rlca_env;
 
 /* Replaces StageNode construction + world->Load (stageros.cpp:311-355): creates the

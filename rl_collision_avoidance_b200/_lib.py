@@ -67,6 +67,7 @@ EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 's
 _P = C.c_void_p
 SYMBOLS = {
     'rlca_walk_tables_host': (C.c_int, [C.c_float, _P, _P, _P, _P, _P, _P, _P]),
+    'rlca_inv_records_host': (C.c_int, [C.c_float, _P, _P, _P, _P]),
     'rlca_env_create': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(_P)]),
     'rlca_env_destroy': (C.c_int, [_P]),
     'rlca_env_set_map': (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
