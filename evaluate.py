@@ -2,11 +2,13 @@
 """Deterministic evaluation of a policy on stage 1, stage 2 or the circle swap, with the metrics of the paper the
 reference accompanies (DESIGN.md §9c): success / crash / time-out rates, and over the successful episodes the mean and
 population std of extra time, extra distance and average speed.  Every robot drives with the policy's mean action
-until it has --episodes recorded episodes (circle: one) or --max-ticks ticks have run.
+(--policy) or with the ORCA-DD baseline controller (--baseline orca, DESIGN.md §9d) until it has --episodes recorded
+episodes (circle: one) or --max-ticks ticks have run.
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
         --circle-robots 24 --circle-radius 12 --json circle.json
+    python evaluate.py --scenario stage2 --baseline orca --num-worlds 8 --episodes 3
 """
 import argparse
 import json
@@ -16,6 +18,7 @@ import torch
 
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, evaluate
 from rl_collision_avoidance_b200.model.net import CNNPolicy
+from rl_collision_avoidance_b200.orca import DEFAULTS as ORCA_DEFAULTS, OrcaController
 from rl_collision_avoidance_b200.scenarios import make_scenario
 from rl_collision_avoidance_b200.stage_world import StageWorld
 
@@ -27,7 +30,14 @@ CIRCLE_MAX_TICKS = 1500          # 25 m radius: the 49.5 m to the goal radius ta
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split('\n\n')[0])
     ap.add_argument('--scenario', required=True, choices=sorted(AUTO_RESET))
-    ap.add_argument('--policy', required=True, help='state_dict of CNNPolicy (e.g. tests/golden/checkpoints/stage2.pth)')
+    who = ap.add_mutually_exclusive_group(required=True)
+    who.add_argument('--policy', help='state_dict of CNNPolicy (e.g. tests/golden/checkpoints/stage2.pth)')
+    who.add_argument('--baseline', choices=['orca'], help='drive with the ORCA-DD controller instead of a policy')
+    ap.add_argument('--orca-radius', type=float, default=ORCA_DEFAULTS['radius'], help='robot radius, m')
+    ap.add_argument('--orca-horizon', type=float, default=ORCA_DEFAULTS['time_horizon'], help='time horizon tau, s')
+    ap.add_argument('--orca-neighbour-dist', type=float, default=ORCA_DEFAULTS['neighbour_dist'],
+                    help='neighbours are the robots closer than this, m')
+    ap.add_argument('--orca-gain', type=float, default=ORCA_DEFAULTS['heading_gain'], help='heading gain k_w, 1/s')
     ap.add_argument('--num-worlds', type=int, default=1)
     ap.add_argument('--episodes', type=int, default=1, help='recorded episodes per robot (circle: at most 1)')
     ap.add_argument('--seed', type=int, default=0)
@@ -38,7 +48,7 @@ def main(argv=None):
     ap.add_argument('--check-every', type=int, default=50)
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
-    if not os.path.exists(args.policy):
+    if args.policy is not None and not os.path.exists(args.policy):
         ap.error('policy file %s not found' % args.policy)
     if args.scenario != 'circle' and (args.circle_robots is not None or args.circle_radius is not None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
@@ -46,20 +56,28 @@ def main(argv=None):
         if args.scenario == 'circle' else make_scenario(args.scenario)
     env = StageWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, seed=args.seed,
                      auto_reset=AUTO_RESET[args.scenario])
-    policy = CNNPolicy(frames=LASER_HIST, action_space=2, max_batch=env.N)
-    policy.load_state_dict(torch.load(args.policy, map_location='cuda'))
+    if args.baseline == 'orca':
+        policy = OrcaController(env, radius=args.orca_radius, neighbour_dist=args.orca_neighbour_dist,
+                                time_horizon=args.orca_horizon, heading_gain=args.orca_gain)
+        controller = 'orca-dd'
+    else:
+        policy = CNNPolicy(frames=LASER_HIST, action_space=2, max_batch=env.N)
+        policy.load_state_dict(torch.load(args.policy, map_location='cuda'))
+        controller = None
     max_ticks = args.max_ticks if args.max_ticks is not None else \
         (CIRCLE_MAX_TICKS if args.scenario == 'circle' else args.episodes * (sc.timeout + 1))
     out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every)
     m = out['metrics']
     f = lambda k: '%.3f +- %.3f' % m[k]
-    print('%s  robots %d  ticks %d  episodes %d  success %.4f  crash %.4f  time-out %.4f  unfinished %d  '
+    print(('%s  ' % controller if controller else '') +
+          '%s  robots %d  ticks %d  episodes %d  success %.4f  crash %.4f  time-out %.4f  unfinished %d  '
           'extra time %s s  extra distance %s m  average speed %s m/s'
           % (args.scenario, env.N, out['ticks'], m['episodes'], m['success_rate'], m['crash_rate'], m['timeout_rate'],
              m['unfinished'], f('extra_time'), f('extra_distance'), f('average_speed')))
     if args.json:
         with open(args.json, 'w') as fh:
-            json.dump({'args': vars(args), 'robots': env.N, 'ticks': out['ticks'], 'metrics': m,
+            json.dump({'args': vars(args), 'controller': controller or 'policy', 'robots': env.N,
+                       'ticks': out['ticks'], 'metrics': m,
                        'columns': list(COLUMNS), 'totals': out['totals'].tolist(),
                        'partials': out['partials'].tolist()}, fh, indent=1)
     return out

@@ -412,6 +412,28 @@ int rlca_eval_reduce_host(const rlca_env_config *cfg, const float *records_host,
                           const int32_t *open_host, int32_t episodes, int32_t world_begin, int32_t world_count,
                           double *partials_host);
 
+/* =====================================================================================
+ * ORCA-DD baseline controller (csrc/rlca_orca.cu, DESIGN.md §9d): reciprocal velocity obstacles (van den Berg et al.
+ * 2011) over the robots of each world with a differential-drive heading tracker.  Not NH-ORCA; static map ignored.
+ * ===================================================================================== */
+
+/* One action per agent from the state the next rlca_env_step reads (pose, goal, meta of `state`): position, heading,
+ * goal, and the current velocity goal.z * (cos, sin)(theta), 0 when the stall flag meta.z is set.  Neighbours are the
+ * other robots of the same world closer than neighbour_dist; radius is one robot's (the pair's is 2 * radius),
+ * time_horizon is tau in s, heading_gain k_w in 1/s.
+ *   action_dev    (N,2) raw action (v, w) for rlca_env_step
+ *   velocity_dev  optional (N,2) ORCA velocity in the world frame
+ *   status_dev    optional (N) 0 = LP feasible, 1 = least-penetration fallback
+ * Every parameter must be finite and > 0 (RLCA_ERR_INVALID otherwise). */
+int rlca_orca_action(const rlca_env_config *cfg, const rlca_env_state *state, float radius, float neighbour_dist,
+                     float time_horizon, float heading_gain, float *action_dev, float *velocity_dev,
+                     int32_t *status_dev, void *stream);
+/* The same from HOST buffers (pose, goal: (N,4) float; meta: (N,4) int32), by serial loops over the same per-line code;
+ * the outputs equal rlca_orca_action's bit for bit.  velocity_host and status_host may be NULL. */
+int rlca_orca_action_host(const rlca_env_config *cfg, const float *pose_host, const float *goal_host,
+                          const int32_t *meta_host, float radius, float neighbour_dist, float time_horizon,
+                          float heading_gain, float *action_host, float *velocity_host, int32_t *status_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

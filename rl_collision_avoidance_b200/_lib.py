@@ -115,6 +115,10 @@ SYMBOLS = {
                                   C.POINTER(EvalState), _P]),
     'rlca_eval_reduce': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EvalState), C.c_int32, C.c_int32, _P, _P]),
     'rlca_eval_reduce_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
+    'rlca_orca_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), C.c_float, C.c_float, C.c_float,
+                                   C.c_float, _P, _P, _P, _P]),
+    'rlca_orca_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_float, C.c_float, C.c_float, C.c_float,
+                                        _P, _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

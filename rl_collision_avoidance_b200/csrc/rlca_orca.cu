@@ -1,0 +1,433 @@
+// rlca_orca.cu — ORCA-DD baseline controller on the device (sm_90a), C ABI in include/rlca.h, DESIGN.md §9d.
+//
+// Reciprocal collision avoidance (van den Berg, Guy, Lin, Manocha, "Reciprocal n-body collision avoidance", 2011,
+// §4-5) for every robot of every world, from the simulator state the next rlca_env_step reads, followed by a
+// differential-drive heading tracker that turns the ORCA velocity into a raw (v, w) action.  This is not NH-ORCA: no
+// tracking-error radius, no non-holonomic constraint set, no static obstacles.
+//
+// One warp per agent, 8 agents per CTA.  The lanes build the half-planes of the world's other robots in parallel and
+// compact the in-range ones into per-warp shared memory in robot-index order.  The 2-D LP is the incremental one; the
+// 1-D LP of line i scans lines 0..i-1 across the lanes and combines the bounds with warp max / min (exact) and a ballot,
+// so it equals the serial loop bit for bit.  The least-penetration fallback (3-D LP) builds its projected lines the same
+// way.  rlca_orca_action_host runs the serial loops over the same per-line functions; -fmad=false on the device and
+// -ffp-contract=off on the host make both round alike.
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <math.h>
+
+#include "../../include/rlca.h"
+#include "rlca_common.cuh"
+
+#define ORCA_THREADS 256
+#define ORCA_WARPS (ORCA_THREADS / 32)
+#define ORCA_MAX_LINES (RLCA_MAX_ROBOTS_PER_WORLD - 1)
+#define ORCA_PARALLEL_EPS 1e-5f     // |det| of two unit directions below which lines count as parallel
+#define ORCA_STILL 1e-6f            // ORCA speeds at or below this give the action (0, 0)
+#define FULL_MASK 0xffffffffu
+
+// Half-plane {v : det(d, v - p) >= 0}: the allowed side is left of the unit direction d.
+struct OrcaLine {
+    float px, py, dx, dy;
+};
+
+struct OrcaAgent {
+    float px, py, vx, vy, ct, st;
+};
+
+struct OrcaParams {
+    float r;            // combined radius 2 * radius
+    float nd2;          // neighbour_dist^2
+    float inv_tau, inv_dt;
+    float v_max, w_min, w_max, gain;
+};
+
+__host__ __device__ __forceinline__ float det2(float ax, float ay, float bx, float by) { return ax * by - ay * bx; }
+
+// Position, heading and current velocity of agent a: the last clipped command goal.z along the heading, 0 when the
+// last move was reverted (stall flag meta.z).
+__host__ __device__ __forceinline__ OrcaAgent orca_agent(const float4 *pose, const float4 *goal, const int4 *meta, int a)
+{
+    const float4 p = pose[a];
+    float s, c;
+    dev_sincosf(p.z, s, c);
+    const float v = meta[a].z ? 0.0f : goal[a].z;
+    OrcaAgent g;
+    g.px = p.x; g.py = p.y; g.vx = v * c; g.vy = v * s; g.ct = c; g.st = s;
+    return g;
+}
+
+__host__ __device__ __forceinline__ bool orca_in_range(const OrcaAgent &a, const OrcaAgent &b, float nd2)
+{
+    const float dx = b.px - a.px, dy = b.py - a.py;
+    return dx * dx + dy * dy < nd2;
+}
+
+// The ORCA half-plane agent a gets from neighbour b: u is the smallest change of the relative velocity that takes it
+// to the boundary of the velocity obstacle (truncated cone with horizon tau; when the pair already overlaps, the disk of
+// one time step), and a takes half of it.  False when the relative velocity is exactly the centre of the one-step disk,
+// where no direction is preferred; the neighbour then adds no line.
+__host__ __device__ __forceinline__ bool orca_line(const OrcaAgent &a, const OrcaAgent &b, const OrcaParams &q,
+                                                   OrcaLine &l)
+{
+    const float rpx = b.px - a.px, rpy = b.py - a.py;
+    const float rvx = a.vx - b.vx, rvy = a.vy - b.vy;
+    const float dist2 = rpx * rpx + rpy * rpy, r = q.r, r2 = r * r;
+    float ux, uy, dx, dy;
+    if (dist2 > r2) {
+        const float wx = rvx - q.inv_tau * rpx, wy = rvy - q.inv_tau * rpy;    // cut-off centre -> relative velocity
+        const float w2 = wx * wx + wy * wy, dot1 = wx * rpx + wy * rpy;
+        if (dot1 < 0.0f && dot1 * dot1 > r2 * w2) {
+            // nearest boundary point on the cut-off arc
+            const float wl = sqrtf(w2), nx = wx / wl, ny = wy / wl;
+            dx = ny; dy = -nx;
+            const float k = r * q.inv_tau - wl;
+            ux = k * nx; uy = k * ny;
+        } else {
+            // nearest boundary point on a leg: the direction is the leg's, pointing away from the apex on the left
+            // leg and towards it on the right one, so that the cone is on the right
+            const float leg = sqrtf(dist2 - r2);
+            if (det2(rpx, rpy, wx, wy) > 0.0f) {
+                dx = (rpx * leg - rpy * r) / dist2;
+                dy = (rpx * r + rpy * leg) / dist2;
+            } else {
+                dx = -(rpx * leg + rpy * r) / dist2;
+                dy = -(rpy * leg - rpx * r) / dist2;
+            }
+            const float t = rvx * dx + rvy * dy;
+            ux = t * dx - rvx; uy = t * dy - rvy;
+        }
+    } else {
+        const float wx = rvx - q.inv_dt * rpx, wy = rvy - q.inv_dt * rpy;
+        const float wl = sqrtf(wx * wx + wy * wy);
+        if (!(wl > 0.0f)) return false;
+        const float nx = wx / wl, ny = wy / wl;
+        dx = ny; dy = -nx;
+        const float k = r * q.inv_dt - wl;
+        ux = k * nx; uy = k * ny;
+    }
+    l.px = a.vx + 0.5f * ux;
+    l.py = a.vy + 0.5f * uy;
+    l.dx = dx;
+    l.dy = dy;
+    return true;
+}
+
+// v_pref = d * min(v_max / |d|, 1 / dt) with d = goal - p; 0 on the goal.
+__host__ __device__ __forceinline__ void orca_pref(const OrcaAgent &a, float4 goal, const OrcaParams &q, float &ox,
+                                                   float &oy)
+{
+    const float dx = goal.x - a.px, dy = goal.y - a.py, d = sqrtf(dx * dx + dy * dy);
+    if (d > 0.0f) {
+        const float k = fminf(q.v_max / d, q.inv_dt);
+        ox = dx * k; oy = dy * k;
+    } else {
+        ox = 0.0f; oy = 0.0f;
+    }
+}
+
+// Start of the 2-D LP: the optimum on the speed disk alone.
+__host__ __device__ __forceinline__ void lp2_start(float radius, float ox, float oy, bool dir_opt, float &rx, float &ry)
+{
+    if (dir_opt) {
+        rx = ox * radius; ry = oy * radius;
+    } else if (ox * ox + oy * oy > radius * radius) {
+        const float n = sqrtf(ox * ox + oy * oy);
+        rx = ox / n * radius; ry = oy / n * radius;
+    } else {
+        rx = ox; ry = oy;
+    }
+}
+
+__host__ __device__ __forceinline__ bool violates(const OrcaLine &l, float rx, float ry)
+{
+    return det2(l.dx, l.dy, l.px - rx, l.py - ry) > 0.0f;
+}
+
+// 1-D LP on line i: the interval [tl, tr] of p + t d inside the speed disk; false when the line misses the disk.
+__host__ __device__ __forceinline__ bool lp1_range(const OrcaLine &l, float radius, float &tl, float &tr)
+{
+    const float dot = l.px * l.dx + l.py * l.dy;
+    const float disc = dot * dot + radius * radius - (l.px * l.px + l.py * l.py);
+    if (disc < 0.0f) return false;
+    const float s = sqrtf(disc);
+    tl = -dot - s;
+    tr = -dot + s;
+    return true;
+}
+
+// The bound line k puts on t along line i: 1 = t <= b, -1 = t >= b, 0 = none (parallel, i inside k),
+// 2 = infeasible (parallel, i outside k).
+__host__ __device__ __forceinline__ int lp1_bound(const OrcaLine &li, const OrcaLine &lk, float &b)
+{
+    const float den = det2(li.dx, li.dy, lk.dx, lk.dy);
+    const float num = det2(lk.dx, lk.dy, li.px - lk.px, li.py - lk.py);
+    if (fabsf(den) <= ORCA_PARALLEL_EPS) return num < 0.0f ? 2 : 0;
+    b = num / den;
+    return den >= 0.0f ? 1 : -1;
+}
+
+// The optimum on line i within [tl, tr]: nearest to opt, or furthest along the direction opt.
+__host__ __device__ __forceinline__ void lp1_pick(const OrcaLine &l, float tl, float tr, float ox, float oy,
+                                                  bool dir_opt, float &rx, float &ry)
+{
+    float t;
+    if (dir_opt) t = (ox * l.dx + oy * l.dy > 0.0f) ? tr : tl;
+    else t = fminf(fmaxf(l.dx * (ox - l.px) + l.dy * (oy - l.py), tl), tr);
+    rx = l.px + t * l.dx;
+    ry = l.py + t * l.dy;
+}
+
+// Line of the least-penetration program of line i for an earlier line j: the points where the penetrations into i and
+// j are equal.  False when j is parallel to i and points the same way (it never binds before i does).
+__host__ __device__ __forceinline__ bool lp3_line(const OrcaLine &li, const OrcaLine &lj, OrcaLine &o)
+{
+    const float den = det2(li.dx, li.dy, lj.dx, lj.dy);
+    if (fabsf(den) <= ORCA_PARALLEL_EPS) {
+        if (li.dx * lj.dx + li.dy * lj.dy > 0.0f) return false;
+        o.px = 0.5f * (li.px + lj.px);
+        o.py = 0.5f * (li.py + lj.py);
+    } else {
+        const float t = det2(lj.dx, lj.dy, li.px - lj.px, li.py - lj.py) / den;
+        o.px = li.px + t * li.dx;
+        o.py = li.py + t * li.dy;
+    }
+    const float ex = lj.dx - li.dx, ey = lj.dy - li.dy, el = sqrtf(ex * ex + ey * ey);
+    o.dx = ex / el;
+    o.dy = ey / el;
+    return true;
+}
+
+// Heading tracker: the ORCA velocity in the robot's frame (c along the heading, s to its left) -> raw (v, w).
+__host__ __device__ __forceinline__ float2 orca_track(const OrcaAgent &a, float vx, float vy, const OrcaParams &q)
+{
+    const float n = sqrtf(vx * vx + vy * vy);
+    if (n <= ORCA_STILL) return make_float2(0.0f, 0.0f);
+    const float c = vx * a.ct + vy * a.st, s = vy * a.ct - vx * a.st;
+    if (c > 0.0f) return make_float2(fminf(c, q.v_max), fminf(fmaxf(q.gain * s / n, q.w_min), q.w_max));
+    return make_float2(0.0f, s >= 0.0f ? q.w_max : q.w_min);
+}
+
+// ------------------------------------------------------------------------------------ device: one warp per agent
+__device__ __forceinline__ float warp_max(float v)
+{
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(FULL_MASK, v, o));
+    return v;
+}
+__device__ __forceinline__ float warp_min(float v)
+{
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v = fminf(v, __shfl_xor_sync(FULL_MASK, v, o));
+    return v;
+}
+
+// 2-D LP over lines[0, n): returns the first line that makes it infeasible (the result is then the optimum of the lines
+// before it), or n.  Every lane holds the same result.
+__device__ int lp2_warp(const OrcaLine *lines, int n, float radius, float ox, float oy, bool dir_opt, float &rx,
+                        float &ry, int lane)
+{
+    lp2_start(radius, ox, oy, dir_opt, rx, ry);
+    for (int i = 0; i < n; ++i) {
+        const OrcaLine li = lines[i];
+        if (!violates(li, rx, ry)) continue;
+        float tl, tr;
+        bool ok = lp1_range(li, radius, tl, tr);
+        if (ok) {
+            float lo = -INFINITY, hi = INFINITY;
+            bool bad = false;
+            for (int k = lane; k < i; k += 32) {
+                float b;
+                const int kind = lp1_bound(li, lines[k], b);
+                if (kind == 2) bad = true;
+                else if (kind == 1) hi = fminf(hi, b);
+                else if (kind == -1) lo = fmaxf(lo, b);
+            }
+            tl = fmaxf(tl, warp_max(lo));
+            tr = fminf(tr, warp_min(hi));
+            ok = !__any_sync(FULL_MASK, bad) && tl <= tr;
+        }
+        if (!ok) return i;
+        lp1_pick(li, tl, tr, ox, oy, dir_opt, rx, ry);
+    }
+    return n;
+}
+
+// Least-penetration fallback from line `begin` on (the result holds the optimum of the lines before it).
+__device__ void lp3_warp(const OrcaLine *lines, int n, int begin, float radius, OrcaLine *proj, float &rx, float &ry,
+                         int lane)
+{
+    float dist = 0.0f;
+    for (int i = begin; i < n; ++i) {
+        const OrcaLine li = lines[i];
+        if (!(det2(li.dx, li.dy, li.px - rx, li.py - ry) > dist)) continue;
+        int np = 0;
+        for (int j0 = 0; j0 < i; j0 += 32) {
+            const int j = j0 + lane;
+            OrcaLine o;
+            const bool keep = j < i && lp3_line(li, lines[j], o);
+            const unsigned m = __ballot_sync(FULL_MASK, keep);
+            if (keep) proj[np + __popc(m & ((1u << lane) - 1u))] = o;
+            np += __popc(m);
+        }
+        __syncwarp();
+        const float sx = rx, sy = ry;
+        if (lp2_warp(proj, np, radius, -li.dy, li.dx, true, rx, ry, lane) < np) { rx = sx; ry = sy; }
+        dist = det2(li.dx, li.dy, li.px - rx, li.py - ry);
+        __syncwarp();
+    }
+}
+
+__global__ void __launch_bounds__(ORCA_THREADS) rlca_orca_kernel(int n, int R, OrcaParams q,
+                                                                  const float4 *__restrict__ pose,
+                                                                  const float4 *__restrict__ goal,
+                                                                  const int4 *__restrict__ meta,
+                                                                  float2 *__restrict__ action,
+                                                                  float2 *__restrict__ velocity,
+                                                                  int32_t *__restrict__ status)
+{
+    __shared__ OrcaLine s_lines[ORCA_WARPS][ORCA_MAX_LINES];
+    __shared__ OrcaLine s_proj[ORCA_WARPS][ORCA_MAX_LINES];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int a = blockIdx.x * ORCA_WARPS + warp;
+    if (a >= n) return;
+    const int base = a - a % R;
+    const OrcaAgent me = orca_agent(pose, goal, meta, a);
+    OrcaLine *lines = s_lines[warp];
+    int nl = 0;
+    for (int r0 = 0; r0 < R; r0 += 32) {
+        const int b = base + r0 + lane;
+        OrcaLine l;
+        bool keep = false;
+        if (r0 + lane < R && b != a) {
+            const OrcaAgent o = orca_agent(pose, goal, meta, b);
+            keep = orca_in_range(me, o, q.nd2) && orca_line(me, o, q, l);
+        }
+        const unsigned m = __ballot_sync(FULL_MASK, keep);
+        if (keep) lines[nl + __popc(m & ((1u << lane) - 1u))] = l;
+        nl += __popc(m);
+    }
+    __syncwarp();
+    float ox, oy, rx, ry;
+    orca_pref(me, goal[a], q, ox, oy);
+    const int fail = lp2_warp(lines, nl, q.v_max, ox, oy, false, rx, ry, lane);
+    if (fail < nl) lp3_warp(lines, nl, fail, q.v_max, s_proj[warp], rx, ry, lane);
+    if (lane == 0) {
+        action[a] = orca_track(me, rx, ry, q);
+        if (velocity) velocity[a] = make_float2(rx, ry);
+        if (status) status[a] = fail < nl;
+    }
+}
+
+// ------------------------------------------------------------------------------------ host: the serial loops
+static int lp2_host(const OrcaLine *lines, int n, float radius, float ox, float oy, bool dir_opt, float &rx, float &ry)
+{
+    lp2_start(radius, ox, oy, dir_opt, rx, ry);
+    for (int i = 0; i < n; ++i) {
+        const OrcaLine &li = lines[i];
+        if (!violates(li, rx, ry)) continue;
+        float tl, tr;
+        if (!lp1_range(li, radius, tl, tr)) return i;
+        for (int k = 0; k < i; ++k) {
+            float b;
+            const int kind = lp1_bound(li, lines[k], b);
+            if (kind == 2) return i;
+            if (kind == 1) tr = fminf(tr, b);
+            else if (kind == -1) tl = fmaxf(tl, b);
+            if (tl > tr) return i;
+        }
+        lp1_pick(li, tl, tr, ox, oy, dir_opt, rx, ry);
+    }
+    return n;
+}
+
+static void lp3_host(const OrcaLine *lines, int n, int begin, float radius, float &rx, float &ry)
+{
+    OrcaLine proj[ORCA_MAX_LINES];
+    float dist = 0.0f;
+    for (int i = begin; i < n; ++i) {
+        const OrcaLine &li = lines[i];
+        if (!(det2(li.dx, li.dy, li.px - rx, li.py - ry) > dist)) continue;
+        int np = 0;
+        for (int j = 0; j < i; ++j)
+            if (lp3_line(li, lines[j], proj[np])) ++np;
+        const float sx = rx, sy = ry;
+        if (lp2_host(proj, np, radius, -li.dy, li.dx, true, rx, ry) < np) { rx = sx; ry = sy; }
+        dist = det2(li.dx, li.dy, li.px - rx, li.py - ry);
+    }
+}
+
+static int check_args(const rlca_env_config *cfg, float radius, float neighbour_dist, float time_horizon,
+                      float heading_gain, OrcaParams &q)
+{
+    if (!cfg) return rlca_set_err(RLCA_ERR_INVALID, "cfg is NULL");
+    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
+        return rlca_set_err(RLCA_ERR_INVALID, "cfg has no robots");
+    if (!(cfg->dt > 0.0f) || !(cfg->v_max > 0.0f)) return rlca_set_err(RLCA_ERR_INVALID, "cfg needs dt > 0 and v_max > 0");
+    const float ps[4] = {radius, neighbour_dist, time_horizon, heading_gain};
+    for (float p : ps)
+        if (!(p > 0.0f && p < INFINITY))
+            return rlca_set_err(RLCA_ERR_INVALID, "ORCA radius, neighbour_dist, time_horizon and heading_gain must be "
+                                                  "finite and > 0");
+    q.r = 2.0f * radius;
+    q.nd2 = neighbour_dist * neighbour_dist;
+    q.inv_tau = 1.0f / time_horizon;
+    q.inv_dt = 1.0f / cfg->dt;
+    q.v_max = cfg->v_max;
+    q.w_min = cfg->w_min;
+    q.w_max = cfg->w_max;
+    q.gain = heading_gain;
+    return RLCA_OK;
+}
+
+extern "C" int rlca_orca_action(const rlca_env_config *cfg, const rlca_env_state *state, float radius,
+                                float neighbour_dist, float time_horizon, float heading_gain, float *action_dev,
+                                float *velocity_dev, int32_t *status_dev, void *stream)
+{
+    OrcaParams q;
+    int rc = check_args(cfg, radius, neighbour_dist, time_horizon, heading_gain, q);
+    if (rc) return rc;
+    if (!state || !state->pose_dev || !state->goal_dev || !state->meta_dev || !action_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_action: state or action buffer is NULL");
+    const int n = cfg->robots_per_world * cfg->num_worlds;
+    rlca_orca_kernel<<<(n + ORCA_WARPS - 1) / ORCA_WARPS, ORCA_THREADS, 0, (cudaStream_t)stream>>>(
+        n, cfg->robots_per_world, q, reinterpret_cast<const float4 *>(state->pose_dev),
+        reinterpret_cast<const float4 *>(state->goal_dev), reinterpret_cast<const int4 *>(state->meta_dev),
+        reinterpret_cast<float2 *>(action_dev), reinterpret_cast<float2 *>(velocity_dev), status_dev);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_orca_action_host(const rlca_env_config *cfg, const float *pose_host, const float *goal_host,
+                                     const int32_t *meta_host, float radius, float neighbour_dist, float time_horizon,
+                                     float heading_gain, float *action_host, float *velocity_host, int32_t *status_host)
+{
+    OrcaParams q;
+    int rc = check_args(cfg, radius, neighbour_dist, time_horizon, heading_gain, q);
+    if (rc) return rc;
+    if (!pose_host || !goal_host || !meta_host || !action_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_action_host: a buffer is NULL");
+    const float4 *pose = reinterpret_cast<const float4 *>(pose_host), *goal = reinterpret_cast<const float4 *>(goal_host);
+    const int4 *meta = reinterpret_cast<const int4 *>(meta_host);
+    const int R = cfg->robots_per_world, n = R * cfg->num_worlds;
+    OrcaLine lines[ORCA_MAX_LINES];
+    for (int a = 0; a < n; ++a) {
+        const int base = a - a % R;
+        const OrcaAgent me = orca_agent(pose, goal, meta, a);
+        int nl = 0;
+        for (int b = base; b < base + R; ++b) {
+            if (b == a) continue;
+            const OrcaAgent o = orca_agent(pose, goal, meta, b);
+            if (orca_in_range(me, o, q.nd2) && orca_line(me, o, q, lines[nl])) ++nl;
+        }
+        float ox, oy, rx, ry;
+        orca_pref(me, goal[a], q, ox, oy);
+        const int fail = lp2_host(lines, nl, q.v_max, ox, oy, false, rx, ry);
+        if (fail < nl) lp3_host(lines, nl, fail, q.v_max, rx, ry);
+        const float2 act = orca_track(me, rx, ry, q);
+        action_host[2 * a] = act.x;
+        action_host[2 * a + 1] = act.y;
+        if (velocity_host) { velocity_host[2 * a] = rx; velocity_host[2 * a + 1] = ry; }
+        if (status_host) status_host[a] = fail < nl;
+    }
+    return RLCA_OK;
+}
