@@ -177,21 +177,20 @@ __host__ __device__ __forceinline__ void lp1_pick(const OrcaLine &l, float tl, f
     ry = l.py + t * l.dy;
 }
 
-// Line of the least-penetration program of line i for an earlier line j: the points where the penetrations into i and
-// j are equal.  False when j is parallel to i and points the same way (it never binds before i does).
+// Line of the least-penetration program of line i for an earlier line j: the points v where the penetrations into i and
+// j are equal, det(e, v - p_i) = det(d_j, p_j - p_i) with e = d_j - d_i.  Its point is the one nearest to p_i, not the
+// crossing of i and j: for nearly parallel i and j the crossing lies far away (1e4 m for lines 0.1 m apart at
+// |det(d_i, d_j)| = 1e-5), and rounding it moves the line by up to 1e-3 m across i, which can cut the optimum off and
+// leave the fallback stuck above it.  False when j is parallel to i and points the same way (it never binds before i
+// does).
 __host__ __device__ __forceinline__ bool lp3_line(const OrcaLine &li, const OrcaLine &lj, OrcaLine &o)
 {
-    const float den = det2(li.dx, li.dy, lj.dx, lj.dy);
-    if (fabsf(den) <= ORCA_PARALLEL_EPS) {
-        if (li.dx * lj.dx + li.dy * lj.dy > 0.0f) return false;
-        o.px = 0.5f * (li.px + lj.px);
-        o.py = 0.5f * (li.py + lj.py);
-    } else {
-        const float t = det2(lj.dx, lj.dy, li.px - lj.px, li.py - lj.py) / den;
-        o.px = li.px + t * li.dx;
-        o.py = li.py + t * li.dy;
-    }
-    const float ex = lj.dx - li.dx, ey = lj.dy - li.dy, el = sqrtf(ex * ex + ey * ey);
+    if (fabsf(det2(li.dx, li.dy, lj.dx, lj.dy)) <= ORCA_PARALLEL_EPS && li.dx * lj.dx + li.dy * lj.dy > 0.0f)
+        return false;
+    const float h = det2(lj.dx, lj.dy, lj.px - li.px, lj.py - li.py);
+    const float ex = lj.dx - li.dx, ey = lj.dy - li.dy, e2 = ex * ex + ey * ey, el = sqrtf(e2), k = h / e2;
+    o.px = li.px - k * ey;
+    o.py = li.py + k * ex;
     o.dx = ex / el;
     o.dy = ey / el;
     return true;

@@ -10,6 +10,7 @@ Nothing here follows the structure of the CUDA code (incremental LPs); only the 
 """
 from __future__ import annotations
 
+from functools import lru_cache
 from itertools import combinations
 
 import numpy as np
@@ -82,6 +83,12 @@ def _line_circle(a, b, rad):
     return np.concatenate((foot + perp * h[:, None], foot - perp * h[:, None]))
 
 
+@lru_cache(maxsize=None)
+def _combinations(k, m):
+    """Index arrays (m, C(k, m)) of every m-subset of range(k), in itertools order."""
+    return np.array(list(combinations(range(k), m)), np.intp).reshape(-1, m).T
+
+
 def _solve2(a1, b1, a2, b2):
     det = a1[:, 0] * a2[:, 1] - a1[:, 1] * a2[:, 0]
     ok = np.abs(det) > 1e-12
@@ -101,7 +108,7 @@ def project(P, n, vmax, vpref):
         cands.append(vpref[None] + penetration(P, n, vpref)[:, None] * n)
         cands.append(_line_circle(n, c, vmax))
         if len(c) > 1:
-            i, j = np.array(list(combinations(range(len(c)), 2))).T
+            i, j = _combinations(len(c), 2)
             cands.append(_solve2(n[i], c[i], n[j], c[j]))
     v = np.concatenate(cands)
     ok = np.hypot(v[:, 0], v[:, 1]) <= vmax + FEAS_TOL
@@ -121,10 +128,10 @@ def min_max_penetration(P, n, vmax):
     k = len(c)
     cands = [vmax * n]
     if k > 1:
-        i, j = np.array(list(combinations(range(k), 2))).T
+        i, j = _combinations(k, 2)
         cands.append(_line_circle(n[j] - n[i], c[j] - c[i], vmax))
     if k > 2:
-        i, j, l = np.array(list(combinations(range(k), 3))).T
+        i, j, l = _combinations(k, 3)
         cands.append(_solve2(n[j] - n[i], c[j] - c[i], n[l] - n[i], c[l] - c[i]))
     v = np.concatenate(cands)
     v = v[np.hypot(v[:, 0], v[:, 1]) <= vmax + FEAS_TOL]

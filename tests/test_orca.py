@@ -4,44 +4,18 @@ import numpy as np
 import pytest
 
 import orca_ref
+from helpers import (ORCA_DT, ORCA_FALLBACK_GAP as FALLBACK_GAP, ORCA_VMAX, ORCA_WMAX, ORCA_WMIN, orca_cfg,
+                     orca_sweep_states, orca_world)
 from rl_collision_avoidance_b200 import _lib
 from rl_collision_avoidance_b200.orca import DEFAULTS, orca_host
 
-DT, VMAX, WMIN, WMAX = 0.1, 1.0, -1.0, 1.0
+DT, VMAX, WMIN, WMAX = ORCA_DT, ORCA_VMAX, ORCA_WMIN, ORCA_WMAX
 PARAMS = dict(DEFAULTS)
-
-
-def _cfg(worlds, robots):
-    c = _lib.EnvConfig()
-    c.robots_per_world, c.num_worlds = robots, worlds
-    c.dt, c.inv_dt = DT, np.float32(1.0) / np.float32(DT)
-    c.v_min, c.v_max, c.w_min, c.w_max = 0.0, VMAX, WMIN, WMAX
-    return c
+_cfg = orca_cfg
 
 
 def _world(rng, R, W, side):
-    """W worlds of R robots in a side x side box: random headings and last commands, some stalled robots and some on
-    their goals; world 0 also gets an overlapping pair and neighbours just inside / outside neighbour_dist."""
-    n = R * W
-    pose = np.zeros((n, 4), np.float32)
-    goal = np.zeros((n, 4), np.float32)
-    meta = np.zeros((n, 4), np.int32)
-    pose[:, 0:2] = rng.uniform(-side / 2, side / 2, (n, 2))
-    pose[:, 2] = rng.uniform(-np.pi, np.pi, n)
-    goal[:, 0:2] = rng.uniform(-10, 10, (n, 2))
-    goal[:, 2] = rng.uniform(0, VMAX, n)
-    goal[:, 3] = rng.uniform(WMIN, WMAX, n)
-    meta[:, 2] = rng.random(n) < 0.15
-    on_goal = rng.random(n) < 0.1
-    goal[on_goal, 0:2] = pose[on_goal, 0:2]
-    nd = PARAMS['neighbour_dist']
-    if R >= 2:
-        pose[1, 0:2] = pose[0, 0:2] + np.float32([0.3, 0.2])                       # overlap: the one-step branch
-    if R >= 4:
-        far = np.float32([np.cos(0.7), np.sin(0.7)])
-        pose[2, 0:2] = pose[0, 0:2] + (nd - 1e-3) * far                             # just inside
-        pose[3, 0:2] = pose[0, 0:2] - (nd + 1e-3) * far                             # just outside
-    return pose, goal, meta
+    return orca_world(rng, R, W, side, PARAMS['neighbour_dist'])
 
 
 CASES = [(1, 4, 8.0), (2, 4, 4.0), (5, 3, 6.0), (24, 3, 12.0), (50, 3, 10.0), (64, 3, 9.0), (64, 2, 5.0)]
@@ -52,7 +26,6 @@ def test_orca_host_matches_float64_reference(built):
     p = PARAMS
     seen = {0: 0, 1: 0}
     seen_overlap = seen_ranges = 0
-    gaps = []
     for R, W, side in CASES:
         pose, goal, meta = _world(rng, R, W, side)
         act, vel, status = orca_host(_cfg(W, R), pose, goal, meta, **p)
@@ -82,16 +55,38 @@ def test_orca_host_matches_float64_reference(built):
                 fstar, _ = orca_ref.min_max_penetration(P, n, VMAX)
                 assert ref is None or fstar > -1e-4, (R, a, fstar)
                 gap = orca_ref.penetration(P, n, v).max() - fstar
-                assert gap >= -1e-4, (R, a, fstar, gap)
-                gaps.append(gap)
+                assert -1e-4 <= gap <= FALLBACK_GAP, (R, a, fstar, gap)
             want = orca_ref.track(th[a], v, VMAX, WMIN, WMAX, p['heading_gain'])
             assert np.abs(act[a] - want).max() <= 1e-5, (R, a, act[a], want)
     assert seen[0] > 0 and seen[1] > 0, seen
     assert seen_overlap > 0 and seen_ranges > 0
-    # the incremental least-penetration program is not exact everywhere: at this seed 1 of the 337 fallback agents
-    # stops 0.065 above the optimum (DESIGN.md §9d)
-    gaps = np.array(gaps)
-    assert (gaps <= 1e-4).mean() >= 0.99 and gaps.max() <= 0.1, (len(gaps), (gaps > 1e-4).sum(), gaps.max())
+
+
+SWEEP_SEEDS = range(1, 9)
+
+
+def test_fallback_reaches_least_penetration_on_seeded_sweep(built):
+    """Every agent of the packed seeded worlds (helpers.ORCA_SWEEP, seeds 1-8: 4 336 agents, 2 689 of them in the
+    least-penetration fallback, up to 63 lines) gets the float64 optimum: status 0 within 1e-4 of the projection,
+    status 1 within FALLBACK_GAP of the least max-penetration.  Seed 3 holds the agent whose fallback stopped 0.33 above
+    the optimum when the projected lines were anchored at the crossing of the two lines (DESIGN.md §9d).  About 25 s on
+    8 CPU cores, mostly in orca_ref.min_max_penetration."""
+    p = PARAMS
+    fallback = 0
+    for (seed, R, W, side), (pose, goal, meta) in orca_sweep_states(SWEEP_SEEDS, p['neighbour_dist']):
+        _, vel, status = orca_host(_cfg(W, R), pose, goal, meta, **p)
+        pos, _, _ = orca_ref.agent_state(pose, goal, meta)
+        for a in range(R * W):
+            P, n = orca_ref.agent_lines(pose, goal, meta, R, a, p['radius'], p['neighbour_dist'], p['time_horizon'], DT)
+            v = vel[a].astype(np.float64)
+            if status[a] == 0:
+                ref = orca_ref.project(P, n, VMAX, orca_ref.preferred(pos[a], goal[a, 0:2], VMAX, DT))
+                assert ref is not None and np.abs(v - ref).max() <= 1e-4, (seed, R, side, a, v, ref)
+                continue
+            gap = orca_ref.penetration(P, n, v).max() - orca_ref.min_max_penetration(P, n, VMAX)[0]
+            assert -1e-4 <= gap <= FALLBACK_GAP, (seed, R, side, a, len(n), gap)
+            fallback += 1
+    assert fallback >= 2500, fallback
 
 
 def _state(xy, th, v, goal_xy, stalled=None):
