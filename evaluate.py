@@ -2,13 +2,15 @@
 """Deterministic evaluation of a policy on stage 1, stage 2 or the circle swap, with the metrics of the paper the
 reference accompanies (DESIGN.md §9c): success / crash / time-out rates, and over the successful episodes the mean and
 population std of extra time, extra distance and average speed.  Every robot drives with the policy's mean action
-(--policy) or with the ORCA-DD baseline controller (--baseline orca, DESIGN.md §9d) until it has --episodes recorded
-episodes (circle: one) or --max-ticks ticks have run.
+(--policy), with the ORCA-DD baseline controller (--baseline orca, DESIGN.md §9d) or with the paper's NH-ORCA baseline
+(--baseline nh-orca, DESIGN.md §9e) until it has --episodes recorded episodes (circle: one) or --max-ticks ticks have
+run.
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
         --circle-robots 24 --circle-radius 12 --json circle.json
     python evaluate.py --scenario stage2 --baseline orca --num-worlds 8 --episodes 3
+    python evaluate.py --scenario stage2 --baseline nh-orca --num-worlds 8 --episodes 3
 """
 import argparse
 import json
@@ -18,7 +20,7 @@ import torch
 
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, evaluate
 from rl_collision_avoidance_b200.model.net import CNNPolicy
-from rl_collision_avoidance_b200.orca import DEFAULTS as ORCA_DEFAULTS, OrcaController
+from rl_collision_avoidance_b200.orca import DEFAULTS as ORCA_DEFAULTS, NH_DEFAULTS, NhOrcaController, OrcaController
 from rl_collision_avoidance_b200.scenarios import make_scenario
 from rl_collision_avoidance_b200.stage_world import StageWorld
 
@@ -32,12 +34,20 @@ def main(argv=None):
     ap.add_argument('--scenario', required=True, choices=sorted(AUTO_RESET))
     who = ap.add_mutually_exclusive_group(required=True)
     who.add_argument('--policy', help='state_dict of CNNPolicy (e.g. tests/golden/checkpoints/stage2.pth)')
-    who.add_argument('--baseline', choices=['orca'], help='drive with the ORCA-DD controller instead of a policy')
-    ap.add_argument('--orca-radius', type=float, default=ORCA_DEFAULTS['radius'], help='robot radius, m')
+    who.add_argument('--baseline', choices=['orca', 'nh-orca'],
+                     help='drive with the ORCA-DD or the NH-ORCA controller instead of a policy')
+    ap.add_argument('--orca-radius', type=float, default=None,
+                    help='robot radius, m (default %g for orca, %g for nh-orca)'
+                    % (ORCA_DEFAULTS['radius'], NH_DEFAULTS['radius']))
     ap.add_argument('--orca-horizon', type=float, default=ORCA_DEFAULTS['time_horizon'], help='time horizon tau, s')
     ap.add_argument('--orca-neighbour-dist', type=float, default=ORCA_DEFAULTS['neighbour_dist'],
                     help='neighbours are the robots closer than this, m')
-    ap.add_argument('--orca-gain', type=float, default=ORCA_DEFAULTS['heading_gain'], help='heading gain k_w, 1/s')
+    ap.add_argument('--orca-gain', type=float, default=None,
+                    help='ORCA-DD heading gain k_w, 1/s (default %g)' % ORCA_DEFAULTS['heading_gain'])
+    ap.add_argument('--nh-error', type=float, default=NH_DEFAULTS['tracking_error'],
+                    help='NH-ORCA tracking error E, m')
+    ap.add_argument('--nh-heading-time', type=float, default=NH_DEFAULTS['heading_time'],
+                    help='NH-ORCA heading time T, s')
     ap.add_argument('--num-worlds', type=int, default=1)
     ap.add_argument('--episodes', type=int, default=1, help='recorded episodes per robot (circle: at most 1)')
     ap.add_argument('--seed', type=int, default=0)
@@ -50,6 +60,8 @@ def main(argv=None):
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
         ap.error('policy file %s not found' % args.policy)
+    if args.baseline != 'orca' and args.orca_gain is not None:
+        ap.error('--orca-gain applies to --baseline orca only')
     if args.scenario != 'circle' and (args.circle_robots is not None or args.circle_radius is not None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
     sc = make_scenario(args.scenario, robots_per_world=args.circle_robots, radius=args.circle_radius) \
@@ -57,9 +69,17 @@ def main(argv=None):
     env = StageWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, seed=args.seed,
                      auto_reset=AUTO_RESET[args.scenario])
     if args.baseline == 'orca':
-        policy = OrcaController(env, radius=args.orca_radius, neighbour_dist=args.orca_neighbour_dist,
-                                time_horizon=args.orca_horizon, heading_gain=args.orca_gain)
+        gain = ORCA_DEFAULTS['heading_gain'] if args.orca_gain is None else args.orca_gain
+        radius = ORCA_DEFAULTS['radius'] if args.orca_radius is None else args.orca_radius
+        policy = OrcaController(env, radius=radius, neighbour_dist=args.orca_neighbour_dist,
+                                time_horizon=args.orca_horizon, heading_gain=gain)
         controller = 'orca-dd'
+    elif args.baseline == 'nh-orca':
+        radius = NH_DEFAULTS['radius'] if args.orca_radius is None else args.orca_radius
+        policy = NhOrcaController(env, radius=radius, neighbour_dist=args.orca_neighbour_dist,
+                                  time_horizon=args.orca_horizon, tracking_error=args.nh_error,
+                                  heading_time=args.nh_heading_time)
+        controller = 'nh-orca'
     else:
         policy = CNNPolicy(frames=LASER_HIST, action_space=2, max_batch=env.N)
         policy.load_state_dict(torch.load(args.policy, map_location='cuda'))

@@ -434,6 +434,42 @@ int rlca_orca_action_host(const rlca_env_config *cfg, const float *pose_host, co
                           const int32_t *meta_host, float radius, float neighbour_dist, float time_horizon,
                           float heading_gain, float *action_host, float *velocity_host, int32_t *status_host);
 
+/* =====================================================================================
+ * NH-ORCA baseline controller (csrc/rlca_orca.cu, DESIGN.md §9e): ORCA for non-holonomic robots (Alonso-Mora,
+ * Breitenmoser, Rufli, Beardsley, Siegwart, DARS 2010), the paper's baseline.  Static map ignored.
+ *
+ * Tracking: a holonomic velocity at speed V and angle th in (-pi, pi] from the heading is tracked by turning at
+ * w = th / T_th, T_th = max(T, th / w_max) (th < 0: th / w_min), T = heading_time, while driving at
+ * v* = V (th/2) cot(th/2) (V at th = 0), then straight at V.  Its largest distance from V t (cos th, sin th) is
+ * V T_th |sin(th/2)|.  The robot may choose among the velocities of P, a convex polygon of at most
+ * RLCA_NH_ORCA_VERTS vertices that contains the origin strictly and lies inside S_E = {V <= min(v_max, E / (T_th
+ * |sin(th/2)|))}, E = tracking_error; P is built on the host in float64 from (E, T, v_max, w_min, w_max).
+ * ORCA: the neighbours, half-planes and preferred velocity of rlca_orca_action with the pair's radius
+ * 2 * (radius + tracking_error).  The LP's lines are P's edges (rotated by the heading) first, then the ORCA lines;
+ * its optimum is the velocity nearest to the preferred one (status 0).  If an ORCA line makes it infeasible, the
+ * least-penetration program takes over from that line with P's edges kept hard (status 1).
+ * Action: (v*, th / T_th) of the chosen velocity clipped to the action bounds; (0, 0) for a speed <= 1e-6.
+ * Every parameter must be finite and > 0, and cfg must have v_min <= 0 < v_max and w_min < 0 < w_max
+ * (RLCA_ERR_INVALID otherwise).
+ * ===================================================================================== */
+#define RLCA_NH_ORCA_VERTS 32
+/*   action_dev    (N,2) raw action (v, w) for rlca_env_step
+ *   velocity_dev  optional (N,2) chosen holonomic velocity in the world frame
+ *   status_dev    optional (N) 0 = LP feasible, 1 = least-penetration fallback */
+int rlca_nh_orca_action(const rlca_env_config *cfg, const rlca_env_state *state, float radius, float neighbour_dist,
+                        float time_horizon, float tracking_error, float heading_time, float *action_dev,
+                        float *velocity_dev, int32_t *status_dev, void *stream);
+/* The same from HOST buffers, by serial loops over the same per-line code; the outputs equal rlca_nh_orca_action's
+ * bit for bit.  velocity_host and status_host may be NULL. */
+int rlca_nh_orca_action_host(const rlca_env_config *cfg, const float *pose_host, const float *goal_host,
+                             const int32_t *meta_host, float radius, float neighbour_dist, float time_horizon,
+                             float tracking_error, float heading_time, float *action_host, float *velocity_host,
+                             int32_t *status_host);
+/* P in the robot frame (x along the heading): *nverts vertices, counter-clockwise, into verts_host
+ * (room for RLCA_NH_ORCA_VERTS x 2 floats). */
+int rlca_nh_orca_polygon_host(const rlca_env_config *cfg, float tracking_error, float heading_time, int32_t *nverts,
+                              float *verts_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

@@ -119,6 +119,11 @@ SYMBOLS = {
                                    C.c_float, _P, _P, _P, _P]),
     'rlca_orca_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_float, C.c_float, C.c_float, C.c_float,
                                         _P, _P, _P]),
+    'rlca_nh_orca_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), C.c_float, C.c_float, C.c_float,
+                                      C.c_float, C.c_float, _P, _P, _P, _P]),
+    'rlca_nh_orca_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_float, C.c_float, C.c_float,
+                                           C.c_float, C.c_float, _P, _P, _P]),
+    'rlca_nh_orca_polygon_host': (C.c_int, [C.POINTER(EnvConfig), C.c_float, C.c_float, _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

@@ -46,3 +46,26 @@ __host__ __device__ __forceinline__ void dev_sincosf(float x, float &s, float &c
     s = ss;
     c = cc;
 }
+
+// atan2(y, x) in (-pi, pi] under the same contract: the cephes atanf polynomial on min / max of |x|, |y| (reduced once
+// more above tan(pi/8)), then the octant and quadrant fix-ups.  +0 and -0 for y both give pi on the negative x axis;
+// atan2(0, 0) = 0.
+__host__ __device__ __forceinline__ float dev_atan2f(float y, float x)
+{
+    const float pio2 = 1.57079632679489662f, pio4 = 0.785398163397448310f, pi = 3.14159265358979324f;
+    const float ax = fabsf(x), ay = fabsf(y), hi = fmaxf(ax, ay);
+    if (!(hi > 0.0f)) return 0.0f;
+    float t = fminf(ax, ay) / hi, base = 0.0f;
+    if (t > 0.4142135623730950f) {
+        base = pio4;
+        t = (t - 1.0f) / (t + 1.0f);
+    }
+    const float z = t * t;
+    float p = fmaf(z, 8.05374449538e-2f, -1.38776856032e-1f);
+    p = fmaf(p, z, 1.99777106478e-1f);
+    p = fmaf(p, z, -3.33329491539e-1f);
+    float a = base + fmaf(p * z, t, t);
+    if (ay > ax) a = pio2 - a;
+    if (x < 0.0f) a = pi - a;
+    return y < 0.0f ? -a : a;
+}

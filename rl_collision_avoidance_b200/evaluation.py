@@ -19,7 +19,7 @@ import torch
 
 from . import _lib
 from .model.ppo import generate_action_no_sampling
-from .orca import OrcaController
+from .orca import NhOrcaController, OrcaController
 
 COLUMNS = _lib.EVAL_PARTIALS
 NPARTIALS = len(COLUMNS)
@@ -130,7 +130,7 @@ def metrics(tot):
 
 def evaluate(env, policy, episodes, max_ticks, check_every=50):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
-    through the env's FIFO), or with the actions of `policy` when it is an OrcaController (orca.py), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
+    through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
     tick; auto_reset 0 (circle) runs one episode per robot: a robot that was terminal on the previous tick gets v = 0
     and its first termination is the record, so at most one record per robot.  Robots that hold all their records keep
@@ -153,7 +153,7 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50):
     ticks = 0
     for tick in range(int(max_ticks)):
         k = tick & 1
-        if isinstance(policy, OrcaController):
+        if isinstance(policy, (OrcaController, NhOrcaController)):
             scaled = policy()
         else:
             _, scaled = generate_action_no_sampling(env=env, state_list=(stacks[k], env.get_local_goal(),

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""Time one rlca_orca_action launch (the ORCA-DD controller, DESIGN.md §9d) with CUDA events over many launches, on
-states after random-action ticks: stage 1 at 171 x 24 agents and the 50-robot circle at 41 x 50.
+"""Time one rlca_orca_action launch (the ORCA-DD controller, DESIGN.md §9d) and one rlca_nh_orca_action launch (NH-ORCA,
+§9e) with CUDA events over many launches, on states after random-action ticks: stage 1 at 171 x 24 agents and the
+50-robot circle at 41 x 50.  The two controllers alternate, each timed twice per size.
 
     python tools/time_orca.py [--launches 2000]
 """
@@ -15,18 +16,18 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET  # noqa: E402
-from rl_collision_avoidance_b200.orca import OrcaController  # noqa: E402
+from rl_collision_avoidance_b200.orca import NhOrcaController, OrcaController  # noqa: E402
 from rl_collision_avoidance_b200.stage_world import StageWorld  # noqa: E402
 
 
-def time_one(scenario, worlds, launches, warmup=200):
+def time_one(scenario, worlds, launches, make, warmup=200):
     env = StageWorld(512, scenario=scenario, num_worlds=worlds, seed=0, auto_reset=AUTO_RESET[scenario])
     env.reset_pose()
     rng = np.random.default_rng(0)
     for _ in range(30):
         a = np.stack([rng.uniform(0, 1, env.N), rng.uniform(-1, 1, env.N)], 1).astype(np.float32)
         env.control_vel(torch.from_numpy(a).cuda())
-    ctrl = OrcaController(env)
+    ctrl = make(env)
     for _ in range(warmup):
         ctrl()
     start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -37,7 +38,7 @@ def time_one(scenario, worlds, launches, warmup=200):
     torch.cuda.synchronize()
     us = start.elapsed_time(end) * 1e3 / launches
     fallback = float(ctrl.status().float().mean())
-    return {'scenario': scenario, 'worlds': worlds, 'agents': env.N, 'us_per_launch': us,
+    return {'controller': make.__name__, 'scenario': scenario, 'worlds': worlds, 'agents': env.N, 'us_per_launch': us,
             'fallback_share': fallback}
 
 
@@ -51,7 +52,8 @@ def main():
                                capture_output=True, text=True, check=True).stdout.strip()
     except (OSError, subprocess.CalledProcessError):
         power = 'unknown'
-    rows = [time_one('stage1', 171, args.launches), time_one('circle', 41, args.launches)]
+    rows = [time_one(scenario, worlds, args.launches, make) for scenario, worlds in (('stage1', 171), ('circle', 41))
+            for _ in range(2) for make in (OrcaController, NhOrcaController)]
     print(json.dumps({'card': card, 'power_limit': power, 'launches': args.launches, 'rows': rows}))
 
 
