@@ -4,13 +4,14 @@ reference accompanies (DESIGN.md §9c): success / crash / time-out rates, and ov
 population std of extra time, extra distance and average speed.  Every robot drives with the policy's mean action
 (--policy), with the ORCA-DD baseline controller (--baseline orca, DESIGN.md §9d) or with the paper's NH-ORCA baseline
 (--baseline nh-orca, DESIGN.md §9e) until it has --episodes recorded episodes (circle: one) or --max-ticks ticks have
-run.
+run.  --orca-map lets either baseline see the static map's walls (obstacle half-planes, DESIGN.md §9f).
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
         --circle-robots 24 --circle-radius 12 --json circle.json
     python evaluate.py --scenario stage2 --baseline orca --num-worlds 8 --episodes 3
     python evaluate.py --scenario stage2 --baseline nh-orca --num-worlds 8 --episodes 3
+    python evaluate.py --scenario stage2 --baseline nh-orca --orca-map --num-worlds 8 --episodes 3
 """
 import argparse
 import json
@@ -20,7 +21,8 @@ import torch
 
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, evaluate
 from rl_collision_avoidance_b200.model.net import CNNPolicy
-from rl_collision_avoidance_b200.orca import DEFAULTS as ORCA_DEFAULTS, NH_DEFAULTS, NhOrcaController, OrcaController
+from rl_collision_avoidance_b200.orca import DEFAULTS as ORCA_DEFAULTS, NH_DEFAULTS, OBSTACLE_TIME_HORIZON, \
+    NhOrcaController, OrcaController
 from rl_collision_avoidance_b200.scenarios import make_scenario
 from rl_collision_avoidance_b200.stage_world import StageWorld
 
@@ -48,6 +50,10 @@ def main(argv=None):
                     help='NH-ORCA tracking error E, m')
     ap.add_argument('--nh-heading-time', type=float, default=NH_DEFAULTS['heading_time'],
                     help='NH-ORCA heading time T, s')
+    ap.add_argument('--orca-map', action='store_true',
+                    help='the baseline also avoids the static map (obstacle half-planes from the occupancy grid)')
+    ap.add_argument('--orca-obstacle-horizon', type=float, default=None,
+                    help='obstacle time horizon tau_o, s, with --orca-map (default %g)' % OBSTACLE_TIME_HORIZON)
     ap.add_argument('--num-worlds', type=int, default=1)
     ap.add_argument('--episodes', type=int, default=1, help='recorded episodes per robot (circle: at most 1)')
     ap.add_argument('--seed', type=int, default=0)
@@ -62,6 +68,11 @@ def main(argv=None):
         ap.error('policy file %s not found' % args.policy)
     if args.baseline != 'orca' and args.orca_gain is not None:
         ap.error('--orca-gain applies to --baseline orca only')
+    if args.baseline is None and args.orca_map:
+        ap.error('--orca-map applies to --baseline orca / nh-orca only')
+    if not args.orca_map and args.orca_obstacle_horizon is not None:
+        ap.error('--orca-obstacle-horizon applies with --orca-map only')
+    obstacle_horizon = OBSTACLE_TIME_HORIZON if args.orca_obstacle_horizon is None else args.orca_obstacle_horizon
     if args.scenario != 'circle' and (args.circle_robots is not None or args.circle_radius is not None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
     sc = make_scenario(args.scenario, robots_per_world=args.circle_robots, radius=args.circle_radius) \
@@ -72,14 +83,16 @@ def main(argv=None):
         gain = ORCA_DEFAULTS['heading_gain'] if args.orca_gain is None else args.orca_gain
         radius = ORCA_DEFAULTS['radius'] if args.orca_radius is None else args.orca_radius
         policy = OrcaController(env, radius=radius, neighbour_dist=args.orca_neighbour_dist,
-                                time_horizon=args.orca_horizon, heading_gain=gain)
-        controller = 'orca-dd'
+                                time_horizon=args.orca_horizon, heading_gain=gain, obstacles=args.orca_map,
+                                obstacle_time_horizon=obstacle_horizon)
+        controller = 'orca-dd+map' if args.orca_map else 'orca-dd'
     elif args.baseline == 'nh-orca':
         radius = NH_DEFAULTS['radius'] if args.orca_radius is None else args.orca_radius
         policy = NhOrcaController(env, radius=radius, neighbour_dist=args.orca_neighbour_dist,
                                   time_horizon=args.orca_horizon, tracking_error=args.nh_error,
-                                  heading_time=args.nh_heading_time)
-        controller = 'nh-orca'
+                                  heading_time=args.nh_heading_time, obstacles=args.orca_map,
+                                  obstacle_time_horizon=obstacle_horizon)
+        controller = 'nh-orca+map' if args.orca_map else 'nh-orca'
     else:
         policy = CNNPolicy(frames=LASER_HIST, action_space=2, max_batch=env.N)
         policy.load_state_dict(torch.load(args.policy, map_location='cuda'))

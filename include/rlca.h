@@ -470,6 +470,72 @@ int rlca_nh_orca_action_host(const rlca_env_config *cfg, const float *pose_host,
 int rlca_nh_orca_polygon_host(const rlca_env_config *cfg, float tracking_error, float heading_time, int32_t *nverts,
                               float *verts_host);
 
+/* =====================================================================================
+ * Static obstacles for both ORCA controllers (csrc/rlca_orca.cu, DESIGN.md §9f): the obstacle half-planes of RVO2
+ * (van den Berg et al. 2011, §6) from the boundary of the static grid.
+ *
+ * Obstacle region: the union of the squares of the non-zero cells (cell (i, j) covers x in [(i - origin_cx) res,
+ * (i + 1 - origin_cx) res), likewise y); cells outside the grid are free.  Its boundary is a set of closed loops of
+ * segments, occupied cells on the LEFT of every segment (counter-clockwise round obstacles, clockwise round holes),
+ * each a maximal run of collinear cell edges; two occupied cells that touch only at a corner are connected (no loop
+ * passes between them).  A vertex is convex when the loop turns left there.  Built on the host in float64 and rounded
+ * to float once; no device is needed.  The lookup bins are RLCA_ORCA_MAP_BIN m squares; each lists the segments within
+ * max_range of it, at most RLCA_ORCA_MAP_MAX_CANDIDATES (RLCA_ERR_UNSUPPORTED otherwise, never truncated).  The device
+ * copy is made at creation when a device is present, else on first device use, on the current device; a set serves
+ * that one device.
+ *
+ * The _map entries take the obstacle set and obstacle_time_horizon tau_o next to the controller's parameters.  The
+ * obstacle radius r_o is the controller's own (ORCA-DD: radius; NH-ORCA: radius + tracking_error), and
+ * tau_o * v_max + r_o must not exceed max_range (RLCA_ERR_INVALID).  Per agent (position and current velocity as the
+ * map-blind controllers take them): the candidates are the segments closer than tau_o * v_max + r_o with the agent
+ * strictly on their free side, taken in order of (squared distance in float32, segment index); a segment whose two
+ * vertices, scaled by 1 / tau_o, lie at least r_o / tau_o beyond an obstacle line built so far is skipped, otherwise it
+ * adds RVO2's obstacle line (none for a colliding non-convex vertex or a nearest point on a foreign leg).  At most
+ * RLCA_ORCA_MAP_MAX_LINES obstacle lines are kept, the nearest; the LP's lines are [P's edges (NH-ORCA)], the obstacle
+ * lines, the agent lines, and P's edges and the obstacle lines are hard in the least-penetration fallback.
+ *   status  bit 0: the least-penetration fallback ran; bit 1: it started at an obstacle line (rounding made the hard
+ *           lines infeasible; the velocity may then violate obstacle lines); bit 2: obstacle lines were dropped at
+ *           RLCA_ORCA_MAP_MAX_LINES.
+ * With an all-free grid the outputs equal the map-blind entries' bit for bit.
+ * ===================================================================================== */
+#define RLCA_ORCA_MAP_BIN 0.25f
+#define RLCA_ORCA_MAP_MAX_CANDIDATES 512
+#define RLCA_ORCA_MAP_MAX_LINES 64
+typedef struct rlca_orca_obstacles rlca_orca_obstacles;
+/* cells_host: grid_h * grid_w bytes, row-major, 0 = free (rlca_env_set_map's layout); cfg gives resolution and
+ * origin_cx / origin_cy; max_range in m, finite and > 0. */
+int rlca_orca_obstacles_create(const rlca_env_config *cfg, const uint8_t *cells_host, int32_t grid_w, int32_t grid_h,
+                               float max_range, rlca_orca_obstacles **out);
+int rlca_orca_obstacles_destroy(rlca_orca_obstacles *obs);
+/* The segments: *nsegments; optional *max_list (longest bin list); optional points_host [4 * nsegments] float
+ * (x0, y0, x1, y1) and links_host [3 * nsegments] int32 (previous segment, next segment, convex flag of the start
+ * vertex).  Segments of one loop are consecutive. */
+int rlca_orca_obstacles_segments(const rlca_orca_obstacles *obs, int32_t *nsegments, int32_t *max_list,
+                                 float *points_host, int32_t *links_host);
+int rlca_orca_action_map(const rlca_env_config *cfg, const rlca_env_state *state, rlca_orca_obstacles *obstacles,
+                         float radius, float neighbour_dist, float time_horizon, float heading_gain,
+                         float obstacle_time_horizon, float *action_dev, float *velocity_dev, int32_t *status_dev,
+                         void *stream);
+int rlca_orca_action_map_host(const rlca_env_config *cfg, rlca_orca_obstacles *obstacles, const float *pose_host,
+                              const float *goal_host, const int32_t *meta_host, float radius, float neighbour_dist,
+                              float time_horizon, float heading_gain, float obstacle_time_horizon, float *action_host,
+                              float *velocity_host, int32_t *status_host);
+int rlca_nh_orca_action_map(const rlca_env_config *cfg, const rlca_env_state *state, rlca_orca_obstacles *obstacles,
+                            float radius, float neighbour_dist, float time_horizon, float tracking_error,
+                            float heading_time, float obstacle_time_horizon, float *action_dev, float *velocity_dev,
+                            int32_t *status_dev, void *stream);
+int rlca_nh_orca_action_map_host(const rlca_env_config *cfg, rlca_orca_obstacles *obstacles, const float *pose_host,
+                                 const float *goal_host, const int32_t *meta_host, float radius, float neighbour_dist,
+                                 float time_horizon, float tracking_error, float heading_time,
+                                 float obstacle_time_horizon, float *action_host, float *velocity_host,
+                                 int32_t *status_host);
+/* The obstacle lines of one agent as the _map entries build them, for tests: *nlines lines (point x, y, unit
+ * direction x, y; allowed side on the left) into lines_host [4 * RLCA_ORCA_MAP_MAX_LINES], *dropped as status bit 2. */
+int rlca_orca_obstacle_lines_host(const rlca_env_config *cfg, rlca_orca_obstacles *obstacles, const float *pose_host,
+                                  const float *goal_host, const int32_t *meta_host, int32_t agent,
+                                  float obstacle_radius, float obstacle_time_horizon, int32_t *nlines,
+                                  int32_t *dropped, float *lines_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

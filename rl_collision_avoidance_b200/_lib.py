@@ -124,6 +124,20 @@ SYMBOLS = {
     'rlca_nh_orca_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_float, C.c_float, C.c_float,
                                            C.c_float, C.c_float, _P, _P, _P]),
     'rlca_nh_orca_polygon_host': (C.c_int, [C.POINTER(EnvConfig), C.c_float, C.c_float, _P, _P]),
+    'rlca_orca_obstacles_create': (C.c_int, [C.POINTER(EnvConfig), _P, C.c_int32, C.c_int32, C.c_float,
+                                             C.POINTER(_P)]),
+    'rlca_orca_obstacles_destroy': (C.c_int, [_P]),
+    'rlca_orca_obstacles_segments': (C.c_int, [_P, _P, _P, _P, _P]),
+    'rlca_orca_action_map': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), _P, C.c_float, C.c_float,
+                                       C.c_float, C.c_float, C.c_float, _P, _P, _P, _P]),
+    'rlca_orca_action_map_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_float, C.c_float, C.c_float,
+                                            C.c_float, C.c_float, _P, _P, _P]),
+    'rlca_nh_orca_action_map': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), _P, C.c_float, C.c_float,
+                                          C.c_float, C.c_float, C.c_float, C.c_float, _P, _P, _P, _P]),
+    'rlca_nh_orca_action_map_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_float, C.c_float,
+                                               C.c_float, C.c_float, C.c_float, C.c_float, _P, _P, _P]),
+    'rlca_orca_obstacle_lines_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_int32, C.c_float,
+                                                C.c_float, _P, _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

@@ -17,6 +17,11 @@
 // tracking error E, the edges of a convex polygon P inside the velocities the robot can track within E come first in the
 // LP as hard lines (one per lane, rotated by the heading), and the action is the arc that tracks the chosen velocity.
 // P is built on the host in float64 (nh_build_polygon).
+//
+// Static obstacles (DESIGN.md §9f), for both controllers: the boundary of the occupied cells of the static grid as
+// closed loops of segments (built once on the host, orca_obstacles_build), a per-bin candidate list, and RVO2's
+// obstacle half-planes (van den Berg et al. 2011, §6) with horizon tau_o and full responsibility, placed after P's edges
+// and before the agent lines and kept hard in the least-penetration fallback.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
@@ -24,6 +29,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
 #include <vector>
 
 #include "../../include/rlca.h"
@@ -34,6 +40,11 @@
 #define ORCA_MAX_LINES (RLCA_MAX_ROBOTS_PER_WORLD - 1)
 #define NH_ORCA_VERTS RLCA_NH_ORCA_VERTS
 #define NH_MAX_LINES (NH_ORCA_VERTS + ORCA_MAX_LINES)
+#define OBS_CAND RLCA_ORCA_MAP_MAX_CANDIDATES
+#define OBS_LINES RLCA_ORCA_MAP_MAX_LINES
+#define ALL_MAX_LINES (NH_ORCA_VERTS + OBS_LINES + ORCA_MAX_LINES)
+#define OBS_BIN ((double)RLCA_ORCA_MAP_BIN)     // side of a lookup bin, m
+#define OBS_SLACK 1e-3              // a bin's list holds the segments within max_range + this of the bin, m
 #define ORCA_PARALLEL_EPS 1e-5f     // |det| of two unit directions below which lines count as parallel
 #define ORCA_STILL 1e-6f            // ORCA speeds at or below this give the action (0, 0)
 #define FULL_MASK 0xffffffffu
@@ -59,6 +70,28 @@ struct NhParams {
     int nv;                         // vertices of P = its hard lines
     float heading_time, v_min;
     OrcaLine edge[NH_ORCA_VERTS];   // in the robot frame: vertex k, unit direction to vertex k + 1 (P on the left)
+};
+
+// One boundary segment of the static map, occupied cells on its left: start vertex (x0, y0), end vertex (x1, y1), unit
+// direction, the directions of the previous and next segments of its loop, and the convex flags of both vertices.
+struct ObsSeg {
+    float x0, y0, x1, y1;
+    float dx, dy, pdx, pdy;
+    float ndx, ndy;
+    int32_t convex0, convex1;
+    int32_t prev, next;
+    int32_t pad[2];
+};
+
+// The obstacle set as one launch reads it (device or host pointers) and the per-call parameters.
+struct ObsParams {
+    const ObsSeg *seg;
+    const int32_t *bin_off;         // nbx * nby + 1 offsets into bin_idx
+    const int32_t *bin_idx;         // per bin: the segments within max_range of it, in index order
+    float bx0, by0, inv_bin;        // world position of bin (0, 0)'s corner, 1 / bin side
+    int32_t nbx, nby;
+    float range2;                   // (tau_o v_max + r_o)^2
+    float inv_tau, r, rt;           // 1 / tau_o, r_o, r_o / tau_o
 };
 
 __host__ __device__ __forceinline__ float det2(float ax, float ay, float bx, float by) { return ax * by - ay * bx; }
@@ -257,6 +290,178 @@ __host__ __device__ __forceinline__ float2 nh_track(const OrcaAgent &a, float vx
     return make_float2(fminf(fmaxf(v, h.v_min), q.v_max), fminf(fmaxf(th / turn, q.w_min), q.w_max));
 }
 
+// ------------------------------------------------------------------------------------ static obstacles (§9f)
+__host__ __device__ __forceinline__ uint32_t float_bits(float x)
+{
+#ifdef __CUDA_ARCH__
+    return __float_as_uint(x);
+#else
+    uint32_t u;
+    memcpy(&u, &x, sizeof u);
+    return u;
+#endif
+}
+
+// Bin of position (x, y), or -1 outside the binned area (no segment lies within max_range there).
+__host__ __device__ __forceinline__ int obs_bin(const ObsParams &m, float x, float y)
+{
+    const float fx = (x - m.bx0) * m.inv_bin, fy = (y - m.by0) * m.inv_bin;
+    if (!(fx >= 0.0f && fx < (float)m.nbx && fy >= 0.0f && fy < (float)m.nby)) return -1;
+    const int ix = (int)fx, iy = (int)fy;
+    return (iy < m.nby - 1 ? iy : m.nby - 1) * m.nbx + (ix < m.nbx - 1 ? ix : m.nbx - 1);
+}
+
+// Segment s is a candidate of agent a when its squared distance from the agent, d2, is below range^2 and the agent is
+// strictly on its free (right) side.  d2: clamp t = -(r1 . e) / |e|^2 to [0, 1], d2 = |r1 + t e|^2 with r1 = s.x0 - a,
+// e = s.x1 - s.x0, in float32; the sort key of the candidates is (d2, segment index).
+__host__ __device__ __forceinline__ bool obs_candidate(const OrcaAgent &a, const ObsSeg &s, float range2, float &d2)
+{
+    const float r1x = s.x0 - a.px, r1y = s.y0 - a.py, ex = s.x1 - s.x0, ey = s.y1 - s.y0;
+    const float t = fminf(fmaxf(-(r1x * ex + r1y * ey) / (ex * ex + ey * ey), 0.0f), 1.0f);
+    const float qx = r1x + t * ex, qy = r1y + t * ey;
+    d2 = qx * qx + qy * qy;
+    return d2 < range2 && det2(s.dx, s.dy, -r1x, -r1y) < 0.0f;
+}
+
+// Segment s is covered by obstacle line l when both its vertices, scaled by 1 / tau_o, lie at least r_o / tau_o -
+// OBS_COVER_EPS beyond l (on its forbidden side).  The tolerance is RVO2's: a cut-off arc line is tangent to the disk of
+// radius r_o / tau_o round a vertex the next segment shares, so that vertex lies exactly r_o / tau_o beyond the line,
+// and without it rounding alone would decide whether the next segment adds a copy of the same line.
+#define OBS_COVER_EPS 1e-5f
+__host__ __device__ __forceinline__ bool obs_covered(const OrcaLine &l, const OrcaAgent &a, const ObsSeg &s,
+                                                     const ObsParams &m)
+{
+    const float ax = m.inv_tau * (s.x0 - a.px) - l.px, ay = m.inv_tau * (s.y0 - a.py) - l.py;
+    const float bx = m.inv_tau * (s.x1 - a.px) - l.px, by = m.inv_tau * (s.y1 - a.py) - l.py;
+    return det2(ax, ay, l.dx, l.dy) - m.rt >= -OBS_COVER_EPS && det2(bx, by, l.dx, l.dy) - m.rt >= -OBS_COVER_EPS;
+}
+
+__host__ __device__ __forceinline__ void obs_unit(float x, float y, float &ux, float &uy)
+{
+    const float n = sqrtf(x * x + y * y);
+    ux = x / n;
+    uy = y / n;
+}
+
+// Leg directions of the truncated velocity obstacle of the disk of radius r at relative position (x, y), d2 = x^2 + y^2
+// > r^2: the tangents from the origin, left and right as seen from the agent.
+__host__ __device__ __forceinline__ void obs_legs(float x, float y, float d2, float r, float &lx, float &ly, float &rx,
+                                                  float &ry)
+{
+    const float leg = sqrtf(d2 - r * r);
+    lx = (x * leg - y * r) / d2;
+    ly = (x * r + y * leg) / d2;
+    rx = (x * leg + y * r) / d2;
+    ry = (-x * r + y * leg) / d2;
+}
+
+// The obstacle half-plane of segment s for agent a (RVO2's Agent::computeNewVelocity, obstacle part): the velocity
+// obstacle of s grown by r_o with horizon tau_o is the cut-off segment (the edge / tau_o grown by r_o / tau_o) and two
+// legs; a leg at a non-convex vertex runs along the segment, and a leg that points into the neighbouring segment
+// (foreign) is replaced by that segment's direction.  The line is tangent to the obstacle at its boundary point nearest
+// to the current velocity, through that point (full responsibility).  When the agent is closer than r_o to s the line
+// passes through the origin, perpendicular to the direction to the nearest point.  False when s adds no line: a
+// colliding non-convex end vertex, a vertex the neighbouring segment handles, or a nearest point on a foreign leg.
+__host__ __device__ __forceinline__ bool obstacle_line(const OrcaAgent &a, const ObsSeg &s, const ObsParams &m,
+                                                       OrcaLine &l)
+{
+    const float r = m.r, r2 = r * r;
+    const float r1x = s.x0 - a.px, r1y = s.y0 - a.py, r2x = s.x1 - a.px, r2y = s.y1 - a.py;
+    const float ex = s.x1 - s.x0, ey = s.y1 - s.y0;
+    const float d1 = r1x * r1x + r1y * r1y, d2 = r2x * r2x + r2y * r2y;
+    const float t = -(r1x * ex + r1y * ey) / (ex * ex + ey * ey);
+    const float qx = -r1x - t * ex, qy = -r1y - t * ey, dline = qx * qx + qy * qy;
+    if (t < 0.0f && d1 <= r2) {                     // collision with the start vertex
+        if (!s.convex0) return false;
+        l.px = 0.0f; l.py = 0.0f;
+        obs_unit(-r1y, r1x, l.dx, l.dy);
+        return true;
+    }
+    if (t > 1.0f && d2 <= r2) {                     // collision with the end vertex
+        if (!s.convex1 || det2(r2x, r2y, s.ndx, s.ndy) < 0.0f) return false;
+        l.px = 0.0f; l.py = 0.0f;
+        obs_unit(-r2y, r2x, l.dx, l.dy);
+        return true;
+    }
+    if (t >= 0.0f && t < 1.0f && dline <= r2) {     // collision with the segment
+        l.px = 0.0f; l.py = 0.0f;
+        l.dx = -s.dx; l.dy = -s.dy;
+        return true;
+    }
+    // legs; `single` when one vertex alone shapes the obstacle (seen obliquely)
+    float llx, lly, rlx, rly, c1x = r1x, c1y = r1y, c2x = r2x, c2y = r2y;
+    float lnx = s.pdx, lny = s.pdy, rnx = s.ndx, rny = s.ndy;    // direction before the left / after the right vertex
+    int lcv = s.convex0, rcv = s.convex1;
+    bool single = false;
+    if (t < 0.0f && dline <= r2) {
+        if (!s.convex0) return false;
+        single = true;
+        c2x = r1x; c2y = r1y;
+        rnx = s.dx; rny = s.dy; rcv = s.convex0;
+        obs_legs(r1x, r1y, d1, r, llx, lly, rlx, rly);
+    } else if (t > 1.0f && dline <= r2) {
+        if (!s.convex1) return false;
+        single = true;
+        c1x = r2x; c1y = r2y;
+        lnx = s.dx; lny = s.dy; lcv = s.convex1;
+        obs_legs(r2x, r2y, d2, r, llx, lly, rlx, rly);
+    } else {
+        float ux, uy;
+        if (s.convex0) obs_legs(r1x, r1y, d1, r, llx, lly, ux, uy);
+        else { llx = -s.dx; lly = -s.dy; }
+        if (s.convex1) obs_legs(r2x, r2y, d2, r, ux, uy, rlx, rly);
+        else { rlx = s.dx; rly = s.dy; }
+    }
+    bool lforeign = false, rforeign = false;
+    if (lcv && det2(llx, lly, -lnx, -lny) >= 0.0f) { llx = -lnx; lly = -lny; lforeign = true; }
+    if (rcv && det2(rlx, rly, rnx, rny) <= 0.0f) { rlx = rnx; rly = rny; rforeign = true; }
+    const float lcx = m.inv_tau * c1x, lcy = m.inv_tau * c1y, rcx = m.inv_tau * c2x, rcy = m.inv_tau * c2y;
+    const float cvx = rcx - lcx, cvy = rcy - lcy;
+    const float wlx = a.vx - lcx, wly = a.vy - lcy, wrx = a.vx - rcx, wry = a.vy - rcy;
+    const float tc = single ? 0.5f : (wlx * cvx + wly * cvy) / (cvx * cvx + cvy * cvy);
+    const float tl = wlx * llx + wly * lly, tr = wrx * rlx + wry * rly;
+    if ((tc < 0.0f && tl < 0.0f) || (single && tl < 0.0f && tr < 0.0f)) {     // the left cut-off arc
+        float ux, uy;
+        obs_unit(wlx, wly, ux, uy);
+        l.dx = uy; l.dy = -ux;
+        l.px = lcx + m.rt * ux; l.py = lcy + m.rt * uy;
+        return true;
+    }
+    if (tc > 1.0f && tr < 0.0f) {                                              // the right cut-off arc
+        float ux, uy;
+        obs_unit(wrx, wry, ux, uy);
+        l.dx = uy; l.dy = -ux;
+        l.px = rcx + m.rt * ux; l.py = rcy + m.rt * uy;
+        return true;
+    }
+    float dc = INFINITY, dl = INFINITY, dr = INFINITY;
+    if (!(tc < 0.0f || tc > 1.0f || single)) {
+        const float x = wlx - tc * cvx, y = wly - tc * cvy;
+        dc = x * x + y * y;
+    }
+    if (!(tl < 0.0f)) {
+        const float x = wlx - tl * llx, y = wly - tl * lly;
+        dl = x * x + y * y;
+    }
+    if (!(tr < 0.0f)) {
+        const float x = wrx - tr * rlx, y = wry - tr * rly;
+        dr = x * x + y * y;
+    }
+    float cx, cy;
+    if (dc <= dl && dc <= dr) {                                                // the cut-off segment
+        l.dx = -s.dx; l.dy = -s.dy; cx = lcx; cy = lcy;
+    } else if (dl <= dr) {                                                     // the left leg
+        if (lforeign) return false;
+        l.dx = llx; l.dy = lly; cx = lcx; cy = lcy;
+    } else {                                                                   // the right leg
+        if (rforeign) return false;
+        l.dx = -rlx; l.dy = -rly; cx = rcx; cy = rcy;
+    }
+    l.px = cx + m.rt * -l.dy;
+    l.py = cy + m.rt * l.dx;
+    return true;
+}
+
 // ------------------------------------------------------------------------------------ device: one warp per agent
 __device__ __forceinline__ float warp_max(float v)
 {
@@ -336,17 +541,74 @@ __device__ void lp3_warp(const OrcaLine *lines, int n, int begin, int hard, floa
     }
 }
 
-// NH = false: ORCA-DD (h unused); NH = true: NH-ORCA, P's lines first in the list.
-template <bool NH>
+// The obstacle lines of agent a into out[0, return): the candidates of its bin (obs_candidate) are compacted into
+// key[] as (d2 bits << 32 | segment index), ranked by counting (keys are distinct) into order[], and then taken in that
+// order: a candidate covered by a line built so far (tested across the lanes, any-ballot) is skipped, else its line is
+// built (every lane computes the same line; lane 0 stores it).  dropped = 1 when a line found no room among the
+// OBS_LINES; the lines kept are then the nearest ones and processing stops.
+__device__ int obs_lines_warp(const OrcaAgent &me, const ObsParams &m, OrcaLine *out, unsigned long long *key,
+                              int32_t *order, int lane, int &dropped)
+{
+    const int bin = obs_bin(m, me.px, me.py);
+    int nc = 0;
+    if (bin >= 0) {
+        const int b0 = m.bin_off[bin], b1 = m.bin_off[bin + 1];
+        for (int k0 = b0; k0 < b1; k0 += 32) {
+            const int k = k0 + lane;
+            unsigned long long kk = 0ull;
+            bool keep = false;
+            if (k < b1) {
+                const int si = m.bin_idx[k];
+                float d2;
+                keep = obs_candidate(me, m.seg[si], m.range2, d2);
+                kk = ((unsigned long long)float_bits(d2) << 32) | (unsigned)si;
+            }
+            const unsigned msk = __ballot_sync(FULL_MASK, keep);
+            if (keep) key[nc + __popc(msk & ((1u << lane) - 1u))] = kk;
+            nc += __popc(msk);
+        }
+    }
+    __syncwarp();
+    for (int k = lane; k < nc; k += 32) {
+        const unsigned long long kk = key[k];
+        int rank = 0;
+        for (int j = 0; j < nc; ++j) rank += key[j] < kk;
+        order[rank] = (int32_t)(kk & 0xffffffffull);
+    }
+    __syncwarp();
+    int no = 0;
+    dropped = 0;
+    for (int c = 0; c < nc; ++c) {
+        const ObsSeg s = m.seg[order[c]];
+        bool cov = false;
+        for (int k = lane; k < no; k += 32) cov |= obs_covered(out[k], me, s, m);
+        if (__any_sync(FULL_MASK, cov)) continue;
+        OrcaLine l;
+        if (!obstacle_line(me, s, m, l)) continue;
+        if (no == OBS_LINES) { dropped = 1; break; }
+        if (lane == 0) out[no] = l;
+        ++no;
+        __syncwarp();
+    }
+    __syncwarp();
+    return no;
+}
+
+// Dynamic shared memory of rlca_orca_kernel<NH, true>: per warp OBS_CAND keys, then per warp OBS_CAND indices.
+#define OBS_SMEM (ORCA_WARPS * OBS_CAND * (sizeof(unsigned long long) + sizeof(int32_t)))
+
+// NH = false: ORCA-DD (h unused); NH = true: NH-ORCA, P's lines first in the list.  MAP = true: the obstacle lines of
+// the static map next (om), hard in the fallback; status bits 1 and 2 as rlca_orca_action_map documents.
+template <bool NH, bool MAP>
 __global__ void __launch_bounds__(ORCA_THREADS) rlca_orca_kernel(int n, int R, OrcaParams q, NhParams h,
                                                                   const float4 *__restrict__ pose,
                                                                   const float4 *__restrict__ goal,
                                                                   const int4 *__restrict__ meta,
                                                                   float2 *__restrict__ action,
                                                                   float2 *__restrict__ velocity,
-                                                                  int32_t *__restrict__ status)
+                                                                  int32_t *__restrict__ status, ObsParams om)
 {
-    constexpr int max_lines = NH ? NH_MAX_LINES : ORCA_MAX_LINES;
+    constexpr int max_lines = (NH ? NH_MAX_LINES : ORCA_MAX_LINES) + (MAP ? OBS_LINES : 0);
     __shared__ OrcaLine s_lines[ORCA_WARPS][max_lines];
     __shared__ OrcaLine s_proj[ORCA_WARPS][max_lines];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -359,6 +621,15 @@ __global__ void __launch_bounds__(ORCA_THREADS) rlca_orca_kernel(int n, int R, O
     if (NH) {
         if (lane < h.nv) lines[lane] = nh_hard_line(me, h.edge[lane]);
         nl = h.nv;
+    }
+    int hard = NH ? h.nv : 0, dropped = 0;
+    if (MAP) {
+        extern __shared__ unsigned long long s_obs[];
+        __syncwarp();
+        nl += obs_lines_warp(me, om, lines + nl, s_obs + warp * OBS_CAND,
+                             reinterpret_cast<int32_t *>(s_obs + ORCA_WARPS * OBS_CAND) + warp * OBS_CAND, lane,
+                             dropped);
+        hard = nl;
     }
     for (int r0 = 0; r0 < R; r0 += 32) {
         const int b = base + r0 + lane;
@@ -376,11 +647,13 @@ __global__ void __launch_bounds__(ORCA_THREADS) rlca_orca_kernel(int n, int R, O
     float ox, oy, rx, ry;
     orca_pref(me, goal[a], q, ox, oy);
     const int fail = lp2_warp(lines, nl, q.v_max, ox, oy, false, rx, ry, lane);
-    if (fail < nl) lp3_warp(lines, nl, fail, NH ? h.nv : 0, q.v_max, s_proj[warp], rx, ry, lane);
+    if (fail < nl) lp3_warp(lines, nl, fail, hard, q.v_max, s_proj[warp], rx, ry, lane);
     if (lane == 0) {
         action[a] = NH ? nh_track(me, rx, ry, q, h) : orca_track(me, rx, ry, q);
         if (velocity) velocity[a] = make_float2(rx, ry);
-        if (status) status[a] = fail < nl;
+        // bit 1: the fallback started at an obstacle line (lines [P's vertex count, hard))
+        if (status) status[a] = MAP ? (fail < nl) | (fail >= (NH ? h.nv : 0) && fail < hard) << 1 | dropped << 2
+                                    : fail < nl;
     }
 }
 
@@ -408,7 +681,7 @@ static int lp2_host(const OrcaLine *lines, int n, float radius, float ox, float 
 
 static void lp3_host(const OrcaLine *lines, int n, int begin, int hard, float radius, float &rx, float &ry)
 {
-    OrcaLine proj[NH_MAX_LINES];
+    OrcaLine proj[ALL_MAX_LINES];
     float dist = 0.0f;
     for (int i = begin; i < n; ++i) {
         const OrcaLine &li = lines[i];
@@ -458,28 +731,61 @@ extern "C" int rlca_orca_action(const rlca_env_config *cfg, const rlca_env_state
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_action: state or action buffer is NULL");
     const int n = cfg->robots_per_world * cfg->num_worlds;
     const NhParams none = {};
-    rlca_orca_kernel<false><<<(n + ORCA_WARPS - 1) / ORCA_WARPS, ORCA_THREADS, 0, (cudaStream_t)stream>>>(
+    const ObsParams no_map = {};
+    rlca_orca_kernel<false, false><<<(n + ORCA_WARPS - 1) / ORCA_WARPS, ORCA_THREADS, 0, (cudaStream_t)stream>>>(
         n, cfg->robots_per_world, q, none, reinterpret_cast<const float4 *>(state->pose_dev),
         reinterpret_cast<const float4 *>(state->goal_dev), reinterpret_cast<const int4 *>(state->meta_dev),
-        reinterpret_cast<float2 *>(action_dev), reinterpret_cast<float2 *>(velocity_dev), status_dev);
+        reinterpret_cast<float2 *>(action_dev), reinterpret_cast<float2 *>(velocity_dev), status_dev, no_map);
     RLCA_CUDA_TRY(cudaGetLastError());
     return RLCA_OK;
 }
 
-// The per-agent steps of rlca_orca_kernel<NH> by serial loops; h = NULL is ORCA-DD.
+// obs_lines_warp by serial loops (std::sort of the same distinct keys gives the same order).
+static int obs_lines_host(const OrcaAgent &me, const ObsParams &m, OrcaLine *out, int &dropped)
+{
+    std::vector<unsigned long long> key;
+    const int bin = obs_bin(m, me.px, me.py);
+    if (bin >= 0)
+        for (int k = m.bin_off[bin]; k < m.bin_off[bin + 1]; ++k) {
+            const int si = m.bin_idx[k];
+            float d2;
+            if (obs_candidate(me, m.seg[si], m.range2, d2))
+                key.push_back(((unsigned long long)float_bits(d2) << 32) | (unsigned)si);
+        }
+    std::sort(key.begin(), key.end());
+    int no = 0;
+    dropped = 0;
+    for (unsigned long long kk : key) {
+        const ObsSeg &s = m.seg[(int32_t)(kk & 0xffffffffull)];
+        bool cov = false;
+        for (int k = 0; k < no && !cov; ++k) cov = obs_covered(out[k], me, s, m);
+        if (cov) continue;
+        OrcaLine l;
+        if (!obstacle_line(me, s, m, l)) continue;
+        if (no == OBS_LINES) { dropped = 1; break; }
+        out[no++] = l;
+    }
+    return no;
+}
+
+// The per-agent steps of rlca_orca_kernel<NH, MAP> by serial loops; h = NULL is ORCA-DD, om = NULL map-blind.
 static void host_actions(const rlca_env_config *cfg, const float *pose_host, const float *goal_host,
-                         const int32_t *meta_host, const OrcaParams &q, const NhParams *h, float *action_host,
-                         float *velocity_host, int32_t *status_host)
+                         const int32_t *meta_host, const OrcaParams &q, const NhParams *h, const ObsParams *om,
+                         float *action_host, float *velocity_host, int32_t *status_host)
 {
     const float4 *pose = reinterpret_cast<const float4 *>(pose_host), *goal = reinterpret_cast<const float4 *>(goal_host);
     const int4 *meta = reinterpret_cast<const int4 *>(meta_host);
-    const int R = cfg->robots_per_world, n = R * cfg->num_worlds, hard = h ? h->nv : 0;
-    OrcaLine lines[NH_MAX_LINES];
+    const int R = cfg->robots_per_world, n = R * cfg->num_worlds, nv = h ? h->nv : 0;
+    OrcaLine lines[ALL_MAX_LINES];
     for (int a = 0; a < n; ++a) {
         const int base = a - a % R;
         const OrcaAgent me = orca_agent(pose, goal, meta, a);
-        int nl = 0;
-        for (; nl < hard; ++nl) lines[nl] = nh_hard_line(me, h->edge[nl]);
+        int nl = 0, hard = nv, dropped = 0;
+        for (; nl < nv; ++nl) lines[nl] = nh_hard_line(me, h->edge[nl]);
+        if (om) {
+            nl += obs_lines_host(me, *om, lines + nl, dropped);
+            hard = nl;
+        }
         for (int b = base; b < base + R; ++b) {
             if (b == a) continue;
             const OrcaAgent o = orca_agent(pose, goal, meta, b);
@@ -493,7 +799,8 @@ static void host_actions(const rlca_env_config *cfg, const float *pose_host, con
         action_host[2 * a] = act.x;
         action_host[2 * a + 1] = act.y;
         if (velocity_host) { velocity_host[2 * a] = rx; velocity_host[2 * a + 1] = ry; }
-        if (status_host) status_host[a] = fail < nl;
+        if (status_host)
+            status_host[a] = om ? (fail < nl) | (fail >= nv && fail < hard) << 1 | dropped << 2 : fail < nl;
     }
 }
 
@@ -506,7 +813,7 @@ extern "C" int rlca_orca_action_host(const rlca_env_config *cfg, const float *po
     if (rc) return rc;
     if (!pose_host || !goal_host || !meta_host || !action_host)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_action_host: a buffer is NULL");
-    host_actions(cfg, pose_host, goal_host, meta_host, q, nullptr, action_host, velocity_host, status_host);
+    host_actions(cfg, pose_host, goal_host, meta_host, q, nullptr, nullptr, action_host, velocity_host, status_host);
     return RLCA_OK;
 }
 
@@ -722,10 +1029,11 @@ extern "C" int rlca_nh_orca_action(const rlca_env_config *cfg, const rlca_env_st
     if (!state || !state->pose_dev || !state->goal_dev || !state->meta_dev || !action_dev)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_nh_orca_action: state or action buffer is NULL");
     const int n = cfg->robots_per_world * cfg->num_worlds;
-    rlca_orca_kernel<true><<<(n + ORCA_WARPS - 1) / ORCA_WARPS, ORCA_THREADS, 0, (cudaStream_t)stream>>>(
+    const ObsParams no_map = {};
+    rlca_orca_kernel<true, false><<<(n + ORCA_WARPS - 1) / ORCA_WARPS, ORCA_THREADS, 0, (cudaStream_t)stream>>>(
         n, cfg->robots_per_world, q, h, reinterpret_cast<const float4 *>(state->pose_dev),
         reinterpret_cast<const float4 *>(state->goal_dev), reinterpret_cast<const int4 *>(state->meta_dev),
-        reinterpret_cast<float2 *>(action_dev), reinterpret_cast<float2 *>(velocity_dev), status_dev);
+        reinterpret_cast<float2 *>(action_dev), reinterpret_cast<float2 *>(velocity_dev), status_dev, no_map);
     RLCA_CUDA_TRY(cudaGetLastError());
     return RLCA_OK;
 }
@@ -741,7 +1049,7 @@ extern "C" int rlca_nh_orca_action_host(const rlca_env_config *cfg, const float 
     if (rc) return rc;
     if (!pose_host || !goal_host || !meta_host || !action_host)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_nh_orca_action_host: a buffer is NULL");
-    host_actions(cfg, pose_host, goal_host, meta_host, q, &h, action_host, velocity_host, status_host);
+    host_actions(cfg, pose_host, goal_host, meta_host, q, &h, nullptr, action_host, velocity_host, status_host);
     return RLCA_OK;
 }
 
@@ -755,5 +1063,414 @@ extern "C" int rlca_nh_orca_polygon_host(const rlca_env_config *cfg, float track
     rc = nh_polygon(cfg, tracking_error, heading_time, verts_host, nv);
     if (rc) return rc;
     *nverts = nv;
+    return RLCA_OK;
+}
+
+// ------------------------------------------------------------------------------------ static obstacles: the set (§9f)
+struct rlca_orca_obstacles {
+    std::vector<ObsSeg> seg;
+    std::vector<int32_t> bin_off, bin_idx;
+    float bx0, by0, max_range;
+    int32_t nbx, nby, max_list;
+    int device;                     // -1 until the device copy exists
+    ObsSeg *seg_dev;
+    int32_t *off_dev, *idx_dev;
+};
+
+// The boundary of the union of the occupied cells as closed loops, occupied cells on the left of every segment (loops
+// run counter-clockwise round obstacles and clockwise round holes).  Unit cell edges are followed from corner to corner;
+// at a corner where two occupied cells touch diagonally the loop turns right, so that it never passes between them
+// (such cells count as connected).  Each segment is a maximal run of collinear unit edges.  Corner (i, j) lies at
+// ((i - origin_cx) res, (j - origin_cy) res), computed in double and rounded to float once.
+static int obs_build_segments(const uint8_t *cells, int W, int H, int ocx, int ocy, double res, std::vector<ObsSeg> &out)
+{
+    static const int DX[4] = {1, 0, -1, 0}, DY[4] = {0, 1, 0, -1};     // 0 +x, 1 +y, 2 -x, 3 -y; k + 1 turns left
+    auto occ = [&](int i, int j) { return i >= 0 && j >= 0 && i < W && j < H && cells[(size_t)j * W + i] != 0; };
+    // does a boundary edge leave corner (i, j) in direction k?  cells NE = (i, j), NW = (i-1, j), SW, SE
+    auto leaves = [&](int i, int j, int k) {
+        switch (k) {
+        case 0: return occ(i, j) && !occ(i, j - 1);
+        case 1: return occ(i - 1, j) && !occ(i, j);
+        case 2: return occ(i - 1, j - 1) && !occ(i - 1, j);
+        default: return occ(i, j - 1) && !occ(i - 1, j - 1);
+        }
+    };
+    const size_t nh = (size_t)(H + 1) * W;
+    auto edge_id = [&](int i, int j, int k) -> size_t {
+        switch (k) {
+        case 0: return (size_t)j * W + i;
+        case 2: return (size_t)j * W + (i - 1);
+        case 1: return nh + (size_t)j * (W + 1) + i;
+        default: return nh + (size_t)(j - 1) * (W + 1) + i;
+        }
+    };
+    std::vector<uint8_t> seen(nh + (size_t)H * (W + 1), 0);
+    std::vector<int> ci, cj, dir;
+    for (int j = 0; j < H; ++j)
+        for (int i = 0; i < W; ++i) {
+            if (!cells[(size_t)j * W + i]) continue;
+            const int starts[4][3] = {{i, j, 0}, {i + 1, j, 1}, {i + 1, j + 1, 2}, {i, j + 1, 3}};
+            for (const auto &st : starts) {
+                if (!leaves(st[0], st[1], st[2]) || seen[edge_id(st[0], st[1], st[2])]) continue;
+                ci.clear(); cj.clear(); dir.clear();
+                int x = st[0], y = st[1], k = st[2];
+                do {
+                    seen[edge_id(x, y, k)] = 1;
+                    ci.push_back(x); cj.push_back(y); dir.push_back(k);
+                    x += DX[k]; y += DY[k];
+                    const int turn[3] = {(k + 3) & 3, k, (k + 1) & 3};     // right, straight, left
+                    int nk = -1;
+                    for (int c : turn)
+                        if (leaves(x, y, c)) { nk = c; break; }
+                    if (nk < 0) return rlca_set_err(RLCA_ERR_INVALID, "obstacle boundary: open loop");
+                    k = nk;
+                } while (!(x == st[0] && y == st[1] && k == st[2]));
+                const int n = (int)dir.size();
+                int s0 = 0;
+                while (dir[s0] == dir[(s0 + n - 1) % n]) ++s0;              // a corner: every loop turns
+                const int first = (int)out.size();
+                for (int e = 0; e < n;) {
+                    const int a = (s0 + e) % n;
+                    int len = 1;
+                    while (e + len < n && dir[(s0 + e + len) % n] == dir[a]) ++len;
+                    ObsSeg s = {};
+                    s.x0 = (float)((ci[a] - ocx) * res);
+                    s.y0 = (float)((cj[a] - ocy) * res);
+                    s.x1 = (float)((ci[a] + len * DX[dir[a]] - ocx) * res);
+                    s.y1 = (float)((cj[a] + len * DY[dir[a]] - ocy) * res);
+                    s.dx = (float)DX[dir[a]];
+                    s.dy = (float)DY[dir[a]];
+                    s.convex0 = dir[a] == ((dir[(a + n - 1) % n] + 1) & 3);  // a left turn into the segment
+                    out.push_back(s);
+                    e += len;
+                }
+                const int last = (int)out.size() - 1;
+                for (int s = first; s <= last; ++s) {
+                    ObsSeg &g = out[s];
+                    g.prev = s == first ? last : s - 1;
+                    g.next = s == last ? first : s + 1;
+                }
+                for (int s = first; s <= last; ++s) {
+                    ObsSeg &g = out[s];
+                    g.pdx = out[g.prev].dx; g.pdy = out[g.prev].dy;
+                    g.ndx = out[g.next].dx; g.ndy = out[g.next].dy;
+                    g.convex1 = out[g.next].convex0;
+                }
+            }
+        }
+    return RLCA_OK;
+}
+
+// Bins of OBS_BIN m over the grid's extent grown by max_range + OBS_SLACK (rounded up to whole bins); a bin's list
+// holds, in index order, every segment whose box is within max_range + OBS_SLACK of the bin's square.  An agent
+// outside the binned area is farther than max_range from every segment.
+static int obs_build_bins(rlca_orca_obstacles &o, int W, int H, int ocx, int ocy, double res)
+{
+    const double reach = (double)o.max_range + OBS_SLACK, margin = ceil(reach / OBS_BIN) * OBS_BIN;
+    const double x0 = -ocx * res - margin, y0 = -ocy * res - margin;
+    const double nbx = ceil((W * res + 2.0 * margin) / OBS_BIN), nby = ceil((H * res + 2.0 * margin) / OBS_BIN);
+    if (nbx * nby > 1e8) return rlca_set_err(RLCA_ERR_UNSUPPORTED, "ORCA obstacles: too many lookup bins");
+    o.bx0 = (float)x0;
+    o.by0 = (float)y0;
+    o.nbx = (int32_t)nbx;
+    o.nby = (int32_t)nby;
+    const size_t nb = (size_t)o.nbx * o.nby;
+    std::vector<int32_t> count(nb + 1, 0);
+    for (int pass = 0; pass < 2; ++pass) {
+        if (pass == 1) {
+            o.bin_off.assign(nb + 1, 0);
+            for (size_t b = 0; b < nb; ++b) o.bin_off[b + 1] = o.bin_off[b] + count[b];
+            o.bin_idx.assign(o.bin_off[nb], 0);
+            std::fill(count.begin(), count.end(), 0);
+        }
+        for (int si = 0; si < (int)o.seg.size(); ++si) {
+            const ObsSeg &s = o.seg[si];
+            const double lx = fmin(s.x0, s.x1), hx = fmax(s.x0, s.x1), ly = fmin(s.y0, s.y1), hy = fmax(s.y0, s.y1);
+            const int ix0 = std::max(0, (int)floor((lx - reach - o.bx0) / OBS_BIN));
+            const int ix1 = std::min(o.nbx - 1, (int)floor((hx + reach - o.bx0) / OBS_BIN));
+            const int iy0 = std::max(0, (int)floor((ly - reach - o.by0) / OBS_BIN));
+            const int iy1 = std::min(o.nby - 1, (int)floor((hy + reach - o.by0) / OBS_BIN));
+            for (int iy = iy0; iy <= iy1; ++iy)
+                for (int ix = ix0; ix <= ix1; ++ix) {
+                    const double bx = (double)o.bx0 + ix * OBS_BIN, by = (double)o.by0 + iy * OBS_BIN;
+                    const double gx = fmax(0.0, fmax(lx - (bx + OBS_BIN), bx - hx));
+                    const double gy = fmax(0.0, fmax(ly - (by + OBS_BIN), by - hy));
+                    if (gx * gx + gy * gy >= reach * reach) continue;
+                    const size_t b = (size_t)iy * o.nbx + ix;
+                    if (pass == 1) o.bin_idx[o.bin_off[b] + count[b]] = si;
+                    ++count[b];
+                }
+        }
+    }
+    o.max_list = 0;
+    for (size_t b = 0; b < nb; ++b) o.max_list = std::max(o.max_list, o.bin_off[b + 1] - o.bin_off[b]);
+    if (o.max_list > OBS_CAND) {
+        char msg[160];      // rlca_set_err formats string arguments only
+        snprintf(msg, sizeof msg, "%d segments within max_range of one lookup bin, above RLCA_ORCA_MAP_MAX_CANDIDATES "
+                 "= %d: lower max_range", o.max_list, OBS_CAND);
+        return rlca_set_err(RLCA_ERR_UNSUPPORTED, "ORCA obstacles: %s", msg);
+    }
+    return RLCA_OK;
+}
+
+static void obs_free_device(rlca_orca_obstacles *o)
+{
+    if (o->device < 0) return;
+    int cur = 0;
+    if (cudaGetDevice(&cur) == cudaSuccess && cur != o->device) cudaSetDevice(o->device);
+    cudaFree(o->seg_dev);
+    cudaFree(o->off_dev);
+    cudaFree(o->idx_dev);
+    if (cur != o->device) cudaSetDevice(cur);
+    o->device = -1;
+}
+
+// The device copy, made on the current device; an obstacle set serves one device.
+static int obs_device(rlca_orca_obstacles *o)
+{
+    int cur = 0;
+    RLCA_CUDA_TRY(cudaGetDevice(&cur));
+    if (o->device >= 0) {
+        if (cur != o->device) return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacles: the set lives on another device");
+        return RLCA_OK;
+    }
+    o->seg_dev = nullptr;
+    o->off_dev = o->idx_dev = nullptr;
+    o->device = cur;
+    const size_t ns = std::max<size_t>(o->seg.size(), 1), no = o->bin_off.size(), ni = std::max<size_t>(o->bin_idx.size(), 1);
+    cudaError_t e = cudaMalloc(&o->seg_dev, ns * sizeof(ObsSeg));
+    if (e == cudaSuccess) e = cudaMalloc(&o->off_dev, no * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&o->idx_dev, ni * sizeof(int32_t));
+    if (e == cudaSuccess && !o->seg.empty())
+        e = cudaMemcpy(o->seg_dev, o->seg.data(), o->seg.size() * sizeof(ObsSeg), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(o->off_dev, o->bin_off.data(), no * sizeof(int32_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && !o->bin_idx.empty())
+        e = cudaMemcpy(o->idx_dev, o->bin_idx.data(), o->bin_idx.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        obs_free_device(o);
+        return rlca_set_err(RLCA_ERR_CUDA, "ORCA obstacles: device copy failed: %s", cudaGetErrorString(e));
+    }
+    return RLCA_OK;
+}
+
+extern "C" int rlca_orca_obstacles_create(const rlca_env_config *cfg, const uint8_t *cells_host, int32_t grid_w,
+                                          int32_t grid_h, float max_range, rlca_orca_obstacles **out)
+{
+    if (!out) return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_obstacles_create: out is NULL");
+    *out = nullptr;
+    if (!cfg || !cells_host) return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_obstacles_create: cfg or cells is NULL");
+    if (grid_w < 1 || grid_h < 1) return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_obstacles_create: empty grid");
+    if (!(cfg->resolution > 0.0f && cfg->resolution < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_obstacles_create: cfg resolution must be finite and > 0");
+    if (!(max_range > 0.0f && max_range < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_obstacles_create: max_range must be finite and > 0");
+    rlca_orca_obstacles *o = new rlca_orca_obstacles();
+    o->device = -1;
+    o->max_range = max_range;
+    const double res = cfg->resolution;
+    int rc = obs_build_segments(cells_host, grid_w, grid_h, cfg->origin_cx, cfg->origin_cy, res, o->seg);
+    if (!rc) rc = obs_build_bins(*o, grid_w, grid_h, cfg->origin_cx, cfg->origin_cy, res);
+    int ndev = 0;
+    if (!rc) {
+        if (cudaGetDeviceCount(&ndev) != cudaSuccess) {
+            cudaGetLastError();
+            ndev = 0;
+        }
+        if (ndev > 0) rc = obs_device(o);
+    }
+    if (rc) {
+        delete o;
+        return rc;
+    }
+    *out = o;
+    return RLCA_OK;
+}
+
+extern "C" int rlca_orca_obstacles_destroy(rlca_orca_obstacles *obs)
+{
+    if (!obs) return RLCA_OK;
+    obs_free_device(obs);
+    delete obs;
+    return RLCA_OK;
+}
+
+extern "C" int rlca_orca_obstacles_segments(const rlca_orca_obstacles *obs, int32_t *nsegments, int32_t *max_list,
+                                            float *points_host, int32_t *links_host)
+{
+    if (!obs || !nsegments) return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_obstacles_segments: obs or nsegments is NULL");
+    *nsegments = (int32_t)obs->seg.size();
+    if (max_list) *max_list = obs->max_list;
+    for (size_t s = 0; s < obs->seg.size(); ++s) {
+        const ObsSeg &g = obs->seg[s];
+        if (points_host) {
+            points_host[4 * s] = g.x0; points_host[4 * s + 1] = g.y0;
+            points_host[4 * s + 2] = g.x1; points_host[4 * s + 3] = g.y1;
+        }
+        if (links_host) {
+            links_host[3 * s] = g.prev; links_host[3 * s + 1] = g.next; links_host[3 * s + 2] = g.convex0;
+        }
+    }
+    return RLCA_OK;
+}
+
+// The launch parameters for obstacle radius r_o and horizon tau_o; device = true takes (or makes) the device copy.
+static int obs_params(rlca_orca_obstacles *obs, const rlca_env_config *cfg, float r_o, float obstacle_time_horizon,
+                      bool device, ObsParams &m)
+{
+    if (!obs) return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacles: the obstacle set is NULL");
+    if (!(obstacle_time_horizon > 0.0f && obstacle_time_horizon < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacle_time_horizon must be finite and > 0");
+    const float range = obstacle_time_horizon * cfg->v_max + r_o;
+    if (!(range <= obs->max_range))
+        return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacles: obstacle_time_horizon * v_max + obstacle radius exceeds "
+                                              "the set's max_range");
+    if (device) {
+        const int rc = obs_device(obs);
+        if (rc) return rc;
+    }
+    m.seg = device ? obs->seg_dev : obs->seg.data();
+    m.bin_off = device ? obs->off_dev : obs->bin_off.data();
+    m.bin_idx = device ? obs->idx_dev : obs->bin_idx.data();
+    m.bx0 = obs->bx0;
+    m.by0 = obs->by0;
+    m.inv_bin = (float)(1.0 / OBS_BIN);
+    m.nbx = obs->nbx;
+    m.nby = obs->nby;
+    m.range2 = range * range;
+    m.inv_tau = 1.0f / obstacle_time_horizon;
+    m.r = r_o;
+    m.rt = r_o * m.inv_tau;
+    return RLCA_OK;
+}
+
+// The map kernels' dynamic shared memory exceeds the default limit; the attribute is set once per device.
+template <bool NH>
+static int map_smem_attribute()
+{
+    static std::atomic<unsigned long long> done{0ull};
+    int dev = 0;
+    RLCA_CUDA_TRY(cudaGetDevice(&dev));
+    const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
+    if (bit && (done.load() & bit)) return RLCA_OK;
+    RLCA_CUDA_TRY(cudaFuncSetAttribute(rlca_orca_kernel<NH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)OBS_SMEM));
+    done.fetch_or(bit);
+    return RLCA_OK;
+}
+
+template <bool NH>
+static int launch_map(const rlca_env_config *cfg, const rlca_env_state *state, const OrcaParams &q, const NhParams &h,
+                      const ObsParams &m, float *action_dev, float *velocity_dev, int32_t *status_dev, void *stream)
+{
+    const int n = cfg->robots_per_world * cfg->num_worlds;
+    const int rc = map_smem_attribute<NH>();
+    if (rc) return rc;
+    rlca_orca_kernel<NH, true><<<(n + ORCA_WARPS - 1) / ORCA_WARPS, ORCA_THREADS, OBS_SMEM, (cudaStream_t)stream>>>(
+        n, cfg->robots_per_world, q, h, reinterpret_cast<const float4 *>(state->pose_dev),
+        reinterpret_cast<const float4 *>(state->goal_dev), reinterpret_cast<const int4 *>(state->meta_dev),
+        reinterpret_cast<float2 *>(action_dev), reinterpret_cast<float2 *>(velocity_dev), status_dev, m);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_orca_action_map(const rlca_env_config *cfg, const rlca_env_state *state,
+                                    rlca_orca_obstacles *obstacles, float radius, float neighbour_dist,
+                                    float time_horizon, float heading_gain, float obstacle_time_horizon,
+                                    float *action_dev, float *velocity_dev, int32_t *status_dev, void *stream)
+{
+    OrcaParams q;
+    ObsParams m;
+    int rc = check_args(cfg, radius, neighbour_dist, time_horizon, heading_gain, q);
+    if (rc) return rc;
+    if (!state || !state->pose_dev || !state->goal_dev || !state->meta_dev || !action_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_action_map: state or action buffer is NULL");
+    rc = obs_params(obstacles, cfg, radius, obstacle_time_horizon, true, m);
+    if (rc) return rc;
+    const NhParams none = {};
+    return launch_map<false>(cfg, state, q, none, m, action_dev, velocity_dev, status_dev, stream);
+}
+
+extern "C" int rlca_orca_action_map_host(const rlca_env_config *cfg, rlca_orca_obstacles *obstacles,
+                                         const float *pose_host, const float *goal_host, const int32_t *meta_host,
+                                         float radius, float neighbour_dist, float time_horizon, float heading_gain,
+                                         float obstacle_time_horizon, float *action_host, float *velocity_host,
+                                         int32_t *status_host)
+{
+    OrcaParams q;
+    ObsParams m;
+    int rc = check_args(cfg, radius, neighbour_dist, time_horizon, heading_gain, q);
+    if (rc) return rc;
+    if (!pose_host || !goal_host || !meta_host || !action_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_action_map_host: a buffer is NULL");
+    rc = obs_params(obstacles, cfg, radius, obstacle_time_horizon, false, m);
+    if (rc) return rc;
+    host_actions(cfg, pose_host, goal_host, meta_host, q, nullptr, &m, action_host, velocity_host, status_host);
+    return RLCA_OK;
+}
+
+extern "C" int rlca_nh_orca_action_map(const rlca_env_config *cfg, const rlca_env_state *state,
+                                       rlca_orca_obstacles *obstacles, float radius, float neighbour_dist,
+                                       float time_horizon, float tracking_error, float heading_time,
+                                       float obstacle_time_horizon, float *action_dev, float *velocity_dev,
+                                       int32_t *status_dev, void *stream)
+{
+    OrcaParams q;
+    NhParams h;
+    ObsParams m;
+    int rc = nh_check_args(cfg, radius, neighbour_dist, time_horizon, tracking_error, heading_time, q, h);
+    if (rc) return rc;
+    if (!state || !state->pose_dev || !state->goal_dev || !state->meta_dev || !action_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_nh_orca_action_map: state or action buffer is NULL");
+    rc = obs_params(obstacles, cfg, radius + tracking_error, obstacle_time_horizon, true, m);
+    if (rc) return rc;
+    return launch_map<true>(cfg, state, q, h, m, action_dev, velocity_dev, status_dev, stream);
+}
+
+extern "C" int rlca_nh_orca_action_map_host(const rlca_env_config *cfg, rlca_orca_obstacles *obstacles,
+                                            const float *pose_host, const float *goal_host, const int32_t *meta_host,
+                                            float radius, float neighbour_dist, float time_horizon,
+                                            float tracking_error, float heading_time, float obstacle_time_horizon,
+                                            float *action_host, float *velocity_host, int32_t *status_host)
+{
+    OrcaParams q;
+    NhParams h;
+    ObsParams m;
+    int rc = nh_check_args(cfg, radius, neighbour_dist, time_horizon, tracking_error, heading_time, q, h);
+    if (rc) return rc;
+    if (!pose_host || !goal_host || !meta_host || !action_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_nh_orca_action_map_host: a buffer is NULL");
+    rc = obs_params(obstacles, cfg, radius + tracking_error, obstacle_time_horizon, false, m);
+    if (rc) return rc;
+    host_actions(cfg, pose_host, goal_host, meta_host, q, &h, &m, action_host, velocity_host, status_host);
+    return RLCA_OK;
+}
+
+extern "C" int rlca_orca_obstacle_lines_host(const rlca_env_config *cfg, rlca_orca_obstacles *obstacles,
+                                             const float *pose_host, const float *goal_host, const int32_t *meta_host,
+                                             int32_t agent, float obstacle_radius, float obstacle_time_horizon,
+                                             int32_t *nlines, int32_t *dropped, float *lines_host)
+{
+    if (!cfg || !pose_host || !goal_host || !meta_host || !nlines || !dropped || !lines_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_obstacle_lines_host: a pointer is NULL");
+    if (agent < 0 || agent >= cfg->robots_per_world * cfg->num_worlds)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_obstacle_lines_host: agent out of range");
+    if (!(obstacle_radius > 0.0f && obstacle_radius < INFINITY) || !(cfg->v_max > 0.0f && cfg->v_max < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_obstacle_lines_host: obstacle_radius and cfg v_max must be "
+                                              "finite and > 0");
+    ObsParams m;
+    const int rc = obs_params(obstacles, cfg, obstacle_radius, obstacle_time_horizon, false, m);
+    if (rc) return rc;
+    const OrcaAgent me = orca_agent(reinterpret_cast<const float4 *>(pose_host),
+                                    reinterpret_cast<const float4 *>(goal_host),
+                                    reinterpret_cast<const int4 *>(meta_host), agent);
+    OrcaLine lines[OBS_LINES];
+    int d = 0;
+    const int no = obs_lines_host(me, m, lines, d);
+    for (int k = 0; k < no; ++k) {
+        lines_host[4 * k] = lines[k].px; lines_host[4 * k + 1] = lines[k].py;
+        lines_host[4 * k + 2] = lines[k].dx; lines_host[4 * k + 3] = lines[k].dy;
+    }
+    *nlines = no;
+    *dropped = d;
     return RLCA_OK;
 }

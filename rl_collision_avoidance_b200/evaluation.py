@@ -130,7 +130,7 @@ def metrics(tot):
 
 def evaluate(env, policy, episodes, max_ticks, check_every=50):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
-    through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
+    through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
     tick; auto_reset 0 (circle) runs one episode per robot: a robot that was terminal on the previous tick gets v = 0
     and its first termination is the record, so at most one record per robot.  Robots that hold all their records keep

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Time one rlca_orca_action launch (the ORCA-DD controller, DESIGN.md §9d) and one rlca_nh_orca_action launch (NH-ORCA,
-§9e) with CUDA events over many launches, on states after random-action ticks: stage 1 at 171 x 24 agents and the
-50-robot circle at 41 x 50.  The two controllers alternate, each timed twice per size.
+§9e), map-blind and map-aware (§9f), with CUDA events over many launches, on states after random-action ticks: stage 1
+at 171 x 24 agents and the 50-robot circle at 41 x 50.  The four rows alternate, each timed twice per size.
 
     python tools/time_orca.py [--launches 2000]
 """
@@ -37,9 +37,18 @@ def time_one(scenario, worlds, launches, make, warmup=200):
     end.record()
     torch.cuda.synchronize()
     us = start.elapsed_time(end) * 1e3 / launches
-    fallback = float(ctrl.status().float().mean())
+    fallback = float((ctrl.status() & 1).float().mean())
+    st = ctrl.status()
     return {'controller': make.__name__, 'scenario': scenario, 'worlds': worlds, 'agents': env.N, 'us_per_launch': us,
-            'fallback_share': fallback}
+            'fallback_share': fallback, 'status_bit_shares': [float(((st >> b) & 1).float().mean()) for b in range(3)]}
+
+
+def OrcaMap(env):
+    return OrcaController(env, obstacles=True)
+
+
+def NhOrcaMap(env):
+    return NhOrcaController(env, obstacles=True)
 
 
 def main():
@@ -53,7 +62,7 @@ def main():
     except (OSError, subprocess.CalledProcessError):
         power = 'unknown'
     rows = [time_one(scenario, worlds, args.launches, make) for scenario, worlds in (('stage1', 171), ('circle', 41))
-            for _ in range(2) for make in (OrcaController, NhOrcaController)]
+            for _ in range(2) for make in (OrcaController, OrcaMap, NhOrcaController, NhOrcaMap)]
     print(json.dumps({'card': card, 'power_limit': power, 'launches': args.launches, 'rows': rows}))
 
 
