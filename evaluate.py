@@ -21,8 +21,8 @@ import torch
 
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, evaluate
 from rl_collision_avoidance_b200.model.net import CNNPolicy
-from rl_collision_avoidance_b200.orca import DEFAULTS as ORCA_DEFAULTS, NH_DEFAULTS, OBSTACLE_TIME_HORIZON, \
-    NhOrcaController, OrcaController
+from rl_collision_avoidance_b200.orca import add_arguments as add_controller_arguments, \
+    check_arguments as check_controller_arguments, from_arguments as controller_from_arguments
 from rl_collision_avoidance_b200.scenarios import make_scenario
 from rl_collision_avoidance_b200.stage_world import StageWorld
 
@@ -38,22 +38,7 @@ def main(argv=None):
     who.add_argument('--policy', help='state_dict of CNNPolicy (e.g. tests/golden/checkpoints/stage2.pth)')
     who.add_argument('--baseline', choices=['orca', 'nh-orca'],
                      help='drive with the ORCA-DD or the NH-ORCA controller instead of a policy')
-    ap.add_argument('--orca-radius', type=float, default=None,
-                    help='robot radius, m (default %g for orca, %g for nh-orca)'
-                    % (ORCA_DEFAULTS['radius'], NH_DEFAULTS['radius']))
-    ap.add_argument('--orca-horizon', type=float, default=ORCA_DEFAULTS['time_horizon'], help='time horizon tau, s')
-    ap.add_argument('--orca-neighbour-dist', type=float, default=ORCA_DEFAULTS['neighbour_dist'],
-                    help='neighbours are the robots closer than this, m')
-    ap.add_argument('--orca-gain', type=float, default=None,
-                    help='ORCA-DD heading gain k_w, 1/s (default %g)' % ORCA_DEFAULTS['heading_gain'])
-    ap.add_argument('--nh-error', type=float, default=NH_DEFAULTS['tracking_error'],
-                    help='NH-ORCA tracking error E, m')
-    ap.add_argument('--nh-heading-time', type=float, default=NH_DEFAULTS['heading_time'],
-                    help='NH-ORCA heading time T, s')
-    ap.add_argument('--orca-map', action='store_true',
-                    help='the baseline also avoids the static map (obstacle half-planes from the occupancy grid)')
-    ap.add_argument('--orca-obstacle-horizon', type=float, default=None,
-                    help='obstacle time horizon tau_o, s, with --orca-map (default %g)' % OBSTACLE_TIME_HORIZON)
+    add_controller_arguments(ap)
     ap.add_argument('--num-worlds', type=int, default=1)
     ap.add_argument('--episodes', type=int, default=1, help='recorded episodes per robot (circle: at most 1)')
     ap.add_argument('--seed', type=int, default=0)
@@ -66,33 +51,17 @@ def main(argv=None):
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
         ap.error('policy file %s not found' % args.policy)
-    if args.baseline != 'orca' and args.orca_gain is not None:
-        ap.error('--orca-gain applies to --baseline orca only')
+    check_controller_arguments(ap, args)
     if args.baseline is None and args.orca_map:
         ap.error('--orca-map applies to --baseline orca / nh-orca only')
-    if not args.orca_map and args.orca_obstacle_horizon is not None:
-        ap.error('--orca-obstacle-horizon applies with --orca-map only')
-    obstacle_horizon = OBSTACLE_TIME_HORIZON if args.orca_obstacle_horizon is None else args.orca_obstacle_horizon
     if args.scenario != 'circle' and (args.circle_robots is not None or args.circle_radius is not None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
     sc = make_scenario(args.scenario, robots_per_world=args.circle_robots, radius=args.circle_radius) \
         if args.scenario == 'circle' else make_scenario(args.scenario)
     env = StageWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, seed=args.seed,
                      auto_reset=AUTO_RESET[args.scenario])
-    if args.baseline == 'orca':
-        gain = ORCA_DEFAULTS['heading_gain'] if args.orca_gain is None else args.orca_gain
-        radius = ORCA_DEFAULTS['radius'] if args.orca_radius is None else args.orca_radius
-        policy = OrcaController(env, radius=radius, neighbour_dist=args.orca_neighbour_dist,
-                                time_horizon=args.orca_horizon, heading_gain=gain, obstacles=args.orca_map,
-                                obstacle_time_horizon=obstacle_horizon)
-        controller = 'orca-dd+map' if args.orca_map else 'orca-dd'
-    elif args.baseline == 'nh-orca':
-        radius = NH_DEFAULTS['radius'] if args.orca_radius is None else args.orca_radius
-        policy = NhOrcaController(env, radius=radius, neighbour_dist=args.orca_neighbour_dist,
-                                  time_horizon=args.orca_horizon, tracking_error=args.nh_error,
-                                  heading_time=args.nh_heading_time, obstacles=args.orca_map,
-                                  obstacle_time_horizon=obstacle_horizon)
-        controller = 'nh-orca+map' if args.orca_map else 'nh-orca'
+    if args.baseline is not None:
+        policy, controller = controller_from_arguments(env, args)
     else:
         policy = CNNPolicy(frames=LASER_HIST, action_space=2, max_batch=env.N)
         policy.load_state_dict(torch.load(args.policy, map_location='cuda'))

@@ -312,6 +312,13 @@ int rlca_ppo_loss_fwd_bwd_weighted(rlca_policy *pol, const float *params_dev, co
                                    float coeff_entropy, float value_coef, float grad_weight, float *losses_dev,
                                    void *stream);
 
+/* Behaviour-cloning loss of one minibatch and its gradient w.r.t. the network outputs (the SL-policy, DESIGN.md §9g):
+ * loss = mean over rows of sum_k (mean_k - target_k)^2, target_action_dev (nb,2) the demonstrated action.
+ * losses_dev[0] = loss.  The output gradients stay in the workspace for rlca_policy_backward: the value's is 0, so the
+ * critic tower's gradients are exactly 0, and so is the logstd gradient. */
+int rlca_bc_loss_fwd_bwd(rlca_policy *pol, const float *params_dev, const float *mean_dev, const float *target_action_dev,
+                         int32_t nb, float *losses_dev, void *stream);
+
 /* Backward of the whole network for the batch of the last rlca_policy_forward: writes the
  * flat gradient buffer (RLCA_POLICY_NPARAMS floats; overwritten, not accumulated).
  * Stream semantics: the call orders all of its work after what is already enqueued on `stream`, and everything the
@@ -535,6 +542,34 @@ int rlca_orca_obstacle_lines_host(const rlca_env_config *cfg, rlca_orca_obstacle
                                   const float *goal_host, const int32_t *meta_host, int32_t agent,
                                   float obstacle_radius, float obstacle_time_horizon, int32_t *nlines,
                                   int32_t *dropped, float *lines_host);
+
+/* =====================================================================================
+ * Demonstration recording (csrc/rlca_demo.cu, DESIGN.md §9g): (observation, expert action) pairs for supervised
+ * training of the policy, appended on the device while a controller drives the env.
+ * ===================================================================================== */
+
+/* A fixed-capacity dataset of rows, in device memory the caller owns:
+ *   obs     (capacity, 3 * beams) the scan stack the controller's tick reads (stack_in of rlca_env_step)
+ *   gs      (capacity, 4) local goal x, y + speed v, w before the tick
+ *   action  (capacity, 2) the action clipped to [v_min, v_max] x [w_min, w_max] as the tick clips it (non-finite -> 0)
+ *   count   2 int64: [0] rows held, [1] zero between calls (completion ticket).  The caller zeroes both. */
+typedef struct rlca_demo_set {
+    float *obs_dev;
+    float *gs_dev;
+    float *action_dev;
+    int64_t *count_dev;
+    int64_t capacity;
+} rlca_demo_set;
+
+/* One launch before the rlca_env_step it records, with that tick's cfg, state_in and io: reads io->stack_in_dev,
+ * io->gs_dev, io->action_dev, state->meta_dev (auto_reset 2) and io->flags_dev as the PREVIOUS tick's flags (auto_reset
+ * 0; NULL = no agent was done).  An agent is recorded when its action drives an episode that has not ended:
+ * auto_reset 1 always, auto_reset 2 when not latched (meta.w == 0), auto_reset 0 when not done on the previous tick.
+ * Rows are appended in agent order; a full dataset keeps its first `capacity` rows.  No host synchronisation.
+ * io->live_dev must be NULL (RLCA_ERR_UNSUPPORTED); 3 * beams must be a multiple of 4; obs and gs buffers 16-byte,
+ * action and count 8-byte aligned. */
+int rlca_demo_append(const rlca_env_config *cfg, const rlca_env_state *state, const rlca_step_io *io,
+                     const rlca_demo_set *demo, void *stream);
 
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);

@@ -57,6 +57,12 @@ class EvalState(C.Structure):
                 ('open_dev', C.c_void_p), ('records_dev', C.c_void_p), ('episodes', C.c_int32)]
 
 
+class DemoSet(C.Structure):
+    """Mirror of rlca_demo_set (include/rlca.h)."""
+    _fields_ = [('obs_dev', C.c_void_p), ('gs_dev', C.c_void_p), ('action_dev', C.c_void_p),
+                ('count_dev', C.c_void_p), ('capacity', C.c_int64)]
+
+
 # rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
 EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
                  'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
@@ -100,6 +106,7 @@ SYMBOLS = {
                                         _P, _P]),
     'rlca_ppo_loss_fwd_bwd_weighted': (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_float, C.c_float,
                                                  C.c_float, C.c_float, _P, _P]),
+    'rlca_bc_loss_fwd_bwd': (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P]),
     'rlca_policy_backward': (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P]),
     'rlca_adam_step': (C.c_int, [_P, _P, _P, _P, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32,
                                  C.c_float, _P]),
@@ -138,6 +145,8 @@ SYMBOLS = {
                                                C.c_float, C.c_float, C.c_float, C.c_float, _P, _P, _P]),
     'rlca_orca_obstacle_lines_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_int32, C.c_float,
                                                 C.c_float, _P, _P, _P]),
+    'rlca_demo_append': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), C.POINTER(StepIO), C.POINTER(DemoSet),
+                                   _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

@@ -887,6 +887,32 @@ __global__ void __launch_bounds__(1024) ppo_loss_kernel(const float *__restrict_
     }
 }
 
+// ------------------------------------------------------------------------------------ behaviour-cloning loss (+ gradient)
+// loss = mean_i sum_k (mean_ik - a_ik)^2 on the deterministic action; single CTA of 1024 threads, deterministic tree
+// reduction.  Only the actor heads get a gradient: dv = 0, so the critic tower's gradients are exactly zero, and the
+// logstd gradient (pol->red) is 0.
+__global__ void __launch_bounds__(1024) bc_loss_kernel(const float *__restrict__ mean, const float *__restrict__ target,
+                                                       int nb, float *__restrict__ dOut, float *__restrict__ loss,
+                                                       float *__restrict__ dlogstd)
+{
+    __shared__ float sh[34];
+    const float inv_nb = 1.0f / (float)nb;
+    float s = 0.f;
+    for (int i = threadIdx.x; i < nb; i += 1024) {
+        const float m0 = mean[2 * i], m1 = mean[2 * i + 1];
+        const float e0 = m0 - target[2 * i], e1 = m1 - target[2 * i + 1];
+        s += e0 * e0 + e1 * e1;
+        const float g0 = 2.0f * inv_nb * e0, g1 = 2.0f * inv_nb * e1;                  // dL/dmean
+        reinterpret_cast<float4 *>(dOut)[i] = make_float4(0.0f, g0 * m0 * (1.0f - m0), g1 * (1.0f - m1 * m1), 0.0f);
+    }
+    const float tot = block_sum_1024(s, sh);
+    if (threadIdx.x == 0) {
+        loss[0] = tot * inv_nb;
+        dlogstd[0] = 0.0f;
+        dlogstd[1] = 0.0f;
+    }
+}
+
 // ------------------------------------------------------------------------------------ Adam / GAE / misc
 __global__ void adam_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
                             float *__restrict__ v, int64_t n, float lr, float b1, float b2, float eps, float bc1,
@@ -1408,6 +1434,17 @@ extern "C" int rlca_ppo_loss_fwd_bwd_weighted(rlca_policy *pol, const float *par
     ppo_loss_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(params + tensor_offset(T_LOGSTD), value, mean, action,
                                                          old_logprob, adv, target, nb, clip_value, coeff_entropy,
                                                          value_coef, grad_weight, pol->dOut, losses, pol->red);
+    pol->launches += 1;
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_bc_loss_fwd_bwd(rlca_policy *pol, const float *params, const float *mean,
+                                    const float *target_action, int32_t nb, float *losses, void *stream)
+{
+    if (!pol || !params || !mean || !target_action || !losses) return rlca_set_err(RLCA_ERR_INVALID, "NULL argument");
+    if (nb < 1 || nb > pol->max_batch) return rlca_set_err(RLCA_ERR_INVALID, "nb exceeds the workspace max_batch");
+    bc_loss_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(mean, target_action, nb, pol->dOut, losses, pol->red);
     pol->launches += 1;
     RLCA_CUDA_TRY(cudaGetLastError());
     return RLCA_OK;

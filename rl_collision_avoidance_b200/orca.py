@@ -17,6 +17,7 @@ The controllers are csrc/rlca_orca.cu; `orca_host` / `nh_orca_host` run the same
 """
 from __future__ import annotations
 
+import argparse
 import ctypes as C
 
 import numpy as np
@@ -165,6 +166,54 @@ class NhOrcaController(_Controller):
                  obstacle_time_horizon=OBSTACLE_TIME_HORIZON):
         super().__init__(env, (radius, neighbour_dist, time_horizon, tracking_error, heading_time), obstacles,
                          np.float32(radius) + np.float32(tracking_error), obstacle_time_horizon)
+
+
+def add_arguments(ap, map_default=False):
+    """The controller flags of the command-line drivers (evaluate.py, sl_train.py) on an argparse parser; `--baseline`
+    is the driver's own.  With map_default the map is on unless --no-orca-map."""
+    ap.add_argument('--orca-radius', type=float, default=None,
+                    help='robot radius, m (default %g for orca, %g for nh-orca)' % (DEFAULTS['radius'], NH_DEFAULTS['radius']))
+    ap.add_argument('--orca-horizon', type=float, default=DEFAULTS['time_horizon'], help='time horizon tau, s')
+    ap.add_argument('--orca-neighbour-dist', type=float, default=DEFAULTS['neighbour_dist'],
+                    help='neighbours are the robots closer than this, m')
+    ap.add_argument('--orca-gain', type=float, default=None,
+                    help='ORCA-DD heading gain k_w, 1/s (default %g)' % DEFAULTS['heading_gain'])
+    ap.add_argument('--nh-error', type=float, default=NH_DEFAULTS['tracking_error'], help='NH-ORCA tracking error E, m')
+    ap.add_argument('--nh-heading-time', type=float, default=NH_DEFAULTS['heading_time'],
+                    help='NH-ORCA heading time T, s')
+    ap.add_argument('--orca-map', action=argparse.BooleanOptionalAction if map_default else 'store_true',
+                    default=map_default,
+                    help='the baseline also avoids the static map (obstacle half-planes from the occupancy grid)')
+    ap.add_argument('--orca-obstacle-horizon', type=float, default=None,
+                    help='obstacle time horizon tau_o, s, with --orca-map (default %g)' % OBSTACLE_TIME_HORIZON)
+
+
+def check_arguments(ap, args):
+    """ap.error() on controller flags that do not apply to args.baseline."""
+    if args.baseline != 'orca' and args.orca_gain is not None:
+        ap.error('--orca-gain applies to --baseline orca only')
+    if not args.orca_map and args.orca_obstacle_horizon is not None:
+        ap.error('--orca-obstacle-horizon applies with --orca-map only')
+
+
+def from_arguments(env, args):
+    """(controller, name) for args.baseline 'orca' or 'nh-orca' and the flags of add_arguments."""
+    horizon = OBSTACLE_TIME_HORIZON if args.orca_obstacle_horizon is None else args.orca_obstacle_horizon
+    if args.baseline == 'orca':
+        gain = DEFAULTS['heading_gain'] if args.orca_gain is None else args.orca_gain
+        radius = DEFAULTS['radius'] if args.orca_radius is None else args.orca_radius
+        ctrl = OrcaController(env, radius=radius, neighbour_dist=args.orca_neighbour_dist,
+                              time_horizon=args.orca_horizon, heading_gain=gain, obstacles=args.orca_map,
+                              obstacle_time_horizon=horizon)
+        return ctrl, 'orca-dd+map' if args.orca_map else 'orca-dd'
+    if args.baseline == 'nh-orca':
+        radius = NH_DEFAULTS['radius'] if args.orca_radius is None else args.orca_radius
+        ctrl = NhOrcaController(env, radius=radius, neighbour_dist=args.orca_neighbour_dist,
+                                time_horizon=args.orca_horizon, tracking_error=args.nh_error,
+                                heading_time=args.nh_heading_time, obstacles=args.orca_map,
+                                obstacle_time_horizon=horizon)
+        return ctrl, 'nh-orca+map' if args.orca_map else 'nh-orca'
+    raise ValueError('unknown baseline %r' % (args.baseline,))
 
 
 def _host(entry, cfg, pose, goal, meta, params, obstacles=None, obstacle_time_horizon=OBSTACLE_TIME_HORIZON):
