@@ -5,6 +5,8 @@ population std of extra time, extra distance and average speed.  Every robot dri
 (--policy), with the ORCA-DD baseline controller (--baseline orca, DESIGN.md §9d) or with the paper's NH-ORCA baseline
 (--baseline nh-orca, DESIGN.md §9e) until it has --episodes recorded episodes (circle: one) or --max-ticks ticks have
 run.  --orca-map lets either baseline see the static map's walls (obstacle half-planes, DESIGN.md §9f).
+--non-cooperative K makes K robots of every world drive straight to their goals, ignoring everyone else, and adds the
+metrics of each role (DESIGN.md §9h).
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -12,6 +14,8 @@ run.  --orca-map lets either baseline see the static map's walls (obstacle half-
     python evaluate.py --scenario stage2 --baseline orca --num-worlds 8 --episodes 3
     python evaluate.py --scenario stage2 --baseline nh-orca --num-worlds 8 --episodes 3
     python evaluate.py --scenario stage2 --baseline nh-orca --orca-map --num-worlds 8 --episodes 3
+    python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 1 \\
+        --non-cooperative 5
 """
 import argparse
 import json
@@ -19,11 +23,11 @@ import os
 
 import torch
 
-from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, evaluate
+from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, evaluate, non_cooperative_mask
 from rl_collision_avoidance_b200.model.net import CNNPolicy
-from rl_collision_avoidance_b200.orca import add_arguments as add_controller_arguments, \
+from rl_collision_avoidance_b200.orca import NonCooperative, add_arguments as add_controller_arguments, \
     check_arguments as check_controller_arguments, from_arguments as controller_from_arguments
-from rl_collision_avoidance_b200.scenarios import make_scenario
+from rl_collision_avoidance_b200.scenarios import COMMON, make_scenario
 from rl_collision_avoidance_b200.stage_world import StageWorld
 
 LASER_BEAM = 512
@@ -47,6 +51,11 @@ def main(argv=None):
     ap.add_argument('--circle-robots', type=int, default=None, help='K robots on the circle (default: the 50-row table)')
     ap.add_argument('--circle-radius', type=float, default=None, help='circle radius in metres (default 25)')
     ap.add_argument('--check-every', type=int, default=50)
+    ap.add_argument('--non-cooperative', type=int, default=None, metavar='K',
+                    help='K robots per world (robots floor(j R / K), j < K) drive straight to their goals and ignore '
+                         'everyone else; the metrics are also printed per role (DESIGN.md §9h)')
+    ap.add_argument('--non-cooperative-speed', type=float, default=None, metavar='S',
+                    help='speed of the non-cooperative robots, m/s, in (0, v_max] (default v_max)')
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -56,8 +65,15 @@ def main(argv=None):
         ap.error('--orca-map applies to --baseline orca / nh-orca only')
     if args.scenario != 'circle' and (args.circle_robots is not None or args.circle_radius is not None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
+    if args.non_cooperative is None and args.non_cooperative_speed is not None:
+        ap.error('--non-cooperative-speed applies with --non-cooperative only')
+    v_max = COMMON['v_max']
+    if args.non_cooperative_speed is not None and not 0.0 < args.non_cooperative_speed <= v_max:
+        ap.error('--non-cooperative-speed must be in (0, %g]' % v_max)
     sc = make_scenario(args.scenario, robots_per_world=args.circle_robots, radius=args.circle_radius) \
         if args.scenario == 'circle' else make_scenario(args.scenario)
+    if args.non_cooperative is not None and not 1 <= args.non_cooperative <= sc.robots_per_world:
+        ap.error('--non-cooperative must be in 1..%d on %s' % (sc.robots_per_world, args.scenario))
     env = StageWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, seed=args.seed,
                      auto_reset=AUTO_RESET[args.scenario])
     if args.baseline is not None:
@@ -68,20 +84,36 @@ def main(argv=None):
         controller = None
     max_ticks = args.max_ticks if args.max_ticks is not None else \
         (CIRCLE_MAX_TICKS if args.scenario == 'circle' else args.episodes * (sc.timeout + 1))
-    out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every)
+    nc = None
+    if args.non_cooperative is not None:
+        nc = NonCooperative(env, non_cooperative_mask(sc.robots_per_world, args.num_worlds, args.non_cooperative),
+                            speed=args.non_cooperative_speed)
+    out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc)
+
+    def line(m, robots, role=''):
+        f = lambda k: '%.3f +- %.3f' % m[k]
+        print(('%s  ' % controller if controller else '') + role +
+              '%s  robots %d  ticks %d  episodes %d  success %.4f  crash %.4f  time-out %.4f  unfinished %d  '
+              'extra time %s s  extra distance %s m  average speed %s m/s'
+              % (args.scenario, robots, out['ticks'], m['episodes'], m['success_rate'], m['crash_rate'],
+                 m['timeout_rate'], m['unfinished'], f('extra_time'), f('extra_distance'), f('average_speed')))
+
     m = out['metrics']
-    f = lambda k: '%.3f +- %.3f' % m[k]
-    print(('%s  ' % controller if controller else '') +
-          '%s  robots %d  ticks %d  episodes %d  success %.4f  crash %.4f  time-out %.4f  unfinished %d  '
-          'extra time %s s  extra distance %s m  average speed %s m/s'
-          % (args.scenario, env.N, out['ticks'], m['episodes'], m['success_rate'], m['crash_rate'], m['timeout_rate'],
-             m['unfinished'], f('extra_time'), f('extra_distance'), f('average_speed')))
+    line(m, env.N)
+    if nc is not None:
+        k = args.non_cooperative * args.num_worlds
+        line(out['by_role']['cooperative'], env.N - k, 'cooperative  ')
+        line(out['by_role']['non_cooperative'], k, 'non-cooperative  ')
     if args.json:
+        res = {'args': vars(args), 'controller': controller or 'policy', 'robots': env.N,
+               'ticks': out['ticks'], 'metrics': m,
+               'columns': list(COLUMNS), 'totals': out['totals'].tolist(),
+               'partials': out['partials'].tolist()}
+        if nc is not None:
+            res['by_role'] = out['by_role']
+            res['partials_split'] = out['partials_split'].tolist()
         with open(args.json, 'w') as fh:
-            json.dump({'args': vars(args), 'controller': controller or 'policy', 'robots': env.N,
-                       'ticks': out['ticks'], 'metrics': m,
-                       'columns': list(COLUMNS), 'totals': out['totals'].tolist(),
-                       'partials': out['partials'].tolist()}, fh, indent=1)
+            json.dump(res, fh, indent=1)
     return out
 
 

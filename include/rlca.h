@@ -418,6 +418,14 @@ int rlca_eval_reduce(const rlca_env_config *cfg, const rlca_eval_state *ev, int3
 int rlca_eval_reduce_host(const rlca_env_config *cfg, const float *records_host, const int32_t *count_host,
                           const int32_t *open_host, int32_t episodes, int32_t world_begin, int32_t world_count,
                           double *partials_host);
+/* The same partials split by an agent mask (N uint8, DESIGN.md §9h): partials_dev (world_count, 2,
+ * RLCA_EVAL_NPARTIALS), row 0 over the agents with mask 0 and row 1 over the others, each in the order of
+ * rlca_eval_reduce (one thread per world and row, no atomics).  A NULL mask is RLCA_ERR_INVALID. */
+int rlca_eval_reduce_split(const rlca_env_config *cfg, const rlca_eval_state *ev, const uint8_t *mask_dev,
+                           int32_t world_begin, int32_t world_count, double *partials_dev, void *stream);
+int rlca_eval_reduce_split_host(const rlca_env_config *cfg, const float *records_host, const int32_t *count_host,
+                                const int32_t *open_host, const uint8_t *mask_host, int32_t episodes,
+                                int32_t world_begin, int32_t world_count, double *partials_host);
 
 /* =====================================================================================
  * ORCA-DD baseline controller (csrc/rlca_orca.cu, DESIGN.md §9d): reciprocal velocity obstacles (van den Berg et al.
@@ -440,6 +448,18 @@ int rlca_orca_action(const rlca_env_config *cfg, const rlca_env_state *state, fl
 int rlca_orca_action_host(const rlca_env_config *cfg, const float *pose_host, const float *goal_host,
                           const int32_t *meta_host, float radius, float neighbour_dist, float time_horizon,
                           float heading_gain, float *action_host, float *velocity_host, int32_t *status_host);
+
+/* Non-cooperative robots (DESIGN.md §9h): drive straight to the goal and ignore every other robot and the map.
+ * action_dev (N,2) is read and written in place: for every agent with mask_dev[a] != 0 (N uint8) the row becomes
+ * ORCA-DD's action for an agent without neighbours, with v_max = speed and k_w = heading_gain (w bounds from cfg);
+ * rows with mask 0 are not touched.  speed must be finite and in (0, cfg->v_max], heading_gain finite and > 0, and
+ * no buffer may be NULL (RLCA_ERR_INVALID otherwise). */
+int rlca_noncoop_action(const rlca_env_config *cfg, const rlca_env_state *state, const uint8_t *mask_dev, float speed,
+                        float heading_gain, float *action_dev, void *stream);
+/* The same from HOST buffers (pose, goal: (N,4) float; meta: (N,4) int32); equal to rlca_noncoop_action bit for bit. */
+int rlca_noncoop_action_host(const rlca_env_config *cfg, const float *pose_host, const float *goal_host,
+                             const int32_t *meta_host, const uint8_t *mask_host, float speed, float heading_gain,
+                             float *action_host);
 
 /* =====================================================================================
  * NH-ORCA baseline controller (csrc/rlca_orca.cu, DESIGN.md §9e): ORCA for non-holonomic robots (Alonso-Mora,

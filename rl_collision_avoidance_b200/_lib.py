@@ -122,10 +122,16 @@ SYMBOLS = {
                                   C.POINTER(EvalState), _P]),
     'rlca_eval_reduce': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EvalState), C.c_int32, C.c_int32, _P, _P]),
     'rlca_eval_reduce_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
+    'rlca_eval_reduce_split': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EvalState), _P, C.c_int32, C.c_int32, _P,
+                                         _P]),
+    'rlca_eval_reduce_split_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32,
+                                              _P]),
     'rlca_orca_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), C.c_float, C.c_float, C.c_float,
                                    C.c_float, _P, _P, _P, _P]),
     'rlca_orca_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_float, C.c_float, C.c_float, C.c_float,
                                         _P, _P, _P]),
+    'rlca_noncoop_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), _P, C.c_float, C.c_float, _P, _P]),
+    'rlca_noncoop_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_float, C.c_float, _P]),
     'rlca_nh_orca_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), C.c_float, C.c_float, C.c_float,
                                       C.c_float, C.c_float, _P, _P, _P, _P]),
     'rlca_nh_orca_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_float, C.c_float, C.c_float,

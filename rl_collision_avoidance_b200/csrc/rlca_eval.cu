@@ -9,6 +9,7 @@
 // rlca_eval_reduce sums the records of each world in float64, in a fixed order (agent, then record), one thread per
 // world and no atomics, so a world's partials do not depend on the launch or on how the worlds are sharded.  The same
 // per-world function runs on the host in rlca_eval_reduce_host, which the CPU tests check against numpy.
+// rlca_eval_reduce_split runs it twice per world, once per role of an agent mask (DESIGN.md §9h).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
@@ -85,15 +86,17 @@ __global__ void __launch_bounds__(EVAL_THREADS) eval_track_kernel(
     open[a] = cl != meta_out[a].y;
 }
 
-// Partials of world w (agents w*R .. w*R+R-1), layout RLCA_EVAL_* of include/rlca.h.
+// Partials of world w (agents w*R .. w*R+R-1), layout RLCA_EVAL_* of include/rlca.h.  With a mask, only the agents
+// whose (mask[a] != 0) equals `want` count.
 __host__ __device__ inline void reduce_world(int R, int episodes, double dt, double v_max, double goal_radius,
                                              const float4 *records, const int32_t *count, const int32_t *open, int w,
-                                             double *out)
+                                             const uint8_t *mask, bool want, double *out)
 {
     double s[RLCA_EVAL_NPARTIALS];
     for (int k = 0; k < RLCA_EVAL_NPARTIALS; ++k) s[k] = 0.0;
     for (int r = 0; r < R; ++r) {
         const int a = w * R + r;
+        if (mask && (mask[a] != 0) != want) continue;
         const int c = count[a];
         const int nrec = c < episodes ? c : episodes;
         if (c < episodes && open[a]) s[RLCA_EVAL_UNFINISHED] = d_add(s[RLCA_EVAL_UNFINISHED], 1.0);
@@ -127,7 +130,20 @@ __global__ void __launch_bounds__(EVAL_THREADS) eval_reduce_kernel(int R, int ep
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= world_count) return;
-    reduce_world(R, episodes, dt, v_max, goal_radius, records, count, open, world_begin + i,
+    reduce_world(R, episodes, dt, v_max, goal_radius, records, count, open, world_begin + i, nullptr, false,
+                 partials + (size_t)i * RLCA_EVAL_NPARTIALS);
+}
+
+// One thread per (world, row): row 0 the agents with mask 0, row 1 the others.
+__global__ void __launch_bounds__(EVAL_THREADS) eval_reduce_split_kernel(int R, int episodes, double dt, double v_max,
+                                                                          double goal_radius, const float4 *records,
+                                                                          const int32_t *count, const int32_t *open,
+                                                                          const uint8_t *mask, int world_begin,
+                                                                          int world_count, double *partials)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 2 * world_count) return;
+    reduce_world(R, episodes, dt, v_max, goal_radius, records, count, open, world_begin + (i >> 1), mask, i & 1,
                  partials + (size_t)i * RLCA_EVAL_NPARTIALS);
 }
 
@@ -197,7 +213,41 @@ extern "C" int rlca_eval_reduce_host(const rlca_env_config *cfg, const float *re
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_eval_reduce_host: a buffer is NULL");
     for (int i = 0; i < world_count; ++i)
         reduce_world(cfg->robots_per_world, episodes, (double)cfg->dt, (double)cfg->v_max, (double)cfg->goal_radius,
-                     reinterpret_cast<const float4 *>(records_host), count_host, open_host, world_begin + i,
-                     partials_host + (size_t)i * RLCA_EVAL_NPARTIALS);
+                     reinterpret_cast<const float4 *>(records_host), count_host, open_host, world_begin + i, nullptr,
+                     false, partials_host + (size_t)i * RLCA_EVAL_NPARTIALS);
+    return RLCA_OK;
+}
+
+extern "C" int rlca_eval_reduce_split(const rlca_env_config *cfg, const rlca_eval_state *ev, const uint8_t *mask_dev,
+                                      int32_t world_begin, int32_t world_count, double *partials_dev, void *stream)
+{
+    int rc = check_cfg(cfg, ev ? ev->episodes : 0);
+    if (rc) return rc;
+    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if (!ev->count_dev || !ev->open_dev || !ev->records_dev || !mask_dev || !partials_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_eval_reduce_split: a buffer is NULL");
+    eval_reduce_split_kernel<<<(2 * world_count + EVAL_THREADS - 1) / EVAL_THREADS, EVAL_THREADS, 0,
+                               (cudaStream_t)stream>>>(
+        cfg->robots_per_world, ev->episodes, (double)cfg->dt, (double)cfg->v_max, (double)cfg->goal_radius,
+        reinterpret_cast<const float4 *>(ev->records_dev), ev->count_dev, ev->open_dev, mask_dev, world_begin,
+        world_count, partials_dev);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_eval_reduce_split_host(const rlca_env_config *cfg, const float *records_host,
+                                           const int32_t *count_host, const int32_t *open_host,
+                                           const uint8_t *mask_host, int32_t episodes, int32_t world_begin,
+                                           int32_t world_count, double *partials_host)
+{
+    int rc = check_cfg(cfg, episodes);
+    if (rc) return rc;
+    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if (!records_host || !count_host || !open_host || !mask_host || !partials_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_eval_reduce_split_host: a buffer is NULL");
+    for (int i = 0; i < 2 * world_count; ++i)
+        reduce_world(cfg->robots_per_world, episodes, (double)cfg->dt, (double)cfg->v_max, (double)cfg->goal_radius,
+                     reinterpret_cast<const float4 *>(records_host), count_host, open_host, world_begin + (i >> 1),
+                     mask_host, i & 1, partials_host + (size_t)i * RLCA_EVAL_NPARTIALS);
     return RLCA_OK;
 }

@@ -22,6 +22,9 @@
 // closed loops of segments (built once on the host, orca_obstacles_build), a per-bin candidate list, and RVO2's
 // obstacle half-planes (van den Berg et al. 2011, §6) with horizon tau_o and full responsibility, placed after P's edges
 // and before the agent lines and kept hard in the least-penetration fallback.
+//
+// The non-cooperative driver (DESIGN.md §9h) overwrites the actions of masked agents with ORCA-DD's answer for an agent
+// without neighbours: straight to the goal, ignoring everyone else.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
@@ -814,6 +817,81 @@ extern "C" int rlca_orca_action_host(const rlca_env_config *cfg, const float *po
     if (!pose_host || !goal_host || !meta_host || !action_host)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_orca_action_host: a buffer is NULL");
     host_actions(cfg, pose_host, goal_host, meta_host, q, nullptr, nullptr, action_host, velocity_host, status_host);
+    return RLCA_OK;
+}
+
+// ------------------------------------------------------------------------------------ non-cooperative driver (§9h)
+// ORCA-DD's action for agent a when it has no neighbours: v_pref on the speed disk, then the heading tracker.
+__host__ __device__ __forceinline__ float2 noncoop_action(const float4 *pose, const float4 *goal, const int4 *meta, int a,
+                                                          const OrcaParams &q)
+{
+    const OrcaAgent me = orca_agent(pose, goal, meta, a);
+    float ox, oy, rx, ry;
+    orca_pref(me, goal[a], q, ox, oy);
+    lp2_start(q.v_max, ox, oy, false, rx, ry);
+    return orca_track(me, rx, ry, q);
+}
+
+// One thread per agent; rows with mask 0 are not touched.
+__global__ void __launch_bounds__(ORCA_THREADS) rlca_noncoop_kernel(int n, OrcaParams q,
+                                                                     const float4 *__restrict__ pose,
+                                                                     const float4 *__restrict__ goal,
+                                                                     const int4 *__restrict__ meta,
+                                                                     const uint8_t *__restrict__ mask,
+                                                                     float2 *__restrict__ action)
+{
+    const int a = blockIdx.x * ORCA_THREADS + threadIdx.x;
+    if (a >= n || !mask[a]) return;
+    action[a] = noncoop_action(pose, goal, meta, a, q);
+}
+
+// ORCA-DD's parameters with v_max = speed and gain = heading_gain (the neighbour terms are unused).
+static int noncoop_args(const rlca_env_config *cfg, float speed, float heading_gain, OrcaParams &q)
+{
+    if (!(heading_gain > 0.0f && heading_gain < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "non-cooperative heading_gain must be finite and > 0");
+    int rc = check_args(cfg, 1.0f, 1.0f, 1.0f, heading_gain, q);
+    if (rc) return rc;
+    if (!(speed > 0.0f && speed <= cfg->v_max && speed < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "non-cooperative speed must be finite and in (0, cfg.v_max]");
+    q.v_max = speed;
+    return RLCA_OK;
+}
+
+extern "C" int rlca_noncoop_action(const rlca_env_config *cfg, const rlca_env_state *state, const uint8_t *mask_dev,
+                                   float speed, float heading_gain, float *action_dev, void *stream)
+{
+    OrcaParams q;
+    int rc = noncoop_args(cfg, speed, heading_gain, q);
+    if (rc) return rc;
+    if (!state || !state->pose_dev || !state->goal_dev || !state->meta_dev || !mask_dev || !action_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_noncoop_action: state, mask or action buffer is NULL");
+    const int n = cfg->robots_per_world * cfg->num_worlds;
+    rlca_noncoop_kernel<<<(n + ORCA_THREADS - 1) / ORCA_THREADS, ORCA_THREADS, 0, (cudaStream_t)stream>>>(
+        n, q, reinterpret_cast<const float4 *>(state->pose_dev), reinterpret_cast<const float4 *>(state->goal_dev),
+        reinterpret_cast<const int4 *>(state->meta_dev), mask_dev, reinterpret_cast<float2 *>(action_dev));
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_noncoop_action_host(const rlca_env_config *cfg, const float *pose_host, const float *goal_host,
+                                        const int32_t *meta_host, const uint8_t *mask_host, float speed,
+                                        float heading_gain, float *action_host)
+{
+    OrcaParams q;
+    int rc = noncoop_args(cfg, speed, heading_gain, q);
+    if (rc) return rc;
+    if (!pose_host || !goal_host || !meta_host || !mask_host || !action_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_noncoop_action_host: a buffer is NULL");
+    const float4 *pose = reinterpret_cast<const float4 *>(pose_host), *goal = reinterpret_cast<const float4 *>(goal_host);
+    const int4 *meta = reinterpret_cast<const int4 *>(meta_host);
+    const int n = cfg->robots_per_world * cfg->num_worlds;
+    for (int a = 0; a < n; ++a) {
+        if (!mask_host[a]) continue;
+        const float2 act = noncoop_action(pose, goal, meta, a, q);
+        action_host[2 * a] = act.x;
+        action_host[2 * a + 1] = act.y;
+    }
     return RLCA_OK;
 }
 

@@ -81,6 +81,19 @@ class EpisodeTracker:
                                             env._stream()))
         return out.cpu().numpy()
 
+    def partials_split(self, mask, world_begin=0, world_count=None):
+        """(world_count, 2, NPARTIALS) per-world partials split by the agent mask (N): row 0 over the agents with mask
+        0, row 1 over the others (rlca_eval_reduce_split)."""
+        env = self.env
+        wc = env.num_worlds - world_begin if world_count is None else int(world_count)
+        m = torch.as_tensor(mask, device=env.device).to(torch.uint8).contiguous()
+        if m.shape != (env.N,):
+            raise ValueError(f'mask must have ({env.N},) entries')
+        out = torch.empty(wc, 2, NPARTIALS, dtype=torch.float64, device=env.device)
+        _lib.check(env.lib.rlca_eval_reduce_split(C.byref(env.cfg), C.byref(self._st), _ptr(m), int(world_begin), wc,
+                                                  _ptr(out), env._stream()))
+        return out.cpu().numpy()
+
 
 def reduce_host(cfg, records, count, open_, world_begin=0, world_count=None):
     """rlca_eval_reduce on host arrays (the same code, run by the CPU): records (N, E, 4) float32, count and open (N)."""
@@ -94,6 +107,34 @@ def reduce_host(cfg, records, count, open_, world_begin=0, world_count=None):
                                          opn.ctypes.data_as(C.c_void_p), rec.shape[1], int(world_begin), wc,
                                          out.ctypes.data_as(C.c_void_p)))
     return out
+
+
+def reduce_split_host(cfg, records, count, open_, mask, world_begin=0, world_count=None):
+    """rlca_eval_reduce_split on host arrays, as reduce_host, with the agent mask (N): (world_count, 2, NPARTIALS)."""
+    lib = _lib.load()
+    rec = np.ascontiguousarray(records, np.float32)
+    cnt = np.ascontiguousarray(count, np.int32)
+    opn = np.ascontiguousarray(open_, np.int32)
+    msk = np.ascontiguousarray(mask, np.uint8)
+    if msk.shape != cnt.shape:
+        raise ValueError('mask must have one entry per agent')
+    wc = cfg.num_worlds - world_begin if world_count is None else int(world_count)
+    out = np.zeros((wc, 2, NPARTIALS), np.float64)
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    _lib.check(lib.rlca_eval_reduce_split_host(C.byref(cfg), vp(rec), vp(cnt), vp(opn), vp(msk), rec.shape[1],
+                                               int(world_begin), wc, vp(out)))
+    return out
+
+
+def non_cooperative_mask(robots_per_world, num_worlds, k):
+    """(robots_per_world * num_worlds,) uint8 with robots floor(j R / k), j < k, of every world set: k robots spread
+    evenly round the circle table (DESIGN.md §9h).  ValueError unless 1 <= k <= R."""
+    R, W, k = int(robots_per_world), int(num_worlds), int(k)
+    if not 1 <= k <= R:
+        raise ValueError(f'the number of non-cooperative robots must be in 1..{R}, got {k}')
+    m = np.zeros((W, R), np.uint8)
+    m[:, [j * R // k for j in range(k)]] = 1
+    return m.reshape(-1)
 
 
 def totals(partials):
@@ -128,14 +169,19 @@ def metrics(tot):
     return out
 
 
-def evaluate(env, policy, episodes, max_ticks, check_every=50):
+def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
     tick; auto_reset 0 (circle) runs one episode per robot: a robot that was terminal on the previous tick gets v = 0
     and its first termination is the record, so at most one record per robot.  Robots that hold all their records keep
     driving: they are obstacles for the others.  Completion is checked every `check_every` ticks (one sync each).
-    Returns {'partials', 'totals', 'metrics', 'ticks', 'tracker'}."""
+    Returns {'partials', 'totals', 'metrics', 'ticks', 'tracker'}.
+
+    With `non_cooperative` (an orca.NonCooperative on `env`) its robots drive straight to their goals instead: the
+    override is applied to every tick's action before the circle rule, so they keep the same episode mechanics.  The
+    result then also holds 'partials_split' (num_worlds, 2, NPARTIALS) and 'by_role' {'cooperative',
+    'non_cooperative'}: the metrics of each role; 'partials', 'totals' and 'metrics' still cover every robot."""
     E = int(episodes)
     if int(check_every) < 1:
         raise ValueError('check_every must be >= 1')
@@ -159,6 +205,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50):
             _, scaled = generate_action_no_sampling(env=env, state_list=(stacks[k], env.get_local_goal(),
                                                                          env.get_self_speed()),
                                                     policy=policy, action_bound=ACTION_BOUND)
+        if non_cooperative is not None:
+            non_cooperative.apply(scaled)
         if circle:
             scaled = torch.stack((torch.where(terminal, 0.0, scaled[:, 0]), scaled[:, 1]), 1)
         env.control_vel(scaled, stack_in=stacks[k], stack_out=stacks[1 - k])
@@ -170,4 +218,10 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50):
             break
     part = tracker.partials()
     tot = totals(part)
-    return {'partials': part, 'totals': tot, 'metrics': metrics(tot), 'ticks': ticks, 'tracker': tracker}
+    out = {'partials': part, 'totals': tot, 'metrics': metrics(tot), 'ticks': ticks, 'tracker': tracker}
+    if non_cooperative is not None:
+        split = tracker.partials_split(non_cooperative.mask)
+        out['partials_split'] = split
+        out['by_role'] = {'cooperative': metrics(totals(split[:, 0])),
+                          'non_cooperative': metrics(totals(split[:, 1]))}
+    return out

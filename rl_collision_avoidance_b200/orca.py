@@ -14,6 +14,9 @@ with horizon `obstacle_time_horizon` (DESIGN.md §9f).
     OrcaController(env, obstacles=True)    # map-aware; status bits as STATUS_* below
 
 The controllers are csrc/rlca_orca.cu; `orca_host` / `nh_orca_host` run the same code on the CPU from numpy arrays.
+
+    nc = NonCooperative(env, mask)         # DESIGN.md §9h: masked robots drive straight to their goals
+    nc.apply(action)                       # overwrites the masked rows of any controller's or policy's action
 """
 from __future__ import annotations
 
@@ -256,6 +259,51 @@ def nh_orca_host(cfg, pose, goal, meta, radius=NH_DEFAULTS['radius'], neighbour_
     orca_host."""
     return _host('rlca_nh_orca_action_host', cfg, pose, goal, meta,
                  (radius, neighbour_dist, time_horizon, tracking_error, heading_time), obstacles, obstacle_time_horizon)
+
+
+class NonCooperative:
+    """Non-cooperative robots (rlca_noncoop_action, DESIGN.md §9h): the agents with `mask` != 0 drive straight to their
+    goals at `speed` (default cfg.v_max) with ORCA-DD's heading tracker (gain `heading_gain`), ignoring every other
+    robot and the map.  `mask` (N) is held on the env's device as uint8."""
+
+    def __init__(self, env, mask, speed=None, heading_gain=DEFAULTS['heading_gain']):
+        self.env = env
+        self.mask = torch.as_tensor(mask, device=env.device).to(torch.uint8).contiguous()
+        if self.mask.shape != (env.N,):
+            raise ValueError(f'mask must have ({env.N},) entries')
+        self.speed = float(env.cfg.v_max) if speed is None else float(speed)
+        self.heading_gain = float(heading_gain)
+
+    def apply(self, action):
+        """Overwrite the masked rows of `action` ((N, 2) float32, contiguous, on the env's device) in place, from the
+        state the next tick reads, on the env's stream; returns `action`."""
+        env = self.env
+        if action.shape != (env.N, 2) or action.dtype != torch.float32 or not action.is_contiguous() or \
+                action.device != self.mask.device:
+            raise ValueError(f'action must be a contiguous ({env.N}, 2) float32 tensor on {self.mask.device}')
+        st = env._state_struct(env._cur)
+        _lib.check(env.lib.rlca_noncoop_action(C.byref(env.cfg), C.byref(st), _ptr(self.mask), self.speed,
+                                               self.heading_gain, _ptr(action), env._stream()))
+        return action
+
+
+def noncoop_host(cfg, pose, goal, meta, mask, action, speed=None, heading_gain=DEFAULTS['heading_gain']):
+    """rlca_noncoop_action_host on numpy arrays, as orca_host: returns a copy of `action` (N, 2) whose rows with
+    mask != 0 are overwritten."""
+    lib = _lib.load()
+    p = np.ascontiguousarray(pose, np.float32)
+    g = np.ascontiguousarray(goal, np.float32)
+    m = np.ascontiguousarray(meta, np.int32)
+    k = np.ascontiguousarray(mask, np.uint8)
+    act = np.array(action, np.float32, order='C', copy=True)
+    n = cfg.robots_per_world * cfg.num_worlds
+    if p.shape != (n, 4) or g.shape != (n, 4) or m.shape != (n, 4) or k.shape != (n,) or act.shape != (n, 2):
+        raise ValueError(f'pose, goal and meta must be ({n}, 4), mask ({n},) and action ({n}, 2)')
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    _lib.check(lib.rlca_noncoop_action_host(C.byref(cfg), vp(p), vp(g), vp(m), vp(k),
+                                            float(cfg.v_max) if speed is None else float(speed), float(heading_gain),
+                                            vp(act)))
+    return act
 
 
 def nh_orca_polygon(cfg, tracking_error=NH_DEFAULTS['tracking_error'], heading_time=NH_DEFAULTS['heading_time']):

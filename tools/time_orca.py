@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Time one rlca_orca_action launch (the ORCA-DD controller, DESIGN.md §9d) and one rlca_nh_orca_action launch (NH-ORCA,
-§9e), map-blind and map-aware (§9f), with CUDA events over many launches, on states after random-action ticks: stage 1
-at 171 x 24 agents and the 50-robot circle at 41 x 50.  The four rows alternate, each timed twice per size.
+§9e), map-blind and map-aware (§9f), and one rlca_noncoop_action launch with every agent non-cooperative (§9h), with
+CUDA events over many launches, on states after random-action ticks: stage 1 at 171 x 24 agents and the 50-robot circle
+at 41 x 50.  The five rows alternate, each timed twice per size.
 
     python tools/time_orca.py [--launches 2000]
 """
@@ -16,7 +17,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET  # noqa: E402
-from rl_collision_avoidance_b200.orca import NhOrcaController, OrcaController  # noqa: E402
+from rl_collision_avoidance_b200.orca import NhOrcaController, NonCooperative, OrcaController  # noqa: E402
 from rl_collision_avoidance_b200.stage_world import StageWorld  # noqa: E402
 
 
@@ -43,6 +44,21 @@ def time_one(scenario, worlds, launches, make, warmup=200):
             'fallback_share': fallback, 'status_bit_shares': [float(((st >> b) & 1).float().mean()) for b in range(3)]}
 
 
+class NonCoop:
+    """rlca_noncoop_action (§9h) with every agent masked, overwriting one action buffer."""
+
+    def __init__(self, env):
+        self.nc = NonCooperative(env, np.ones(env.N, np.uint8))
+        self.action = torch.zeros(env.N, 2, device=env.device)
+        self._status = torch.zeros(env.N, dtype=torch.int32, device=env.device)
+
+    def __call__(self):
+        return self.nc.apply(self.action)
+
+    def status(self):
+        return self._status
+
+
 def OrcaMap(env):
     return OrcaController(env, obstacles=True)
 
@@ -62,7 +78,7 @@ def main():
     except (OSError, subprocess.CalledProcessError):
         power = 'unknown'
     rows = [time_one(scenario, worlds, args.launches, make) for scenario, worlds in (('stage1', 171), ('circle', 41))
-            for _ in range(2) for make in (OrcaController, OrcaMap, NhOrcaController, NhOrcaMap)]
+            for _ in range(2) for make in (OrcaController, OrcaMap, NhOrcaController, NhOrcaMap, NonCoop)]
     print(json.dumps({'card': card, 'power_limit': power, 'launches': args.launches, 'rows': rows}))
 
 
