@@ -1,12 +1,14 @@
 #!/usr/bin/env python
-"""Deterministic evaluation of a policy on stage 1, stage 2 or the circle swap, with the metrics of the paper the
-reference accompanies (DESIGN.md §9c): success / crash / time-out rates, and over the successful episodes the mean and
-population std of extra time, extra distance and average speed.  Every robot drives with the policy's mean action
-(--policy), with the ORCA-DD baseline controller (--baseline orca, DESIGN.md §9d) or with the paper's NH-ORCA baseline
-(--baseline nh-orca, DESIGN.md §9e) until it has --episodes recorded episodes (circle: one) or --max-ticks ticks have
-run.  --orca-map lets either baseline see the static map's walls (obstacle half-planes, DESIGN.md §9f).
---non-cooperative K makes K robots of every world drive straight to their goals, ignoring everyone else, and adds the
-metrics of each role (DESIGN.md §9h).
+"""Deterministic evaluation of a policy on stage 1, stage 2, the circle swap or random scenarios, with the metrics of
+the paper the reference accompanies (DESIGN.md §9c): success / crash / time-out rates, and over the successful episodes
+the mean and population std of extra time, extra distance and average speed.  Every robot drives with the policy's
+mean action (--policy), with the ORCA-DD baseline controller (--baseline orca, DESIGN.md §9d) or with the paper's
+NH-ORCA baseline (--baseline nh-orca, DESIGN.md §9e) until it has --episodes recorded episodes (circle and random: one)
+or --max-ticks ticks have run.  --orca-map lets either baseline see the static map's walls (obstacle half-planes,
+DESIGN.md §9f).  --non-cooperative K makes K robots of every world drive straight to their goals, ignoring everyone else, and adds the
+metrics of each role (DESIGN.md §9h).  --scenario random gives every world its own layout: --random-robots K robots
+start at random positions in a --random-side S m square on circle.world's map, at least --random-separation D m apart,
+with random goals at least --random-min-travel L m away (defaults 8, 10, 1 and S / 2; DESIGN.md §9i).
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -16,9 +18,11 @@ metrics of each role (DESIGN.md §9h).
     python evaluate.py --scenario stage2 --baseline nh-orca --orca-map --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 1 \\
         --non-cooperative 5
+    python evaluate.py --scenario random --baseline nh-orca --orca-map --num-worlds 1024 --random-robots 16
 """
 import argparse
 import json
+import math
 import os
 
 import torch
@@ -27,12 +31,17 @@ from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, evaluate
 from rl_collision_avoidance_b200.model.net import CNNPolicy
 from rl_collision_avoidance_b200.orca import NonCooperative, add_arguments as add_controller_arguments, \
     check_arguments as check_controller_arguments, from_arguments as controller_from_arguments
-from rl_collision_avoidance_b200.scenarios import COMMON, make_scenario
+from rl_collision_avoidance_b200.scenarios import COMMON, RANDOM_DEFAULTS, make_scenario
 from rl_collision_avoidance_b200.stage_world import StageWorld
 
 LASER_BEAM = 512
 LASER_HIST = 3
 CIRCLE_MAX_TICKS = 1500          # 25 m radius: the 49.5 m to the goal radius take at least 495 ticks at v_max
+
+
+def random_max_ticks(side):
+    """3 x the ticks the square's diagonal takes at v_max: the default tick budget of a random scenario."""
+    return 3 * math.ceil(side * math.sqrt(2.0) / (COMMON['v_max'] * COMMON['dt']))
 
 
 def main(argv=None):
@@ -44,12 +53,22 @@ def main(argv=None):
                      help='drive with the ORCA-DD or the NH-ORCA controller instead of a policy')
     add_controller_arguments(ap)
     ap.add_argument('--num-worlds', type=int, default=1)
-    ap.add_argument('--episodes', type=int, default=1, help='recorded episodes per robot (circle: at most 1)')
+    ap.add_argument('--episodes', type=int, default=1, help='recorded episodes per robot (circle, random: at most 1)')
     ap.add_argument('--seed', type=int, default=0)
     ap.add_argument('--max-ticks', type=int, default=None,
-                    help='default: episodes x (timeout + 1) on stage 1 / 2, %d on the circle' % CIRCLE_MAX_TICKS)
+                    help='default: episodes x (timeout + 1) on stage 1 / 2, %d on the circle, '
+                         '3 ceil(S sqrt(2) / (v_max dt)) on random' % CIRCLE_MAX_TICKS)
     ap.add_argument('--circle-robots', type=int, default=None, help='K robots on the circle (default: the 50-row table)')
     ap.add_argument('--circle-radius', type=float, default=None, help='circle radius in metres (default 25)')
+    ap.add_argument('--random-robots', type=int, default=None, metavar='K',
+                    help='random: robots per world, 2..64 (default %d)' % RANDOM_DEFAULTS['robots_per_world'])
+    ap.add_argument('--random-side', type=float, default=None, metavar='S',
+                    help='random: side of the square of starts and goals, m (default %g)' % RANDOM_DEFAULTS['side'])
+    ap.add_argument('--random-separation', type=float, default=None, metavar='D',
+                    help='random: least start-start and goal-goal distance, m (default %g)'
+                         % RANDOM_DEFAULTS['separation'])
+    ap.add_argument('--random-min-travel', type=float, default=None, metavar='L',
+                    help='random: least start-goal distance, m (default S / 2)')
     ap.add_argument('--check-every', type=int, default=50)
     ap.add_argument('--non-cooperative', type=int, default=None, metavar='K',
                     help='K robots per world (robots floor(j R / K), j < K) drive straight to their goals and ignore '
@@ -65,13 +84,25 @@ def main(argv=None):
         ap.error('--orca-map applies to --baseline orca / nh-orca only')
     if args.scenario != 'circle' and (args.circle_robots is not None or args.circle_radius is not None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
+    random_args = (args.random_robots, args.random_side, args.random_separation, args.random_min_travel)
+    if args.scenario != 'random' and any(a is not None for a in random_args):
+        ap.error('--random-robots / --random-side / --random-separation / --random-min-travel apply to '
+                 '--scenario random only')
     if args.non_cooperative is None and args.non_cooperative_speed is not None:
         ap.error('--non-cooperative-speed applies with --non-cooperative only')
     v_max = COMMON['v_max']
     if args.non_cooperative_speed is not None and not 0.0 < args.non_cooperative_speed <= v_max:
         ap.error('--non-cooperative-speed must be in (0, %g]' % v_max)
-    sc = make_scenario(args.scenario, robots_per_world=args.circle_robots, radius=args.circle_radius) \
-        if args.scenario == 'circle' else make_scenario(args.scenario)
+    if args.scenario == 'circle':
+        sc = make_scenario(args.scenario, robots_per_world=args.circle_robots, radius=args.circle_radius)
+    elif args.scenario == 'random':
+        try:
+            sc = make_scenario('random', robots_per_world=args.random_robots, side=args.random_side,
+                               separation=args.random_separation, min_travel=args.random_min_travel)
+        except ValueError as e:
+            ap.error(str(e))
+    else:
+        sc = make_scenario(args.scenario)
     if args.non_cooperative is not None and not 1 <= args.non_cooperative <= sc.robots_per_world:
         ap.error('--non-cooperative must be in 1..%d on %s' % (sc.robots_per_world, args.scenario))
     env = StageWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, seed=args.seed,
@@ -82,8 +113,14 @@ def main(argv=None):
         policy = CNNPolicy(frames=LASER_HIST, action_space=2, max_batch=env.N)
         policy.load_state_dict(torch.load(args.policy, map_location='cuda'))
         controller = None
-    max_ticks = args.max_ticks if args.max_ticks is not None else \
-        (CIRCLE_MAX_TICKS if args.scenario == 'circle' else args.episodes * (sc.timeout + 1))
+    if args.max_ticks is not None:
+        max_ticks = args.max_ticks
+    elif args.scenario == 'circle':
+        max_ticks = CIRCLE_MAX_TICKS
+    elif args.scenario == 'random':
+        max_ticks = random_max_ticks(sc.layout.side)
+    else:
+        max_ticks = args.episodes * (sc.timeout + 1)
     nc = None
     if args.non_cooperative is not None:
         nc = NonCooperative(env, non_cooperative_mask(sc.robots_per_world, args.num_worlds, args.non_cooperative),

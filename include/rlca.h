@@ -591,6 +591,40 @@ typedef struct rlca_demo_set {
 int rlca_demo_append(const rlca_env_config *cfg, const rlca_env_state *state, const rlca_step_io *io,
                      const rlca_demo_set *demo, void *stream);
 
+/* =====================================================================================
+ * Random layouts (csrc/rlca_layout.cu, DESIGN.md §9i): every world of an evaluation gets its own starts and goals,
+ * drawn on the device once before the episode.
+ * ===================================================================================== */
+
+/* side        edge of the square [-side/2, side/2]^2 that holds every start and goal, m
+ * separation  least distance between two starts and between two goals, m
+ * min_travel  least distance from a robot's start to its goal, m */
+typedef struct rlca_layout_params {
+    float side;
+    float separation;
+    float min_travel;
+} rlca_layout_params;
+
+/* Writes a layout into `state` in place.  World w (global index cfg->world_offset + w), robots r = 0 .. R-1 in order:
+ * the start is the first try k < cfg->max_reject whose uniform draw in the square is at least `separation` from the
+ * starts of robots 0 .. r-1; the goal the first try whose draw is at least `min_travel` from this start and
+ * `separation` from the goals of robots 0 .. r-1; the heading one draw u * 2 pi wrapped into (-pi, pi].  Draws are the
+ * env's Philox draws with agent = global world * R + r, episode 0, draw k and purposes 3 (start), 4 (goal), 5
+ * (heading), so a world's layout does not depend on num_worlds or on sharding.  Distances are compared squared in
+ * float32.  Written per robot: pose = (x, y, theta, pre_distance) with pre_distance 0 when cfg->pre_distance_zero and
+ * |goal - start| otherwise, goal.xy, acc.zw = (x, y) (the init pose); every other field is kept.
+ *   status_dev  (num_worlds) int32: 0 = placed; 1 + r when robot r found no accepted try, and the world's rows are then
+ *               left untouched
+ * RLCA_ERR_INVALID for a NULL pointer, robots_per_world outside 2..64, side not finite and > 0, min_travel outside
+ * [0, side sqrt(2)], or separation <= 2 (r_c + sqrt(2) resolution), r_c = sqrt(half_len^2 + half_wid^2): two
+ * footprints that far apart share no cell whatever their headings. */
+int rlca_layout_random(const rlca_env_config *cfg, const rlca_layout_params *params, const rlca_env_state *state,
+                       int32_t *status_dev, void *stream);
+/* The same from HOST buffers (pose, goal, acc: (N,4) float; status: (num_worlds) int32) by a sequential loop over
+ * the tries; the outputs equal rlca_layout_random's bit for bit. */
+int rlca_layout_random_host(const rlca_env_config *cfg, const rlca_layout_params *params, float *pose_host,
+                            float *goal_host, float *acc_host, int32_t *status_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

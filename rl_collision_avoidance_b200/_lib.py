@@ -63,6 +63,11 @@ class DemoSet(C.Structure):
                 ('count_dev', C.c_void_p), ('capacity', C.c_int64)]
 
 
+class LayoutParams(C.Structure):
+    """Mirror of rlca_layout_params (include/rlca.h)."""
+    _fields_ = [('side', C.c_float), ('separation', C.c_float), ('min_travel', C.c_float)]
+
+
 # rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
 EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
                  'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
@@ -153,6 +158,8 @@ SYMBOLS = {
                                                 C.c_float, _P, _P, _P]),
     'rlca_demo_append': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), C.POINTER(StepIO), C.POINTER(DemoSet),
                                    _P]),
+    'rlca_layout_random': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), C.POINTER(EnvState), _P, _P]),
+    'rlca_layout_random_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), _P, _P, _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

@@ -21,6 +21,51 @@ inline int rlca_set_err(int code, const char *fmt, const char *a = "", const cha
             return rlca_set_err(RLCA_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e__)); \
     } while (0)
 
+// angle wrap of the numerics contract: at most one step of 2 pi towards (-pi, pi]
+__host__ __device__ __forceinline__ float dev_normalize(float a)
+{
+    const float pi_f = 3.14159274101257324219f;
+    const float two_pi_f = 6.28318548202514648438f;
+    if (a > pi_f) a -= two_pi_f;
+    else if (a <= -pi_f) a += two_pi_f;
+    return a;
+}
+
+// high 32 bits of a * b
+__host__ __device__ __forceinline__ uint32_t dev_umulhi(uint32_t a, uint32_t b)
+{
+#ifdef __CUDA_ARCH__
+    return __umulhi(a, b);
+#else
+    return (uint32_t)(((uint64_t)a * (uint64_t)b) >> 32);
+#endif
+}
+
+// Philox-4x32-10 on the counter c with key (k0, k1)
+__host__ __device__ __forceinline__ void dev_philox(uint32_t (&c)[4], uint32_t k0, uint32_t k1)
+{
+#pragma unroll
+    for (int i = 0; i < 10; ++i) {
+        uint32_t hi0 = dev_umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
+        uint32_t hi1 = dev_umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
+        uint32_t n0 = hi1 ^ c[1] ^ k0;
+        uint32_t n2 = hi0 ^ c[3] ^ k1;
+        c[0] = n0; c[1] = lo1; c[2] = n2; c[3] = lo0;
+        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+    }
+}
+
+// Four uniforms in [0, 1) (24 bits each) keyed by (seed, agent, episode, draw, purpose).  Purposes: 1 spawn and
+// heading, 2 goal (rlca_env.cu); 3 start, 4 goal, 5 heading of a random layout (rlca_layout.cu).
+__host__ __device__ __forceinline__ void dev_rand4(uint64_t seed, uint32_t agent, uint32_t episode, uint32_t draw,
+                                                   uint32_t purpose, float (&u)[4])
+{
+    uint32_t c[4] = { agent, episode, draw, purpose };
+    dev_philox(c, (uint32_t)seed, (uint32_t)(seed >> 32));
+#pragma unroll
+    for (int i = 0; i < 4; ++i) u[i] = (float)(c[i] >> 8) * 5.9604644775390625e-08f;
+}
+
 // sin / cos of the numerics contract (DESIGN.md §4): explicit FMAs only, so a host build without contraction
 // (-ffp-contract=off) rounds exactly as the device does.
 __host__ __device__ __forceinline__ void dev_sincosf(float x, float &s, float &c)

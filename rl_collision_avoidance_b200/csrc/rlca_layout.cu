@@ -1,0 +1,234 @@
+// rlca_layout.cu — random start / goal layouts for evaluation (sm_90a), C ABI in include/rlca.h, DESIGN.md §9i.
+//
+// rlca_layout_random writes a layout into an env state in place, once before an episode: for world w (global index
+// cfg.world_offset + w) and robots r = 0 .. R-1 in order, the start is the first try k < max_reject whose draw,
+// uniform in the square [-side/2, side/2]^2, is at least `separation` from the starts placed so far; the goal the
+// first try whose draw is at least `min_travel` from this start and `separation` from the goals placed so far; the
+// heading one draw u * 2 pi, wrapped as the env's spawn wraps it.  Draws use the env's Philox keys with agent =
+// global world * R + r, episode 0, draw k and purposes 3 (start), 4 (goal), 5 (heading), so a world's layout depends
+// only on (seed, global world, R, parameters, max_reject).
+//
+// Distances are compared squared, and draws and tests use plain float32 + - x (this file is compiled with
+// -fmad=false on the device and -ffp-contract=off on the host), so rlca_layout_random_host gives the same bits.
+//
+// One warp per world, the world's placed starts and goals in shared memory: lane l evaluates try base + l and the
+// lowest accepting lane wins (ballot, shuffle) in rounds of 32 tries — the order of the host's sequential loop.  When
+// no try of the budget is accepted the world's rows are left untouched and status[w] = 1 + r.
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <math.h>
+
+#include "../../include/rlca.h"
+#include "rlca_common.cuh"
+
+#define LAYOUT_THREADS 256
+#define LAYOUT_WARPS (LAYOUT_THREADS / 32)
+
+namespace {
+
+struct LayoutConsts {
+    uint64_t seed;
+    uint32_t agent0;         // global agent index of the world's robot 0
+    float side, sep2, travel2;
+};
+
+// try k of robot r's start (purpose 3) or goal (purpose 4): uniform in the square, one rounding per coordinate
+// ((u - 0.5) is exact for the 24-bit uniforms)
+__host__ __device__ __forceinline__ void layout_draw(const LayoutConsts &c, uint32_t r, uint32_t k, uint32_t purpose,
+                                                     float &x, float &y)
+{
+    float u[4];
+    dev_rand4(c.seed, c.agent0 + r, 0u, k, purpose, u);
+    x = (u[0] - 0.5f) * c.side;
+    y = (u[1] - 0.5f) * c.side;
+}
+
+__host__ __device__ __forceinline__ float layout_heading(const LayoutConsts &c, uint32_t r)
+{
+    float u[4];
+    dev_rand4(c.seed, c.agent0 + r, 0u, 0u, 5u, u);
+    return dev_normalize(u[0] * 6.28318548202514648438f);
+}
+
+__host__ __device__ __forceinline__ float dist2(float ax, float ay, float bx, float by)
+{
+    const float dx = ax - bx, dy = ay - by;
+    return dx * dx + dy * dy;
+}
+
+// a start draw at least `separation` from the starts px/py[0 .. r-1]
+__host__ __device__ __forceinline__ bool start_ok(const LayoutConsts &c, const float *px, const float *py, int r,
+                                                  float x, float y)
+{
+    for (int j = 0; j < r; ++j)
+        if (!(dist2(x, y, px[j], py[j]) >= c.sep2)) return false;
+    return true;
+}
+
+// a goal draw at least `min_travel` from the start (sx, sy) and `separation` from the goals qx/qy[0 .. r-1]
+__host__ __device__ __forceinline__ bool goal_ok(const LayoutConsts &c, const float *qx, const float *qy, int r,
+                                                 float sx, float sy, float x, float y)
+{
+    if (!(dist2(x, y, sx, sy) >= c.travel2)) return false;
+    return start_ok(c, qx, qy, r, x, y);
+}
+
+// The records of one placed robot, as apply_spawn (rlca_env.cu) writes a spawn without starting an episode.
+__host__ __device__ __forceinline__ void layout_apply(int pre_distance_zero, float x, float y, float th, float gx,
+                                                      float gy, float4 &pose, float4 &goal, float4 &acc)
+{
+    pose.x = x; pose.y = y; pose.z = th;
+    goal.x = gx; goal.y = gy;
+    const float ddx = gx - x, ddy = gy - y;
+    const float d0 = sqrtf(fmaf(ddx, ddx, ddy * ddy));
+    pose.w = pre_distance_zero ? 0.0f : d0;
+    acc.z = x; acc.w = y;
+}
+
+struct LayoutSmem {
+    float sx[RLCA_MAX_ROBOTS_PER_WORLD], sy[RLCA_MAX_ROBOTS_PER_WORLD];
+    float gx[RLCA_MAX_ROBOTS_PER_WORLD], gy[RLCA_MAX_ROBOTS_PER_WORLD];
+};
+
+// The first accepted try of robot r (purpose 3: start, 4: goal) by the whole warp; false when none of the budget is.
+__device__ __forceinline__ bool warp_place(const LayoutConsts &c, const LayoutSmem &s, int r, uint32_t purpose,
+                                           int max_reject, int lane, float &ox, float &oy)
+{
+    for (int base = 0; base < max_reject; base += 32) {
+        const int k = base + lane;
+        float x = 0.f, y = 0.f;
+        bool ok = false;
+        if (k < max_reject) {
+            layout_draw(c, (uint32_t)r, (uint32_t)k, purpose, x, y);
+            ok = purpose == 3u ? start_ok(c, s.sx, s.sy, r, x, y) : goal_ok(c, s.gx, s.gy, r, s.sx[r], s.sy[r], x, y);
+        }
+        const uint32_t mask = __ballot_sync(0xffffffffu, ok);
+        if (mask) {
+            const int src = __ffs(mask) - 1;
+            ox = __shfl_sync(0xffffffffu, x, src);
+            oy = __shfl_sync(0xffffffffu, y, src);
+            return true;
+        }
+    }
+    return false;
+}
+
+__global__ void __launch_bounds__(LAYOUT_THREADS)
+rlca_layout_random_kernel(int num_worlds, int R, int max_reject, int pre_distance_zero, int world_offset,
+                          uint64_t seed, float side, float sep2, float travel2, float4 *__restrict__ pose,
+                          float4 *__restrict__ goal, float4 *__restrict__ acc, int32_t *__restrict__ status)
+{
+    __shared__ LayoutSmem smem[LAYOUT_WARPS];
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int w = blockIdx.x * LAYOUT_WARPS + wib;
+    if (w >= num_worlds) return;                     // warp-uniform
+    LayoutSmem &s = smem[wib];
+    const LayoutConsts c = { seed, (uint32_t)(world_offset + w) * (uint32_t)R, side, sep2, travel2 };
+    for (int r = 0; r < R; ++r) {
+        float x, y, gx, gy;
+        if (!warp_place(c, s, r, 3u, max_reject, lane, x, y)) {
+            if (lane == 0) status[w] = 1 + r;
+            return;
+        }
+        if (lane == 0) { s.sx[r] = x; s.sy[r] = y; }
+        __syncwarp();
+        if (!warp_place(c, s, r, 4u, max_reject, lane, gx, gy)) {
+            if (lane == 0) status[w] = 1 + r;
+            return;
+        }
+        if (lane == 0) { s.gx[r] = gx; s.gy[r] = gy; }
+        __syncwarp();
+    }
+    for (int r = lane; r < R; r += 32) {
+        const size_t i = (size_t)w * R + r;
+        float4 p = pose[i], g = goal[i], a = acc[i];
+        layout_apply(pre_distance_zero, s.sx[r], s.sy[r], layout_heading(c, (uint32_t)r), s.gx[r], s.gy[r], p, g, a);
+        pose[i] = p; goal[i] = g; acc[i] = a;
+    }
+    if (lane == 0) status[w] = 0;
+}
+
+int check_layout(const rlca_env_config *cfg, const rlca_layout_params *params, const char *who)
+{
+    if (!cfg || !params) return rlca_set_err(RLCA_ERR_INVALID, "%s: cfg or params is NULL", who);
+    if (cfg->robots_per_world < 2 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD)
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: robots_per_world must be in [2, 64]", who);
+    if (cfg->num_worlds < 1) return rlca_set_err(RLCA_ERR_INVALID, "%s: num_worlds must be >= 1", who);
+    if (cfg->max_reject < 1) return rlca_set_err(RLCA_ERR_INVALID, "%s: max_reject must be >= 1", who);
+    if (cfg->world_offset < 0) return rlca_set_err(RLCA_ERR_INVALID, "%s: world_offset must be >= 0", who);
+    const double side = params->side;
+    if (!(side > 0.0 && side < INFINITY)) return rlca_set_err(RLCA_ERR_INVALID, "%s: side must be finite and > 0", who);
+    if (!(params->min_travel >= 0.0f && (double)params->min_travel <= side * sqrt(2.0)))
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: min_travel must be in [0, side * sqrt(2)]", who);
+    // two footprints whose centres are this far apart share no cell, whatever their headings
+    const double rc = sqrt((double)cfg->half_len * cfg->half_len + (double)cfg->half_wid * cfg->half_wid);
+    if (!(params->separation > 2.0 * (rc + sqrt(2.0) * (double)cfg->resolution) && params->separation < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID,
+                            "%s: separation must be finite and > 2 (r_c + sqrt(2) resolution), r_c the footprint's "
+                            "circumradius", who);
+    return RLCA_OK;
+}
+
+LayoutConsts layout_consts(const rlca_env_config *cfg, const rlca_layout_params *params, int w)
+{
+    return { cfg->seed, (uint32_t)(cfg->world_offset + w) * (uint32_t)cfg->robots_per_world, params->side,
+             params->separation * params->separation, params->min_travel * params->min_travel };
+}
+
+}  // namespace
+
+extern "C" int rlca_layout_random(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                  const rlca_env_state *state, int32_t *status_dev, void *stream)
+{
+    int rc = check_layout(cfg, params, "rlca_layout_random");
+    if (rc) return rc;
+    if (!state || !state->pose_dev || !state->goal_dev || !state->acc_dev || !status_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_layout_random: a state or status buffer is NULL");
+    const LayoutConsts c = layout_consts(cfg, params, 0);
+    const int ctas = (cfg->num_worlds + LAYOUT_WARPS - 1) / LAYOUT_WARPS;
+    rlca_layout_random_kernel<<<ctas, LAYOUT_THREADS, 0, (cudaStream_t)stream>>>(
+        cfg->num_worlds, cfg->robots_per_world, cfg->max_reject, cfg->pre_distance_zero, cfg->world_offset, c.seed,
+        c.side, c.sep2, c.travel2, reinterpret_cast<float4 *>(state->pose_dev),
+        reinterpret_cast<float4 *>(state->goal_dev), reinterpret_cast<float4 *>(state->acc_dev), status_dev);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_layout_random_host(const rlca_env_config *cfg, const rlca_layout_params *params, float *pose_host,
+                                       float *goal_host, float *acc_host, int32_t *status_host)
+{
+    int rc = check_layout(cfg, params, "rlca_layout_random_host");
+    if (rc) return rc;
+    if (!pose_host || !goal_host || !acc_host || !status_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_layout_random_host: a buffer is NULL");
+    const int R = cfg->robots_per_world;
+    float4 *pose = reinterpret_cast<float4 *>(pose_host), *goal = reinterpret_cast<float4 *>(goal_host);
+    float4 *acc = reinterpret_cast<float4 *>(acc_host);
+    for (int w = 0; w < cfg->num_worlds; ++w) {
+        const LayoutConsts c = layout_consts(cfg, params, w);
+        float sx[RLCA_MAX_ROBOTS_PER_WORLD], sy[RLCA_MAX_ROBOTS_PER_WORLD];
+        float gx[RLCA_MAX_ROBOTS_PER_WORLD], gy[RLCA_MAX_ROBOTS_PER_WORLD];
+        int failed = 0;
+        for (int r = 0; r < R && !failed; ++r) {
+            int k = 0;
+            for (; k < cfg->max_reject; ++k) {
+                layout_draw(c, (uint32_t)r, (uint32_t)k, 3u, sx[r], sy[r]);
+                if (start_ok(c, sx, sy, r, sx[r], sy[r])) break;
+            }
+            if (k == cfg->max_reject) { failed = 1 + r; break; }
+            for (k = 0; k < cfg->max_reject; ++k) {
+                layout_draw(c, (uint32_t)r, (uint32_t)k, 4u, gx[r], gy[r]);
+                if (goal_ok(c, gx, gy, r, sx[r], sy[r], gx[r], gy[r])) break;
+            }
+            if (k == cfg->max_reject) failed = 1 + r;
+        }
+        status_host[w] = failed;
+        if (failed) continue;
+        for (int r = 0; r < R; ++r) {
+            const size_t i = (size_t)w * R + r;
+            layout_apply(cfg->pre_distance_zero, sx[r], sy[r], layout_heading(c, (uint32_t)r), gx[r], gy[r], pose[i],
+                         goal[i], acc[i]);
+        }
+    }
+    return RLCA_OK;
+}

@@ -20,6 +20,14 @@ from .worldfile import WorldMap, load_map
 ASSETS = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'assets')
 
 
+@dataclass(frozen=True)
+class Layout:
+    """Parameters of a random layout (rlca_layout_params, DESIGN.md §9i), in metres."""
+    side: float                # starts and goals lie in the square [-side/2, side/2]^2
+    separation: float          # least start-start and goal-goal distance
+    min_travel: float          # least start-goal distance
+
+
 @dataclass
 class Scenario:
     name: str
@@ -32,6 +40,7 @@ class Scenario:
     init_tab: np.ndarray       # (R,4) x,y,theta,random_flag  float32
     goal_tab: np.ndarray       # (R,4) gx,gy,random_flag,group id   float32
     groups: tuple = ()         # stage-2 group boundaries (model/utils.py:83)
+    layout: Layout | None = None   # random scenario: every world draws its own layout (StageWorld.random_layout)
 
 
 # constants shared by the three env clients (stage_world1.py:34,183-204)
@@ -109,11 +118,81 @@ def circle_layout(m: WorldMap, robots: int, radius: float):
     return init, goal
 
 
+RANDOM_DEFAULTS = dict(robots_per_world=8, side=10.0, separation=1.0)     # min_travel defaults to side / 2
+
+
+def random_layout_params(m: WorldMap, robots: int, side: float, separation: float, min_travel: float) -> Layout:
+    """The Layout of a random scenario on map `m` after the checks rlca_layout_random makes (in float32, as it sees the
+    values), and that the square grown by the footprint's circumradius r_c and one cell lies on free cells of the map.
+    ValueError otherwise."""
+    K = int(robots)
+    if not 2 <= K <= 64:
+        raise ValueError(f'random: robots_per_world must be in 2..64, got {robots}')
+    S, D, L = (float(np.float32(v)) for v in (side, separation, min_travel))
+    if not (math.isfinite(S) and S > 0):
+        raise ValueError(f'random: side must be finite and > 0, got {side}')
+    if not 0 <= L <= S * math.sqrt(2.0):
+        raise ValueError(f'random: min_travel must be in [0, side * sqrt(2)] = [0, {S * math.sqrt(2.0):.4g}], '
+                         f'got {min_travel}')
+    hl, hw = (float(np.float32(COMMON[k])) for k in ('half_len', 'half_wid'))
+    res = float(np.float32(m.resolution))
+    rc = math.sqrt(hl * hl + hw * hw)
+    d_min = 2.0 * (rc + math.sqrt(2.0) * res)
+    if not (math.isfinite(D) and D > d_min):
+        raise ValueError(f'random: separation must be finite and > {d_min:.4g} m (two footprints closer than that can '
+                         f'share a cell), got {separation}')
+    e = 0.5 * S + rc + res
+    ppm = 1.0 / m.resolution
+    c0, c1 = math.floor(-e * ppm) + m.origin_cx, math.floor(e * ppm) + m.origin_cx
+    r0, r1 = math.floor(-e * ppm) + m.origin_cy, math.floor(e * ppm) + m.origin_cy
+    if c0 < 0 or r0 < 0 or c1 >= m.grid_w or r1 >= m.grid_h or m.cells[r0:r1 + 1, c0:c1 + 1].any():
+        raise ValueError(f'random: the {S:g} m square grown by {rc + res:.3f} m is not on free cells of the map')
+    return Layout(S, D, L)
+
+
+def random_layout_host(cfg, layout: Layout, pose, goal, acc):
+    """rlca_layout_random_host: the layout of every world of `cfg` (an EnvConfig) written into copies of the host
+    arrays pose, goal, acc (N, 4) float32.  Returns (pose, goal, acc, status (num_worlds,) int32: 0 placed, 1 + r when
+    robot r was not)."""
+    import ctypes as C
+    from . import _lib
+    lib = _lib.load()
+    pose, goal, acc = (np.array(a, np.float32, order='C', copy=True) for a in (pose, goal, acc))
+    n = int(cfg.robots_per_world) * int(cfg.num_worlds)
+    if any(a.shape != (n, 4) for a in (pose, goal, acc)):
+        raise ValueError(f'pose, goal and acc must be ({n}, 4)')
+    status = np.full(int(cfg.num_worlds), -1, np.int32)
+    params = _lib.LayoutParams(layout.side, layout.separation, layout.min_travel)
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    _lib.check(lib.rlca_layout_random_host(C.byref(cfg), C.byref(params), vp(pose), vp(goal), vp(acc), vp(status)))
+    return pose, goal, acc, status
+
+
 def make_scenario(name: str, map_: WorldMap | None = None, robots_per_world: int | None = None,
-                  radius: float | None = None) -> Scenario:
+                  radius: float | None = None, *, side: float | None = None, separation: float | None = None,
+                  min_travel: float | None = None) -> Scenario:
     """`robots_per_world` and `radius` shape the circle scenario (see circle_layout); both None, or 50 robots with no
-    radius, keep the shipped 50-row table of the reference's circle.world."""
+    radius, keep the shipped 50-row table of the reference's circle.world.
+
+    'random' (DESIGN.md §9i): `robots_per_world` robots (default 8) on circle.world's map with the circle's tick
+    constants, whose starts and goals every world draws itself (StageWorld.random_layout) in a `side` m square (default
+    10), starts and goals at least `separation` m apart (default 1), each goal at least `min_travel` m from its start
+    (default side / 2).  The tables are zero; ValueError for parameters rlca_layout_random rejects or a square that
+    leaves the map's free cells."""
     name = name.lower()
+    if name != 'random' and (side is not None or separation is not None or min_travel is not None):
+        raise ValueError('side, separation and min_travel shape the random scenario only')
+    if name == 'random':
+        if radius is not None:
+            raise ValueError('radius shapes the circle scenario only')
+        m = map_ or load_map(os.path.join(ASSETS, 'circle_map.npz'))
+        K = RANDOM_DEFAULTS['robots_per_world'] if robots_per_world is None else robots_per_world
+        S = RANDOM_DEFAULTS['side'] if side is None else side
+        D = RANDOM_DEFAULTS['separation'] if separation is None else separation
+        lay = random_layout_params(m, K, S, D, 0.5 * float(S) if min_travel is None else min_travel)
+        K = int(K)
+        zero = np.zeros((K, 4), np.float32)
+        return Scenario('random', 2, K, 10000, 0.7, 1, m, zero, zero.copy(), layout=lay)
     if name == 'stage1':
         m = map_ or load_map(os.path.join(ASSETS, 'stage1_map.npz'))
         R = robots_per_world or 24

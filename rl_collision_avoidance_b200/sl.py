@@ -68,6 +68,8 @@ def collect(env, controller, samples, record_every=1, check_every=50):
     env.reset_world()
     env.reset_pose()
     env.generate_goal_point()
+    if env.sc.layout is not None:
+        env.random_layout()
     obs = env.get_laser_observation()
     stacks = [obs[:, None, :].repeat(1, 3, 1).contiguous(), torch.empty(N, 3, env.beam_mum, device=dev)]
     terminal = torch.zeros(N, dtype=torch.bool, device=dev)

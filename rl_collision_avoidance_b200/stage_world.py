@@ -179,6 +179,26 @@ class StageWorld:
         _lib.check(self.lib.rlca_env_reset(self._h, C.byref(st), _ptr(None), mode, self._stream()))
         return sc
 
+    def random_layout(self):
+        """A random layout (DESIGN.md §9i) in every world of the current state: starts, goals and headings drawn on the
+        device from the scenario's Layout (rlca_layout_random), then the scan and local goal from the new poses.  One
+        synchronisation reads the per-world status; ValueError names the first world whose robots could not all be
+        placed, and that world keeps its rows."""
+        lay = self.sc.layout
+        if lay is None:
+            raise ValueError(f'scenario {self.sc.name} has no random layout')
+        params = _lib.LayoutParams(lay.side, lay.separation, lay.min_travel)
+        status = torch.empty(self.num_worlds, dtype=torch.int32, device=self.device)
+        st = self._state_struct(self._cur)
+        _lib.check(self.lib.rlca_layout_random(C.byref(self.cfg), C.byref(params), C.byref(st), _ptr(status),
+                                               self._stream()))
+        self._observe()
+        bad = torch.nonzero(status).flatten().cpu()
+        if len(bad):
+            w = int(bad[0])
+            raise ValueError(f'world {int(self.cfg.world_offset) + w}: robot {int(status[w]) - 1} not placed in '
+                             f'{int(self.cfg.max_reject)} tries; lower the density')
+
     def control_pose(self, pose, mask=None):
         """cmd_pose (stage_world1.py:237-249 -> stageros.cpp:282-296): teleport the masked agents (all when None) to
         pose (N, 3) = x, y, yaw; no collision test, stall flag untouched; the next scan is taken from the new pose."""
