@@ -8,7 +8,10 @@ or --max-ticks ticks have run.  --orca-map lets either baseline see the static m
 DESIGN.md §9f).  --non-cooperative K makes K robots of every world drive straight to their goals, ignoring everyone else, and adds the
 metrics of each role (DESIGN.md §9h).  --scenario random gives every world its own layout: --random-robots K robots
 start at random positions in a --random-side S m square on circle.world's map, at least --random-separation D m apart,
-with random goals at least --random-min-travel L m away (defaults 8, 10, 1 and S / 2; DESIGN.md §9i).
+with random goals at least --random-min-travel L m away (defaults 8, 10, 1 and S / 2; DESIGN.md §9i).  --hybrid switches
+the policy per robot by the nearest return of its newest scan: straight to the goal when it is beyond
+--hybrid-r-safe, the policy's action with v capped at --hybrid-v-safe when it is within --hybrid-r-risk, the policy's
+action otherwise, and prints the share of robot-ticks in each mode (DESIGN.md §9j).
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -19,6 +22,7 @@ with random goals at least --random-min-travel L m away (defaults 8, 10, 1 and S
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 1 \\
         --non-cooperative 5
     python evaluate.py --scenario random --baseline nh-orca --orca-map --num-worlds 1024 --random-robots 16
+    python evaluate.py --scenario random --policy tests/golden/checkpoints/stage2.pth --num-worlds 1024 --hybrid
 """
 import argparse
 import json
@@ -29,8 +33,9 @@ import torch
 
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, evaluate, non_cooperative_mask
 from rl_collision_avoidance_b200.model.net import CNNPolicy
-from rl_collision_avoidance_b200.orca import NonCooperative, add_arguments as add_controller_arguments, \
-    check_arguments as check_controller_arguments, from_arguments as controller_from_arguments
+from rl_collision_avoidance_b200.orca import HYBRID_DEFAULTS, Hybrid, NonCooperative, \
+    add_arguments as add_controller_arguments, check_arguments as check_controller_arguments, check_hybrid, \
+    from_arguments as controller_from_arguments
 from rl_collision_avoidance_b200.scenarios import COMMON, RANDOM_DEFAULTS, make_scenario
 from rl_collision_avoidance_b200.stage_world import StageWorld
 
@@ -75,6 +80,16 @@ def main(argv=None):
                          'everyone else; the metrics are also printed per role (DESIGN.md §9h)')
     ap.add_argument('--non-cooperative-speed', type=float, default=None, metavar='S',
                     help='speed of the non-cooperative robots, m/s, in (0, v_max] (default v_max)')
+    ap.add_argument('--hybrid', action='store_true',
+                    help='switch the policy per robot by its nearest scan return: drive straight to the goal in free '
+                         'space, cap the speed near obstacles (DESIGN.md §9j)')
+    ap.add_argument('--hybrid-r-safe', type=float, default=None, metavar='R',
+                    help='hybrid: drive straight to the goal when nothing is within R m (default %g)'
+                         % HYBRID_DEFAULTS['r_safe'])
+    ap.add_argument('--hybrid-r-risk', type=float, default=None, metavar='R',
+                    help='hybrid: cap the speed when something is within R m (default %g)' % HYBRID_DEFAULTS['r_risk'])
+    ap.add_argument('--hybrid-v-safe', type=float, default=None, metavar='V',
+                    help='hybrid: the capped speed, m/s (default %g)' % HYBRID_DEFAULTS['v_safe'])
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -93,6 +108,21 @@ def main(argv=None):
     v_max = COMMON['v_max']
     if args.non_cooperative_speed is not None and not 0.0 < args.non_cooperative_speed <= v_max:
         ap.error('--non-cooperative-speed must be in (0, %g]' % v_max)
+    hybrid_args = (args.hybrid_r_safe, args.hybrid_r_risk, args.hybrid_v_safe)
+    if not args.hybrid and any(a is not None for a in hybrid_args):
+        ap.error('--hybrid-r-safe / --hybrid-r-risk / --hybrid-v-safe apply with --hybrid only')
+    if args.hybrid and args.baseline is not None:
+        ap.error('--hybrid applies to --policy only')
+    hybrid_params = None
+    if args.hybrid:
+        hybrid_params = dict(HYBRID_DEFAULTS)
+        for k, a in zip(('r_safe', 'r_risk', 'v_safe'), hybrid_args):
+            if a is not None:
+                hybrid_params[k] = a
+        try:
+            check_hybrid(COMMON['range_max'], v_max, **hybrid_params)
+        except ValueError as e:
+            ap.error(str(e))
     if args.scenario == 'circle':
         sc = make_scenario(args.scenario, robots_per_world=args.circle_robots, radius=args.circle_radius)
     elif args.scenario == 'random':
@@ -125,7 +155,8 @@ def main(argv=None):
     if args.non_cooperative is not None:
         nc = NonCooperative(env, non_cooperative_mask(sc.robots_per_world, args.num_worlds, args.non_cooperative),
                             speed=args.non_cooperative_speed)
-    out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc)
+    hy = Hybrid(env, **hybrid_params) if args.hybrid else None
+    out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy)
 
     def line(m, robots, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -141,6 +172,10 @@ def main(argv=None):
         k = args.non_cooperative * args.num_worlds
         line(out['by_role']['cooperative'], env.N - k, 'cooperative  ')
         line(out['by_role']['non_cooperative'], k, 'non-cooperative  ')
+    if hy is not None:
+        s = out['modes']
+        print('hybrid modes over %d %srobot-ticks: policy %.4f  driver %.4f  safe %.4f'
+              % (s['agent_ticks'], 'cooperative ' if nc is not None else '', s['policy'], s['driver'], s['safe']))
     if args.json:
         res = {'args': vars(args), 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
@@ -149,6 +184,9 @@ def main(argv=None):
         if nc is not None:
             res['by_role'] = out['by_role']
             res['partials_split'] = out['partials_split'].tolist()
+        if hy is not None:
+            res['modes'] = out['modes']
+            res['mode_counts'] = out['mode_counts'].tolist()
         with open(args.json, 'w') as fh:
             json.dump(res, fh, indent=1)
     return out

@@ -461,6 +461,31 @@ int rlca_noncoop_action_host(const rlca_env_config *cfg, const float *pose_host,
                              const int32_t *meta_host, const uint8_t *mask_host, float speed, float heading_gain,
                              float *action_host);
 
+/* Hybrid controller (DESIGN.md §9j): switches a policy's action per agent by the nearest return of its newest scan.
+ * With m the minimum of frame 2 of the (N,3,beams) scan stack the tick reads (values scan / range_max - 0.5) and
+ * d = (m + 0.5f) * cfg->range_max in metres, action_dev (N,2) is rewritten in place:
+ *   mode 1  d > r_safe   the non-cooperative driver's action at speed cfg->v_max with k_w = heading_gain
+ *   mode 2  d < r_risk   (fminf(v, v_safe), w)
+ *   mode 0  otherwise    unchanged
+ * mode_dev (N uint8) receives the mode.  With open_dev (N int32, rlca_eval_state.open) and counts_dev (N,3 int32) both
+ * set, counts[a][mode] += 1 for every agent with open[a] != 0; both NULL counts nothing.  Needs
+ * 0 <= r_risk <= r_safe <= cfg->range_max (all finite), v_safe in (0, cfg->v_max], heading_gain finite and > 0, and
+ * no NULL buffer (RLCA_ERR_INVALID otherwise).  r_risk = 0 turns mode 2 off; r_safe = range_max turns mode 1 off. */
+typedef struct rlca_hybrid_params {
+    float r_safe;
+    float r_risk;
+    float v_safe;
+    float heading_gain;
+} rlca_hybrid_params;
+int rlca_hybrid_action(const rlca_env_config *cfg, const rlca_hybrid_params *params, const rlca_env_state *state,
+                       const float *stack_dev, const int32_t *open_dev, float *action_dev, uint8_t *mode_dev,
+                       int32_t *counts_dev, void *stream);
+/* The same from HOST buffers (stack (N,3,beams) float; pose, goal: (N,4) float; meta: (N,4) int32); equal to
+ * rlca_hybrid_action bit for bit. */
+int rlca_hybrid_action_host(const rlca_env_config *cfg, const rlca_hybrid_params *params, const float *stack_host,
+                            const float *pose_host, const float *goal_host, const int32_t *meta_host,
+                            const int32_t *open_host, float *action_host, uint8_t *mode_host, int32_t *counts_host);
+
 /* =====================================================================================
  * NH-ORCA baseline controller (csrc/rlca_orca.cu, DESIGN.md §9e): ORCA for non-holonomic robots (Alonso-Mora,
  * Breitenmoser, Rufli, Beardsley, Siegwart, DARS 2010), the paper's baseline.  Static map ignored.

@@ -68,6 +68,11 @@ class LayoutParams(C.Structure):
     _fields_ = [('side', C.c_float), ('separation', C.c_float), ('min_travel', C.c_float)]
 
 
+class HybridParams(C.Structure):
+    """Mirror of rlca_hybrid_params (include/rlca.h)."""
+    _fields_ = [('r_safe', C.c_float), ('r_risk', C.c_float), ('v_safe', C.c_float), ('heading_gain', C.c_float)]
+
+
 # rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
 EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
                  'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
@@ -137,6 +142,10 @@ SYMBOLS = {
                                         _P, _P, _P]),
     'rlca_noncoop_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), _P, C.c_float, C.c_float, _P, _P]),
     'rlca_noncoop_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_float, C.c_float, _P]),
+    'rlca_hybrid_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(HybridParams), C.POINTER(EnvState), _P, _P, _P,
+                                     _P, _P, _P]),
+    'rlca_hybrid_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(HybridParams), _P, _P, _P, _P, _P, _P, _P,
+                                          _P]),
     'rlca_nh_orca_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), C.c_float, C.c_float, C.c_float,
                                       C.c_float, C.c_float, _P, _P, _P, _P]),
     'rlca_nh_orca_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, C.c_float, C.c_float, C.c_float,

@@ -25,6 +25,9 @@
 //
 // The non-cooperative driver (DESIGN.md §9h) overwrites the actions of masked agents with ORCA-DD's answer for an agent
 // without neighbours: straight to the goal, ignoring everyone else.
+//
+// The hybrid controller (DESIGN.md §9j) switches each agent's policy action by the nearest return of its newest scan:
+// the §9h driver in free space, the policy's action with a capped speed near obstacles, the policy's action otherwise.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
@@ -891,6 +894,122 @@ extern "C" int rlca_noncoop_action_host(const rlca_env_config *cfg, const float 
         const float2 act = noncoop_action(pose, goal, meta, a, q);
         action_host[2 * a] = act.x;
         action_host[2 * a + 1] = act.y;
+    }
+    return RLCA_OK;
+}
+
+// ------------------------------------------------------------------------------------ hybrid controller (§9j)
+// The scan minimum d (metres) of frame 2 of the stack picks the mode: 1 = the §9h driver at v_max when d > r_safe,
+// 2 = the policy's action with v capped at v_safe when d < r_risk, 0 = the policy's action otherwise.
+#define HYBRID_MODES 3
+
+struct HybridParams {
+    float r_safe, r_risk, v_safe, range_max;
+};
+
+__host__ __device__ __forceinline__ int hybrid_mode(float scan_min, const HybridParams &h)
+{
+    const float d = (scan_min + 0.5f) * h.range_max;
+    return d > h.r_safe ? 1 : d < h.r_risk ? 2 : 0;
+}
+
+// Agent a's action for `mode`, in place; the count of the mode goes up when the tick belongs to a tracked episode.
+__host__ __device__ __forceinline__ void hybrid_apply(int mode, const float4 *pose, const float4 *goal, const int4 *meta,
+                                                      int a, const OrcaParams &q, const HybridParams &h,
+                                                      const int32_t *open, float2 *action, uint8_t *mode_out,
+                                                      int32_t *counts)
+{
+    if (mode == 1) action[a] = noncoop_action(pose, goal, meta, a, q);
+    else if (mode == 2) action[a].x = fminf(action[a].x, h.v_safe);
+    mode_out[a] = (uint8_t)mode;
+    if (counts && open[a]) ++counts[(size_t)a * HYBRID_MODES + mode];
+}
+
+// One warp per agent: the lanes read beams lane, lane + 32, ... of frame 2 and take a shuffle minimum (exact and
+// order-free, so it equals the host's serial loop); lane 0 picks the mode and writes.
+__global__ void __launch_bounds__(ORCA_THREADS) rlca_hybrid_kernel(int n, int beams, OrcaParams q, HybridParams h,
+                                                                    const float4 *__restrict__ pose,
+                                                                    const float4 *__restrict__ goal,
+                                                                    const int4 *__restrict__ meta,
+                                                                    const float *__restrict__ stack,
+                                                                    const int32_t *__restrict__ open,
+                                                                    float2 *__restrict__ action,
+                                                                    uint8_t *__restrict__ mode,
+                                                                    int32_t *__restrict__ counts)
+{
+    const int a = blockIdx.x * ORCA_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (a >= n) return;
+    const float *scan = stack + ((size_t)a * 3 + 2) * beams;
+    float m = INFINITY;
+    for (int k = lane; k < beams; k += 32) m = fminf(m, __ldg(scan + k));
+#pragma unroll
+    for (int o = 16; o; o >>= 1) m = fminf(m, __shfl_xor_sync(FULL_MASK, m, o));
+    if (lane == 0) hybrid_apply(hybrid_mode(m, h), pose, goal, meta, a, q, h, open, action, mode, counts);
+}
+
+static int hybrid_args(const rlca_env_config *cfg, const rlca_hybrid_params *p, OrcaParams &q, HybridParams &h)
+{
+    if (!cfg || !p) return rlca_set_err(RLCA_ERR_INVALID, "hybrid: cfg or params is NULL");
+    if (cfg->beams < 1) return rlca_set_err(RLCA_ERR_INVALID, "hybrid: cfg has no beams");
+    const float rm = cfg->range_max;
+    if (!(p->r_risk >= 0.0f && p->r_risk <= p->r_safe && p->r_safe <= rm && rm < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "hybrid: need 0 <= r_risk <= r_safe <= cfg.range_max, all finite");
+    if (!(p->heading_gain > 0.0f && p->heading_gain < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "hybrid: heading_gain must be finite and > 0");
+    int rc = noncoop_args(cfg, cfg->v_max, p->heading_gain, q);
+    if (rc) return rc;
+    if (!(p->v_safe > 0.0f && p->v_safe <= cfg->v_max))
+        return rlca_set_err(RLCA_ERR_INVALID, "hybrid: v_safe must be in (0, cfg.v_max]");
+    h.r_safe = p->r_safe;
+    h.r_risk = p->r_risk;
+    h.v_safe = p->v_safe;
+    h.range_max = rm;
+    return RLCA_OK;
+}
+
+extern "C" int rlca_hybrid_action(const rlca_env_config *cfg, const rlca_hybrid_params *params,
+                                  const rlca_env_state *state, const float *stack_dev, const int32_t *open_dev,
+                                  float *action_dev, uint8_t *mode_dev, int32_t *counts_dev, void *stream)
+{
+    OrcaParams q;
+    HybridParams h;
+    int rc = hybrid_args(cfg, params, q, h);
+    if (rc) return rc;
+    if (!state || !state->pose_dev || !state->goal_dev || !state->meta_dev || !stack_dev || !action_dev || !mode_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_hybrid_action: state, stack, action or mode buffer is NULL");
+    if (!open_dev != !counts_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_hybrid_action: open and counts must be both set or both NULL");
+    const int n = cfg->robots_per_world * cfg->num_worlds;
+    rlca_hybrid_kernel<<<(n + ORCA_WARPS - 1) / ORCA_WARPS, ORCA_THREADS, 0, (cudaStream_t)stream>>>(
+        n, cfg->beams, q, h, reinterpret_cast<const float4 *>(state->pose_dev),
+        reinterpret_cast<const float4 *>(state->goal_dev), reinterpret_cast<const int4 *>(state->meta_dev), stack_dev,
+        open_dev, reinterpret_cast<float2 *>(action_dev), mode_dev, counts_dev);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_hybrid_action_host(const rlca_env_config *cfg, const rlca_hybrid_params *params,
+                                       const float *stack_host, const float *pose_host, const float *goal_host,
+                                       const int32_t *meta_host, const int32_t *open_host, float *action_host,
+                                       uint8_t *mode_host, int32_t *counts_host)
+{
+    OrcaParams q;
+    HybridParams h;
+    int rc = hybrid_args(cfg, params, q, h);
+    if (rc) return rc;
+    if (!stack_host || !pose_host || !goal_host || !meta_host || !action_host || !mode_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_hybrid_action_host: a buffer is NULL");
+    if (!open_host != !counts_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_hybrid_action_host: open and counts must be both set or both NULL");
+    const float4 *pose = reinterpret_cast<const float4 *>(pose_host), *goal = reinterpret_cast<const float4 *>(goal_host);
+    const int4 *meta = reinterpret_cast<const int4 *>(meta_host);
+    const int n = cfg->robots_per_world * cfg->num_worlds, beams = cfg->beams;
+    for (int a = 0; a < n; ++a) {
+        const float *scan = stack_host + ((size_t)a * 3 + 2) * beams;
+        float m = INFINITY;
+        for (int k = 0; k < beams; ++k) m = fminf(m, scan[k]);
+        hybrid_apply(hybrid_mode(m, h), pose, goal, meta, a, q, h, open_host, reinterpret_cast<float2 *>(action_host),
+                     mode_host, counts_host);
     }
     return RLCA_OK;
 }

@@ -19,7 +19,7 @@ import torch
 
 from . import _lib
 from .model.ppo import generate_action_no_sampling
-from .orca import NhOrcaController, OrcaController
+from .orca import NhOrcaController, OrcaController, mode_shares
 
 COLUMNS = _lib.EVAL_PARTIALS
 NPARTIALS = len(COLUMNS)
@@ -169,7 +169,7 @@ def metrics(tot):
     return out
 
 
-def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None):
+def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
@@ -182,10 +182,18 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     With `non_cooperative` (an orca.NonCooperative on `env`) its robots drive straight to their goals instead: the
     override is applied to every tick's action before the circle rule, so they keep the same episode mechanics.  The
     result then also holds 'partials_split' (num_worlds, 2, NPARTIALS) and 'by_role' {'cooperative',
-    'non_cooperative'}: the metrics of each role; 'partials', 'totals' and 'metrics' still cover every robot."""
+    'non_cooperative'}: the metrics of each role; 'partials', 'totals' and 'metrics' still cover every robot.
+
+    With `hybrid` (an orca.Hybrid on `env`, policies only) the policy's action is switched per robot by its newest scan
+    before the non-cooperative override, so masked robots still get the driver's action.  The result then also holds
+    'mode_counts' (num_worlds, 3) int64, the ticks of tracked episodes each world's robots spent in each mode, and
+    'modes' (orca.mode_shares: the share of those agent-ticks per mode and 'agent_ticks'); with `non_cooperative`
+    both cover the cooperative robots only."""
     E = int(episodes)
     if int(check_every) < 1:
         raise ValueError('check_every must be >= 1')
+    if hybrid is not None and isinstance(policy, (OrcaController, NhOrcaController)):
+        raise ValueError('hybrid switches a policy; the ORCA baselines are not switched')
     tracker = EpisodeTracker(env, E)
     N, dev = env.N, env.device
     circle = int(env.cfg.auto_reset) == 0
@@ -195,6 +203,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     if env.sc.layout is not None:
         env.random_layout()
     tracker.reset()
+    if hybrid is not None:
+        hybrid.reset()
     obs = env.get_laser_observation()
     stacks = [obs[:, None, :].repeat(1, 3, 1).contiguous(), torch.empty(N, 3, env.beam_mum, device=dev)]
     terminal = torch.zeros(N, dtype=torch.bool, device=dev)
@@ -208,6 +218,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             _, scaled = generate_action_no_sampling(env=env, state_list=(stacks[k], env.get_local_goal(),
                                                                          env.get_self_speed()),
                                                     policy=policy, action_bound=ACTION_BOUND)
+            if hybrid is not None:
+                hybrid.apply(scaled, stacks[k], tracker)
         if non_cooperative is not None:
             non_cooperative.apply(scaled)
         if circle:
@@ -227,4 +239,7 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         out['partials_split'] = split
         out['by_role'] = {'cooperative': metrics(totals(split[:, 0])),
                           'non_cooperative': metrics(totals(split[:, 1]))}
+    if hybrid is not None:
+        out['mode_counts'] = hybrid.counts_per_world(None if non_cooperative is None else non_cooperative.mask)
+        out['modes'] = mode_shares(out['mode_counts'])
     return out

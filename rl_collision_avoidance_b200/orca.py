@@ -17,11 +17,15 @@ The controllers are csrc/rlca_orca.cu; `orca_host` / `nh_orca_host` run the same
 
     nc = NonCooperative(env, mask)         # DESIGN.md §9h: masked robots drive straight to their goals
     nc.apply(action)                       # overwrites the masked rows of any controller's or policy's action
+
+    hy = Hybrid(env)                       # DESIGN.md §9j: driver in free space, capped speed near obstacles
+    hy.apply(action, stack, tracker)       # switches a policy's action by the nearest return of its newest scan
 """
 from __future__ import annotations
 
 import argparse
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -304,6 +308,113 @@ def noncoop_host(cfg, pose, goal, meta, mask, action, speed=None, heading_gain=D
                                             float(cfg.v_max) if speed is None else float(speed), float(heading_gain),
                                             vp(act)))
     return act
+
+
+# starting values, not tuned ones (DESIGN.md §9j); heading_gain is the §9h driver's
+HYBRID_DEFAULTS = dict(r_safe=2.0, r_risk=0.8, v_safe=0.5, heading_gain=2.0)
+HYBRID_MODES = ('policy', 'driver', 'safe')      # mode 0, 1, 2
+
+
+def check_hybrid(range_max, v_max, r_safe, r_risk, v_safe, heading_gain):
+    """ValueError unless 0 <= r_risk <= r_safe <= range_max (all finite), 0 < v_safe <= v_max and heading_gain is
+    finite and > 0: the rule rlca_hybrid_action applies, checked before any device work."""
+    f = np.float32
+    r_safe, r_risk, v_safe, gain, rm = (f(x) for x in (r_safe, r_risk, v_safe, heading_gain, range_max))
+    if not (0.0 <= r_risk <= r_safe <= rm and math.isfinite(rm)):
+        raise ValueError('hybrid radii need 0 <= r_risk <= r_safe <= range_max (%g), got r_risk %g, r_safe %g'
+                         % (rm, r_risk, r_safe))
+    if not 0.0 < v_safe <= f(v_max):
+        raise ValueError('hybrid v_safe must be in (0, %g], got %g' % (f(v_max), v_safe))
+    if not (gain > 0.0 and math.isfinite(gain)):
+        raise ValueError('hybrid heading_gain must be finite and > 0, got %g' % gain)
+
+
+class Hybrid:
+    """The hybrid controller (rlca_hybrid_action, DESIGN.md §9j): per agent and tick, with d the nearest return of the
+    newest scan in metres, the §9h driver at v_max when d > r_safe (mode 1), the policy's action with v capped at
+    v_safe when d < r_risk (mode 2), the policy's action otherwise (mode 0).  Holds the per-agent mode counters (N, 3)
+    int32 on the env's device; they count the ticks of the episodes an EpisodeTracker follows."""
+
+    def __init__(self, env, r_safe=HYBRID_DEFAULTS['r_safe'], r_risk=HYBRID_DEFAULTS['r_risk'],
+                 v_safe=HYBRID_DEFAULTS['v_safe'], heading_gain=HYBRID_DEFAULTS['heading_gain']):
+        check_hybrid(env.cfg.range_max, env.cfg.v_max, r_safe, r_risk, v_safe, heading_gain)
+        self.env = env
+        self.params = _lib.HybridParams(r_safe, r_risk, v_safe, heading_gain)
+        self.counts = torch.zeros(env.N, len(HYBRID_MODES), dtype=torch.int32, device=env.device)
+        self.mode = torch.zeros(env.N, dtype=torch.uint8, device=env.device)
+
+    def reset(self):
+        """Zero the mode counters."""
+        self.counts.zero_()
+
+    def apply(self, action, stack, tracker=None):
+        """Rewrite `action` ((N, 2) float32, contiguous) in place from `stack` ((N, 3, beams) float32, the scan FIFO
+        the next tick reads) and the state the next tick reads, on the env's stream without synchronisation; with an
+        EpisodeTracker, count each agent's mode when its `open` flag is set.  `self.mode` holds the modes; returns
+        `action`."""
+        env = self.env
+        dev = self.counts.device
+        if action.shape != (env.N, 2) or action.dtype != torch.float32 or not action.is_contiguous() or \
+                action.device != dev:
+            raise ValueError(f'action must be a contiguous ({env.N}, 2) float32 tensor on {dev}')
+        if stack.shape != (env.N, 3, env.cfg.beams) or stack.dtype != torch.float32 or not stack.is_contiguous() or \
+                stack.device != dev:
+            raise ValueError(f'stack must be a contiguous ({env.N}, 3, {env.cfg.beams}) float32 tensor on {dev}')
+        st = env._state_struct(env._cur)
+        open_, counts = (tracker.open, self.counts) if tracker is not None else (None, None)
+        _lib.check(env.lib.rlca_hybrid_action(C.byref(env.cfg), C.byref(self.params), C.byref(st), _ptr(stack),
+                                              _ptr(open_), _ptr(action), _ptr(self.mode), _ptr(counts),
+                                              env._stream()))
+        return action
+
+    def counts_per_world(self, mask=None):
+        """(num_worlds, 3) int64 mode counts summed over each world's agents, over those with mask 0 when an agent
+        mask (N) is given (exact integers, so shards give the same rows)."""
+        c = self.counts.to(torch.int64)
+        if mask is not None:
+            keep = torch.as_tensor(mask, device=c.device) == 0
+            if keep.shape != (self.env.N,):
+                raise ValueError(f'mask must have ({self.env.N},) entries')
+            c = c * keep[:, None]
+        return c.view(self.env.num_worlds, -1, len(HYBRID_MODES)).sum(1).cpu().numpy()
+
+
+def mode_shares(mode_counts):
+    """{'policy', 'driver', 'safe': share of the counted agent-ticks (NaN when none), 'agent_ticks'} of (W, 3)
+    counts."""
+    tot = np.asarray(mode_counts, np.int64).reshape(-1, len(HYBRID_MODES)).sum(0)
+    n = int(tot.sum())
+    out = {name: (int(c) / n if n else math.nan) for name, c in zip(HYBRID_MODES, tot)}
+    out['agent_ticks'] = n
+    return out
+
+
+def hybrid_host(cfg, stack, pose, goal, meta, action, open_=None, counts=None, r_safe=HYBRID_DEFAULTS['r_safe'],
+                r_risk=HYBRID_DEFAULTS['r_risk'], v_safe=HYBRID_DEFAULTS['v_safe'],
+                heading_gain=HYBRID_DEFAULTS['heading_gain']):
+    """rlca_hybrid_action_host on numpy arrays (stack (N, 3, beams) float32, pose / goal / meta as orca_host): returns
+    (action (N, 2), mode (N) uint8, counts (N, 3) int32), copies of `action` and `counts` (zeros when None) rewritten;
+    counting happens only with `open_` (N)."""
+    lib = _lib.load()
+    n, beams = cfg.robots_per_world * cfg.num_worlds, cfg.beams
+    s = np.ascontiguousarray(stack, np.float32)
+    p = np.ascontiguousarray(pose, np.float32)
+    g = np.ascontiguousarray(goal, np.float32)
+    m = np.ascontiguousarray(meta, np.int32)
+    act = np.array(action, np.float32, order='C', copy=True)
+    cnt = np.zeros((n, len(HYBRID_MODES)), np.int32) if counts is None else np.array(counts, np.int32, order='C',
+                                                                                       copy=True)
+    opn = None if open_ is None else np.ascontiguousarray(open_, np.int32)
+    if s.shape != (n, 3, beams) or p.shape != (n, 4) or g.shape != (n, 4) or m.shape != (n, 4) or \
+            act.shape != (n, 2) or cnt.shape != (n, 3) or (opn is not None and opn.shape != (n,)):
+        raise ValueError(f'stack must be ({n}, 3, {beams}), pose, goal and meta ({n}, 4), action ({n}, 2), '
+                         f'open ({n},) and counts ({n}, 3)')
+    mode = np.zeros(n, np.uint8)
+    vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
+    prm = _lib.HybridParams(r_safe, r_risk, v_safe, heading_gain)
+    _lib.check(lib.rlca_hybrid_action_host(C.byref(cfg), C.byref(prm), vp(s), vp(p), vp(g), vp(m), vp(opn), vp(act),
+                                           vp(mode), vp(cnt if opn is not None else None)))
+    return act, mode, cnt
 
 
 def nh_orca_polygon(cfg, tracking_error=NH_DEFAULTS['tracking_error'], heading_time=NH_DEFAULTS['heading_time']):

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Time one rlca_orca_action launch (the ORCA-DD controller, DESIGN.md §9d) and one rlca_nh_orca_action launch (NH-ORCA,
-§9e), map-blind and map-aware (§9f), and one rlca_noncoop_action launch with every agent non-cooperative (§9h), with
-CUDA events over many launches, on states after random-action ticks: stage 1 at 171 x 24 agents and the 50-robot circle
-at 41 x 50.  The five rows alternate, each timed twice per size.
+§9e), map-blind and map-aware (§9f), one rlca_noncoop_action launch with every agent non-cooperative (§9h) and one
+rlca_hybrid_action launch with the default thresholds and counting on (§9j), with CUDA events over many launches, on
+states after random-action ticks: stage 1 at 171 x 24 agents and the 50-robot circle at 41 x 50.  The six rows
+alternate, each timed twice per size.
 
     python tools/time_orca.py [--launches 2000]
 """
@@ -17,7 +18,8 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET  # noqa: E402
-from rl_collision_avoidance_b200.orca import NhOrcaController, NonCooperative, OrcaController  # noqa: E402
+from rl_collision_avoidance_b200.evaluation import EpisodeTracker  # noqa: E402
+from rl_collision_avoidance_b200.orca import Hybrid, NhOrcaController, NonCooperative, OrcaController  # noqa: E402
 from rl_collision_avoidance_b200.stage_world import StageWorld  # noqa: E402
 
 
@@ -59,6 +61,24 @@ class NonCoop:
         return self._status
 
 
+class HybridCtl:
+    """rlca_hybrid_action (§9j) with the defaults, on a scan stack of three copies of the last scan, counting every
+    agent."""
+
+    def __init__(self, env):
+        self.hy = Hybrid(env)
+        self.stack = env.obs[:, None, :].repeat(1, 3, 1).contiguous()
+        self.tracker = EpisodeTracker(env, 1)
+        self.action = torch.zeros(env.N, 2, device=env.device)
+        self._status = torch.zeros(env.N, dtype=torch.int32, device=env.device)
+
+    def __call__(self):
+        return self.hy.apply(self.action, self.stack, self.tracker)
+
+    def status(self):
+        return self._status
+
+
 def OrcaMap(env):
     return OrcaController(env, obstacles=True)
 
@@ -78,7 +98,7 @@ def main():
     except (OSError, subprocess.CalledProcessError):
         power = 'unknown'
     rows = [time_one(scenario, worlds, args.launches, make) for scenario, worlds in (('stage1', 171), ('circle', 41))
-            for _ in range(2) for make in (OrcaController, OrcaMap, NhOrcaController, NhOrcaMap, NonCoop)]
+            for _ in range(2) for make in (OrcaController, OrcaMap, NhOrcaController, NhOrcaMap, NonCoop, HybridCtl)]
     print(json.dumps({'card': card, 'power_limit': power, 'launches': args.launches, 'rows': rows}))
 
 
