@@ -26,7 +26,6 @@ action otherwise, and prints the share of robot-ticks in each mode (DESIGN.md §
 """
 import argparse
 import json
-import math
 import os
 
 import torch
@@ -36,17 +35,13 @@ from rl_collision_avoidance_b200.model.net import CNNPolicy
 from rl_collision_avoidance_b200.orca import HYBRID_DEFAULTS, Hybrid, NonCooperative, \
     add_arguments as add_controller_arguments, check_arguments as check_controller_arguments, check_hybrid, \
     from_arguments as controller_from_arguments
-from rl_collision_avoidance_b200.scenarios import COMMON, RANDOM_DEFAULTS, make_scenario
+from rl_collision_avoidance_b200.scenarios import COMMON, add_random_arguments, check_random_arguments, make_scenario, \
+    random_max_ticks, random_scenario_from_arguments
 from rl_collision_avoidance_b200.stage_world import StageWorld
 
 LASER_BEAM = 512
 LASER_HIST = 3
 CIRCLE_MAX_TICKS = 1500          # 25 m radius: the 49.5 m to the goal radius take at least 495 ticks at v_max
-
-
-def random_max_ticks(side):
-    """3 x the ticks the square's diagonal takes at v_max: the default tick budget of a random scenario."""
-    return 3 * math.ceil(side * math.sqrt(2.0) / (COMMON['v_max'] * COMMON['dt']))
 
 
 def main(argv=None):
@@ -65,15 +60,7 @@ def main(argv=None):
                          '3 ceil(S sqrt(2) / (v_max dt)) on random' % CIRCLE_MAX_TICKS)
     ap.add_argument('--circle-robots', type=int, default=None, help='K robots on the circle (default: the 50-row table)')
     ap.add_argument('--circle-radius', type=float, default=None, help='circle radius in metres (default 25)')
-    ap.add_argument('--random-robots', type=int, default=None, metavar='K',
-                    help='random: robots per world, 2..64 (default %d)' % RANDOM_DEFAULTS['robots_per_world'])
-    ap.add_argument('--random-side', type=float, default=None, metavar='S',
-                    help='random: side of the square of starts and goals, m (default %g)' % RANDOM_DEFAULTS['side'])
-    ap.add_argument('--random-separation', type=float, default=None, metavar='D',
-                    help='random: least start-start and goal-goal distance, m (default %g)'
-                         % RANDOM_DEFAULTS['separation'])
-    ap.add_argument('--random-min-travel', type=float, default=None, metavar='L',
-                    help='random: least start-goal distance, m (default S / 2)')
+    add_random_arguments(ap)
     ap.add_argument('--check-every', type=int, default=50)
     ap.add_argument('--non-cooperative', type=int, default=None, metavar='K',
                     help='K robots per world (robots floor(j R / K), j < K) drive straight to their goals and ignore '
@@ -99,10 +86,7 @@ def main(argv=None):
         ap.error('--orca-map applies to --baseline orca / nh-orca only')
     if args.scenario != 'circle' and (args.circle_robots is not None or args.circle_radius is not None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
-    random_args = (args.random_robots, args.random_side, args.random_separation, args.random_min_travel)
-    if args.scenario != 'random' and any(a is not None for a in random_args):
-        ap.error('--random-robots / --random-side / --random-separation / --random-min-travel apply to '
-                 '--scenario random only')
+    check_random_arguments(ap, args)
     if args.non_cooperative is None and args.non_cooperative_speed is not None:
         ap.error('--non-cooperative-speed applies with --non-cooperative only')
     v_max = COMMON['v_max']
@@ -126,11 +110,7 @@ def main(argv=None):
     if args.scenario == 'circle':
         sc = make_scenario(args.scenario, robots_per_world=args.circle_robots, radius=args.circle_radius)
     elif args.scenario == 'random':
-        try:
-            sc = make_scenario('random', robots_per_world=args.random_robots, side=args.random_side,
-                               separation=args.random_separation, min_travel=args.random_min_travel)
-        except ValueError as e:
-            ap.error(str(e))
+        sc = random_scenario_from_arguments(ap, args)
     else:
         sc = make_scenario(args.scenario)
     if args.non_cooperative is not None and not 1 <= args.non_cooperative <= sc.robots_per_world:

@@ -650,6 +650,33 @@ int rlca_layout_random(const rlca_env_config *cfg, const rlca_layout_params *par
 int rlca_layout_random_host(const rlca_env_config *cfg, const rlca_layout_params *params, float *pose_host,
                             float *goal_host, float *acc_host, int32_t *status_host);
 
+/* Training on random layouts (DESIGN.md §9k): one launch after each rlca_env_step of an env with auto_reset 0, in place
+ * on the state that tick wrote, with that tick's flags.  Per world (global index cfg->world_offset + w):
+ *   - a latched robot (meta.w != 0) is parked: goal.zw (its last command) = 0 and live[a] = 0; every other robot gets
+ *     live[a] = 1.  Passed as the next tick's io->live_dev, a parked robot stands still.
+ *   - a world whose robots are all latched is re-laid at once: the draws of rlca_layout_random with episode
+ *     e = meta.y + 1 of robot 0 instead of 0, written as the tick's re-spawn writes a new episode (pose, goal.xy,
+ *     pre_distance, acc.zw = start, acc.x = 0, meta.x = 1, meta.y = e, meta.w = 0, stall flag and acc.y kept) with
+ *     goal.zw = 0, live = 1 and flags[a].w (was_reset) = 1.
+ *   - status_dev[w] = 0, or 1 + r when a re-layout could not place robot r; that world keeps its rows, parked.
+ * RLCA_ERR_INVALID for what rlca_layout_random rejects, cfg->auto_reset != 0, or a NULL buffer (meta included).
+ *   flags_dev (N) uchar4, live_dev (N) uint8, status_dev (num_worlds) int32. */
+int rlca_layout_respawn(const rlca_env_config *cfg, const rlca_layout_params *params, const rlca_env_state *state,
+                        uint8_t *flags_dev, uint8_t *live_dev, int32_t *status_dev, void *stream);
+/* The same from HOST buffers (pose, goal, acc (N,4) float; meta (N,4) int32; flags (N,4) uint8; live (N) uint8;
+ * status (num_worlds) int32) by the sequential loop of rlca_layout_random_host; the outputs equal the device's bit for
+ * bit. */
+int rlca_layout_respawn_host(const rlca_env_config *cfg, const rlca_layout_params *params, float *pose_host,
+                             float *goal_host, float *acc_host, int32_t *meta_host, uint8_t *flags_host,
+                             uint8_t *live_host, int32_t *status_host);
+/* For every agent with flags_dev[a].w set: stack_dev[a][0..2] = obs_dev[a] (three copies of the scan, (N,3,beams)
+ * float) and gs_dev[a] = gs_src_dev[a] ((N,4) float); every other row is untouched.  Run after rlca_env_observe on
+ * the state rlca_layout_respawn re-laid, so a re-laid agent's FIFO and goal | speed are those the tick writes after
+ * an in-tick re-spawn.  RLCA_ERR_INVALID for a NULL pointer, 3 * beams not a multiple of 4, or a buffer that is not
+ * 16-byte aligned. */
+int rlca_stack_refresh(const rlca_env_config *cfg, const uint8_t *flags_dev, const float *obs_dev,
+                       const float *gs_src_dev, float *stack_dev, float *gs_dev, void *stream);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

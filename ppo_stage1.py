@@ -4,6 +4,7 @@
 Same hyper-parameters, log files and checkpoint names; `mpiexec -np 24` is replaced by one process per GPU:
     python ppo_stage1.py --num-worlds 43                       # 1 GPU, 43 x 24 = 1032 robots
     torchrun --nproc-per-node 8 --master-addr 127.0.0.1 ppo_stage1.py --num-worlds 43
+Fine-tuning on random layouts (DESIGN.md §9k) runs through ppo_stage2.py --scenario random.
 """
 import argparse
 import logging
@@ -15,6 +16,9 @@ import torch
 
 from rl_collision_avoidance_b200.model.net import Adam, CNNPolicy
 from rl_collision_avoidance_b200.model.ppo import setup_ppo_log
+from rl_collision_avoidance_b200.scenarios import add_random_arguments, check_random_arguments, \
+    random_scenario_from_arguments
+from rl_collision_avoidance_b200.stage_world import StageWorld as RandomWorld
 from rl_collision_avoidance_b200.stage_world1 import StageWorld
 from rl_collision_avoidance_b200.trainer import run
 
@@ -51,7 +55,8 @@ def make_loggers():
     return logger, logger_cal
 
 
-def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, epoch=EPOCH, ckpt='stage1_2.pth'):
+def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, epoch=EPOCH, ckpt='stage1_2.pth',
+         argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument('--num-worlds', type=int, default=1, help='independent worlds per GPU (x %d robots each)' % num_env)
     ap.add_argument('--updates', type=int, default=None, help='stop after this many PPO updates')
@@ -59,9 +64,18 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     ap.add_argument('--policy-path', default='policy')
     ap.add_argument('--resume', default=None, help='checkpoint written by this trainer (e.g. policy/Stage1_40): restores the\n'
                     'weights and, from <file>.trainer, the Adam moments / step and the sampling counter')
-    ap.add_argument('--scenario', default=None, choices=[None, 'stage1', 'stage2', 'circle'],
-                    help='override the world (e.g. circle: BASELINE config 4 trains on circle.world)')
-    args = ap.parse_args()
+    ap.add_argument('--scenario', default=None, choices=[None, 'stage1', 'stage2', 'circle', 'random'],
+                    help='override the world (e.g. circle: BASELINE config 4 trains on circle.world; random: a new '
+                         'layout in a world whenever all its robots have ended their episodes, stage 2 only)')
+    add_random_arguments(ap, timeout=True)
+    args = ap.parse_args(argv)
+    check_random_arguments(ap, args)
+    sc = None
+    if args.scenario == 'random':
+        if stage != 2:
+            ap.error('--scenario random trains with ppo_stage2.py: its layouts are per world, and stage 1 re-spawns '
+                     'each robot on its own')
+        sc = random_scenario_from_arguments(ap, args)
     rank = int(os.environ.get('RANK', '0'))
     world_size = int(os.environ.get('WORLD_SIZE', '1'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))
@@ -76,8 +90,13 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     if args.scenario == 'circle':
         from rl_collision_avoidance_b200.circle_world import StageWorld as world_cls   # noqa: N813
         num_env = 50
-    env = world_cls(LASER_BEAM, index=0, num_env=num_env, num_worlds=args.num_worlds, device=device, seed=args.seed,
-                    auto_reset=1 if stage == 1 else 2, world_offset=rank * args.num_worlds)
+    if sc is not None:
+        env = RandomWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, device=device, seed=args.seed,
+                          auto_reset=0, world_offset=rank * args.num_worlds)
+        num_env = sc.robots_per_world
+    else:
+        env = world_cls(LASER_BEAM, index=0, num_env=num_env, num_worlds=args.num_worlds, device=device,
+                        seed=args.seed, auto_reset=1 if stage == 1 else 2, world_offset=rank * args.num_worlds)
     action_bound = [[0, -1], [1, 1]]
     policy = CNNPolicy(frames=LASER_HIST, action_space=2, device=device, seed=args.seed, max_batch=max(batch_size, env.N))
     policy.sample_seed = args.seed * 1000003 + rank              # every rank draws its own action noise

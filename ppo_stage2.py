@@ -1,7 +1,14 @@
 #!/usr/bin/env python
 """Stage-2 trainer (drop-in for /root/reference/ppo_stage2.py): testenv map + polygon obstacles, 44 robots per
 world, group-synchronous episodes, filtered idle transitions, BATCH_SIZE 512, EPOCH 4, drop_last.
-Curriculum: copy a stage-1 checkpoint to policy/stage2.pth (README.md:18 of the reference)."""
+Curriculum: copy a stage-1 checkpoint to policy/stage2.pth (README.md:18 of the reference).
+
+--scenario random fine-tunes on random layouts (DESIGN.md §9k): --random-robots K robots per world in a --random-side
+S m square on circle.world's map, a new layout in a world whenever all its robots have ended their episodes, episodes
+timing out after --random-timeout ticks (default 3 ceil(S sqrt(2) / (v_max dt)), 426 for the default 10 m square):
+    mkdir -p policy && cp tests/golden/checkpoints/stage2.pth policy/stage2.pth
+    python ppo_stage2.py --scenario random --random-robots 16 --num-worlds 256 --updates 100
+"""
 from ppo_stage1 import main
 from rl_collision_avoidance_b200.stage_world2 import StageWorld
 

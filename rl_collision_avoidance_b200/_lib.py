@@ -169,6 +169,11 @@ SYMBOLS = {
                                    _P]),
     'rlca_layout_random': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), C.POINTER(EnvState), _P, _P]),
     'rlca_layout_random_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), _P, _P, _P, _P]),
+    'rlca_layout_respawn': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), C.POINTER(EnvState), _P, _P, _P,
+                                      _P]),
+    'rlca_layout_respawn_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), _P, _P, _P, _P, _P, _P,
+                                           _P]),
+    'rlca_stack_refresh': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

@@ -1,4 +1,5 @@
-// rlca_layout.cu — random start / goal layouts for evaluation (sm_90a), C ABI in include/rlca.h, DESIGN.md §9i.
+// rlca_layout.cu — random start / goal layouts for evaluation and training (sm_90a), C ABI in include/rlca.h,
+// DESIGN.md §9i and §9k.
 //
 // rlca_layout_random writes a layout into an env state in place, once before an episode: for world w (global index
 // cfg.world_offset + w) and robots r = 0 .. R-1 in order, the start is the first try k < max_reject whose draw,
@@ -14,6 +15,12 @@
 // One warp per world, the world's placed starts and goals in shared memory: lane l evaluates try base + l and the
 // lowest accepting lane wins (ballot, shuffle) in rounds of 32 tries — the order of the host's sequential loop.  When
 // no try of the budget is accepted the world's rows are left untouched and status[w] = 1 + r.
+//
+// Training (§9k) runs two launches after each tick of an env with auto_reset 0: rlca_layout_respawn parks the robots
+// whose episode ended and re-lays a world whose robots have all ended theirs with the same sampler at episode
+// meta.y + 1 (so a re-layout never repeats an earlier layout's draws), and, after rlca_env_observe on the new state,
+// rlca_stack_refresh makes the re-laid robots' scan FIFOs three copies of their new scan, as the tick does after an
+// in-tick re-spawn.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
@@ -30,6 +37,7 @@ struct LayoutConsts {
     uint64_t seed;
     uint32_t agent0;         // global agent index of the world's robot 0
     float side, sep2, travel2;
+    uint32_t episode;        // Philox episode counter of the draws: 0 for rlca_layout_random, meta.y + 1 for a re-layout
 };
 
 // try k of robot r's start (purpose 3) or goal (purpose 4): uniform in the square, one rounding per coordinate
@@ -38,7 +46,7 @@ __host__ __device__ __forceinline__ void layout_draw(const LayoutConsts &c, uint
                                                      float &x, float &y)
 {
     float u[4];
-    dev_rand4(c.seed, c.agent0 + r, 0u, k, purpose, u);
+    dev_rand4(c.seed, c.agent0 + r, c.episode, k, purpose, u);
     x = (u[0] - 0.5f) * c.side;
     y = (u[1] - 0.5f) * c.side;
 }
@@ -46,7 +54,7 @@ __host__ __device__ __forceinline__ void layout_draw(const LayoutConsts &c, uint
 __host__ __device__ __forceinline__ float layout_heading(const LayoutConsts &c, uint32_t r)
 {
     float u[4];
-    dev_rand4(c.seed, c.agent0 + r, 0u, 0u, 5u, u);
+    dev_rand4(c.seed, c.agent0 + r, c.episode, 0u, 5u, u);
     return dev_normalize(u[0] * 6.28318548202514648438f);
 }
 
@@ -113,6 +121,49 @@ __device__ __forceinline__ bool warp_place(const LayoutConsts &c, const LayoutSm
     return false;
 }
 
+// The starts and goals of robots 0 .. R-1 of one world into s by the whole warp: true, or false with *status = 1 + r
+// when robot r found no accepted try (s then holds robots 0 .. r-1 only).  The loop of rlca_layout_random_kernel, which
+// keeps it inline: written through this function its SASS is scheduled differently, though it computes the same.
+__device__ __forceinline__ bool warp_layout(const LayoutConsts &c, LayoutSmem &s, int R, int max_reject, int lane,
+                                            int32_t *status)
+{
+    for (int r = 0; r < R; ++r) {
+        float x, y, gx, gy;
+        if (!warp_place(c, s, r, 3u, max_reject, lane, x, y)) {
+            if (lane == 0) *status = 1 + r;
+            return false;
+        }
+        if (lane == 0) { s.sx[r] = x; s.sy[r] = y; }
+        __syncwarp();
+        if (!warp_place(c, s, r, 4u, max_reject, lane, gx, gy)) {
+            if (lane == 0) *status = 1 + r;
+            return false;
+        }
+        if (lane == 0) { s.gx[r] = gx; s.gy[r] = gy; }
+        __syncwarp();
+    }
+    return true;
+}
+
+// The same by one thread, trying in order: the host twins' loop.
+inline int host_layout(const LayoutConsts &c, int R, int max_reject, float *sx, float *sy, float *gx, float *gy)
+{
+    for (int r = 0; r < R; ++r) {
+        int k = 0;
+        for (; k < max_reject; ++k) {
+            layout_draw(c, (uint32_t)r, (uint32_t)k, 3u, sx[r], sy[r]);
+            if (start_ok(c, sx, sy, r, sx[r], sy[r])) break;
+        }
+        if (k == max_reject) return 1 + r;
+        for (k = 0; k < max_reject; ++k) {
+            layout_draw(c, (uint32_t)r, (uint32_t)k, 4u, gx[r], gy[r]);
+            if (goal_ok(c, gx, gy, r, sx[r], sy[r], gx[r], gy[r])) break;
+        }
+        if (k == max_reject) return 1 + r;
+    }
+    return 0;
+}
+
 __global__ void __launch_bounds__(LAYOUT_THREADS)
 rlca_layout_random_kernel(int num_worlds, int R, int max_reject, int pre_distance_zero, int world_offset,
                           uint64_t seed, float side, float sep2, float travel2, float4 *__restrict__ pose,
@@ -123,7 +174,7 @@ rlca_layout_random_kernel(int num_worlds, int R, int max_reject, int pre_distanc
     const int w = blockIdx.x * LAYOUT_WARPS + wib;
     if (w >= num_worlds) return;                     // warp-uniform
     LayoutSmem &s = smem[wib];
-    const LayoutConsts c = { seed, (uint32_t)(world_offset + w) * (uint32_t)R, side, sep2, travel2 };
+    const LayoutConsts c = { seed, (uint32_t)(world_offset + w) * (uint32_t)R, side, sep2, travel2, 0u };
     for (int r = 0; r < R; ++r) {
         float x, y, gx, gy;
         if (!warp_place(c, s, r, 3u, max_reject, lane, x, y)) {
@@ -148,6 +199,83 @@ rlca_layout_random_kernel(int num_worlds, int R, int max_reject, int pre_distanc
     if (lane == 0) status[w] = 0;
 }
 
+// The records of one re-laid robot, as apply_spawn writes a spawn that starts episode e; its last command is zero.
+__host__ __device__ __forceinline__ void relayout_apply(int pre_distance_zero, float x, float y, float th, float gx,
+                                                        float gy, int e, float4 &pose, float4 &goal, float4 &acc,
+                                                        int4 &meta)
+{
+    layout_apply(pre_distance_zero, x, y, th, gx, gy, pose, goal, acc);
+    goal.z = 0.0f; goal.w = 0.0f;
+    acc.x = 0.0f;
+    meta.x = 1; meta.y = e; meta.w = 0;
+}
+
+// After a tick (auto_reset 0): park the latched robots (meta.w != 0) of every world and re-lay a world whose robots
+// are all latched with the sampler of rlca_layout_random_kernel at episode meta.y + 1.  One warp per world.
+__global__ void __launch_bounds__(LAYOUT_THREADS)
+rlca_layout_respawn_kernel(int num_worlds, int R, int max_reject, int pre_distance_zero, int world_offset,
+                           uint64_t seed, float side, float sep2, float travel2, float4 *__restrict__ pose,
+                           float4 *__restrict__ goal, float4 *__restrict__ acc, int4 *__restrict__ meta,
+                           uint8_t *__restrict__ flags, uint8_t *__restrict__ live, int32_t *__restrict__ status)
+{
+    __shared__ LayoutSmem smem[LAYOUT_WARPS];
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int w = blockIdx.x * LAYOUT_WARPS + wib;
+    if (w >= num_worlds) return;                     // warp-uniform
+    LayoutSmem &s = smem[wib];
+    const size_t i0 = (size_t)w * R;
+    // robots lane and lane + 32 (R <= 64)
+    const bool l0 = lane < R && meta[i0 + lane].w != 0;
+    const bool l1 = lane + 32 < R && meta[i0 + lane + 32].w != 0;
+    const int latched = __popc(__ballot_sync(0xffffffffu, l0)) + __popc(__ballot_sync(0xffffffffu, l1));
+    if (latched == R) {                              // warp-uniform
+        const int e = meta[i0].y + 1;
+        const LayoutConsts c = { seed, (uint32_t)(world_offset + w) * (uint32_t)R, side, sep2, travel2, (uint32_t)e };
+        if (warp_layout(c, s, R, max_reject, lane, status + w)) {
+            for (int r = lane; r < R; r += 32) {
+                const size_t i = i0 + r;
+                float4 p = pose[i], g = goal[i], a = acc[i];
+                int4 m = meta[i];
+                relayout_apply(pre_distance_zero, s.sx[r], s.sy[r], layout_heading(c, (uint32_t)r), s.gx[r], s.gy[r],
+                               e, p, g, a, m);
+                pose[i] = p; goal[i] = g; acc[i] = a; meta[i] = m;
+                flags[4 * i + 3] = 1;
+                live[i] = 1;
+            }
+            if (lane == 0) status[w] = 0;
+            return;
+        }
+    }
+    for (int r = lane; r < R; r += 32) {
+        const size_t i = i0 + r;
+        const bool parked = (r < 32 ? l0 : l1);
+        if (parked) {
+            float4 g = goal[i];
+            g.z = 0.0f; g.w = 0.0f;
+            goal[i] = g;
+        }
+        live[i] = parked ? 0 : 1;
+    }
+    if (lane == 0 && latched != R) status[w] = 0;    // a failed re-layout keeps the status warp_layout wrote
+}
+
+// The FIFO slot of a re-laid agent (flags.w set) becomes three copies of its scan, and its goal | speed row is
+// replaced.  One warp per agent, coalesced 16-byte copies.
+__global__ void __launch_bounds__(LAYOUT_THREADS)
+rlca_stack_refresh_kernel(int n, int scan4, const uint8_t *__restrict__ flags, const float4 *__restrict__ obs,
+                          const float4 *__restrict__ gs_src, float4 *__restrict__ stack, float4 *__restrict__ gs)
+{
+    const int a = blockIdx.x * LAYOUT_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (a >= n || flags[4 * (size_t)a + 3] == 0) return;          // warp-uniform
+    const float4 *src = obs + (size_t)a * scan4;
+    float4 *dst = stack + (size_t)a * 3 * scan4;
+    for (int c = lane; c < scan4; c += 32) {
+        const float4 v = src[c];
+        dst[c] = v; dst[scan4 + c] = v; dst[2 * scan4 + c] = v;
+    }
+    if (lane == 0) gs[a] = gs_src[a];
+}
+
 int check_layout(const rlca_env_config *cfg, const rlca_layout_params *params, const char *who)
 {
     if (!cfg || !params) return rlca_set_err(RLCA_ERR_INVALID, "%s: cfg or params is NULL", who);
@@ -169,10 +297,10 @@ int check_layout(const rlca_env_config *cfg, const rlca_layout_params *params, c
     return RLCA_OK;
 }
 
-LayoutConsts layout_consts(const rlca_env_config *cfg, const rlca_layout_params *params, int w)
+LayoutConsts layout_consts(const rlca_env_config *cfg, const rlca_layout_params *params, int w, uint32_t episode)
 {
     return { cfg->seed, (uint32_t)(cfg->world_offset + w) * (uint32_t)cfg->robots_per_world, params->side,
-             params->separation * params->separation, params->min_travel * params->min_travel };
+             params->separation * params->separation, params->min_travel * params->min_travel, episode };
 }
 
 }  // namespace
@@ -184,7 +312,7 @@ extern "C" int rlca_layout_random(const rlca_env_config *cfg, const rlca_layout_
     if (rc) return rc;
     if (!state || !state->pose_dev || !state->goal_dev || !state->acc_dev || !status_dev)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_layout_random: a state or status buffer is NULL");
-    const LayoutConsts c = layout_consts(cfg, params, 0);
+    const LayoutConsts c = layout_consts(cfg, params, 0, 0u);
     const int ctas = (cfg->num_worlds + LAYOUT_WARPS - 1) / LAYOUT_WARPS;
     rlca_layout_random_kernel<<<ctas, LAYOUT_THREADS, 0, (cudaStream_t)stream>>>(
         cfg->num_worlds, cfg->robots_per_world, cfg->max_reject, cfg->pre_distance_zero, cfg->world_offset, c.seed,
@@ -205,23 +333,10 @@ extern "C" int rlca_layout_random_host(const rlca_env_config *cfg, const rlca_la
     float4 *pose = reinterpret_cast<float4 *>(pose_host), *goal = reinterpret_cast<float4 *>(goal_host);
     float4 *acc = reinterpret_cast<float4 *>(acc_host);
     for (int w = 0; w < cfg->num_worlds; ++w) {
-        const LayoutConsts c = layout_consts(cfg, params, w);
+        const LayoutConsts c = layout_consts(cfg, params, w, 0u);
         float sx[RLCA_MAX_ROBOTS_PER_WORLD], sy[RLCA_MAX_ROBOTS_PER_WORLD];
         float gx[RLCA_MAX_ROBOTS_PER_WORLD], gy[RLCA_MAX_ROBOTS_PER_WORLD];
-        int failed = 0;
-        for (int r = 0; r < R && !failed; ++r) {
-            int k = 0;
-            for (; k < cfg->max_reject; ++k) {
-                layout_draw(c, (uint32_t)r, (uint32_t)k, 3u, sx[r], sy[r]);
-                if (start_ok(c, sx, sy, r, sx[r], sy[r])) break;
-            }
-            if (k == cfg->max_reject) { failed = 1 + r; break; }
-            for (k = 0; k < cfg->max_reject; ++k) {
-                layout_draw(c, (uint32_t)r, (uint32_t)k, 4u, gx[r], gy[r]);
-                if (goal_ok(c, gx, gy, r, sx[r], sy[r], gx[r], gy[r])) break;
-            }
-            if (k == cfg->max_reject) failed = 1 + r;
-        }
+        const int failed = host_layout(c, R, cfg->max_reject, sx, sy, gx, gy);
         status_host[w] = failed;
         if (failed) continue;
         for (int r = 0; r < R; ++r) {
@@ -230,5 +345,101 @@ extern "C" int rlca_layout_random_host(const rlca_env_config *cfg, const rlca_la
                          goal[i], acc[i]);
         }
     }
+    return RLCA_OK;
+}
+
+static int check_respawn(const rlca_env_config *cfg, const rlca_layout_params *params, const char *who)
+{
+    int rc = check_layout(cfg, params, who);
+    if (rc) return rc;
+    if (cfg->auto_reset != 0) return rlca_set_err(RLCA_ERR_INVALID, "%s: cfg.auto_reset must be 0", who);
+    return RLCA_OK;
+}
+
+extern "C" int rlca_layout_respawn(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                   const rlca_env_state *state, uint8_t *flags_dev, uint8_t *live_dev,
+                                   int32_t *status_dev, void *stream)
+{
+    int rc = check_respawn(cfg, params, "rlca_layout_respawn");
+    if (rc) return rc;
+    if (!state || !state->pose_dev || !state->goal_dev || !state->acc_dev || !state->meta_dev || !flags_dev ||
+        !live_dev || !status_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_layout_respawn: a state, flags, live or status buffer is NULL");
+    const LayoutConsts c = layout_consts(cfg, params, 0, 0u);
+    const int ctas = (cfg->num_worlds + LAYOUT_WARPS - 1) / LAYOUT_WARPS;
+    rlca_layout_respawn_kernel<<<ctas, LAYOUT_THREADS, 0, (cudaStream_t)stream>>>(
+        cfg->num_worlds, cfg->robots_per_world, cfg->max_reject, cfg->pre_distance_zero, cfg->world_offset, c.seed,
+        c.side, c.sep2, c.travel2, reinterpret_cast<float4 *>(state->pose_dev),
+        reinterpret_cast<float4 *>(state->goal_dev), reinterpret_cast<float4 *>(state->acc_dev),
+        reinterpret_cast<int4 *>(state->meta_dev), flags_dev, live_dev, status_dev);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_layout_respawn_host(const rlca_env_config *cfg, const rlca_layout_params *params, float *pose_host,
+                                        float *goal_host, float *acc_host, int32_t *meta_host, uint8_t *flags_host,
+                                        uint8_t *live_host, int32_t *status_host)
+{
+    int rc = check_respawn(cfg, params, "rlca_layout_respawn_host");
+    if (rc) return rc;
+    if (!pose_host || !goal_host || !acc_host || !meta_host || !flags_host || !live_host || !status_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_layout_respawn_host: a buffer is NULL");
+    const int R = cfg->robots_per_world;
+    float4 *pose = reinterpret_cast<float4 *>(pose_host), *goal = reinterpret_cast<float4 *>(goal_host);
+    float4 *acc = reinterpret_cast<float4 *>(acc_host);
+    int4 *meta = reinterpret_cast<int4 *>(meta_host);
+    for (int w = 0; w < cfg->num_worlds; ++w) {
+        const size_t i0 = (size_t)w * R;
+        int latched = 0;
+        for (int r = 0; r < R; ++r) latched += meta[i0 + r].w != 0;
+        int failed = 0;
+        if (latched == R) {
+            const int e = meta[i0].y + 1;
+            const LayoutConsts c = layout_consts(cfg, params, w, (uint32_t)e);
+            float sx[RLCA_MAX_ROBOTS_PER_WORLD], sy[RLCA_MAX_ROBOTS_PER_WORLD];
+            float gx[RLCA_MAX_ROBOTS_PER_WORLD], gy[RLCA_MAX_ROBOTS_PER_WORLD];
+            failed = host_layout(c, R, cfg->max_reject, sx, sy, gx, gy);
+            if (!failed) {
+                for (int r = 0; r < R; ++r) {
+                    const size_t i = i0 + r;
+                    relayout_apply(cfg->pre_distance_zero, sx[r], sy[r], layout_heading(c, (uint32_t)r), gx[r], gy[r],
+                                   e, pose[i], goal[i], acc[i], meta[i]);
+                    flags_host[4 * i + 3] = 1;
+                    live_host[i] = 1;
+                }
+                status_host[w] = 0;
+                continue;
+            }
+        }
+        for (int r = 0; r < R; ++r) {
+            const size_t i = i0 + r;
+            const bool parked = meta[i].w != 0;
+            if (parked) { goal[i].z = 0.0f; goal[i].w = 0.0f; }
+            live_host[i] = parked ? 0 : 1;
+        }
+        status_host[w] = failed;
+    }
+    return RLCA_OK;
+}
+
+extern "C" int rlca_stack_refresh(const rlca_env_config *cfg, const uint8_t *flags_dev, const float *obs_dev,
+                                  const float *gs_src_dev, float *stack_dev, float *gs_dev, void *stream)
+{
+    if (!cfg) return rlca_set_err(RLCA_ERR_INVALID, "rlca_stack_refresh: cfg is NULL");
+    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_stack_refresh: cfg has no robots");
+    if (cfg->beams < 1 || (3 * cfg->beams) % 4 != 0)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_stack_refresh: 3 * beams must be a multiple of 4");
+    if (!flags_dev || !obs_dev || !gs_src_dev || !stack_dev || !gs_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_stack_refresh: a buffer is NULL");
+    if (((uintptr_t)obs_dev | (uintptr_t)gs_src_dev | (uintptr_t)stack_dev | (uintptr_t)gs_dev) & 15)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_stack_refresh: misaligned buffer");
+    const int n = cfg->robots_per_world * cfg->num_worlds;
+    const int ctas = (n + LAYOUT_WARPS - 1) / LAYOUT_WARPS;
+    rlca_stack_refresh_kernel<<<ctas, LAYOUT_THREADS, 0, (cudaStream_t)stream>>>(
+        n, cfg->beams / 4, flags_dev, reinterpret_cast<const float4 *>(obs_dev),
+        reinterpret_cast<const float4 *>(gs_src_dev), reinterpret_cast<float4 *>(stack_dev),
+        reinterpret_cast<float4 *>(gs_dev));
+    RLCA_CUDA_TRY(cudaGetLastError());
     return RLCA_OK;
 }

@@ -8,6 +8,7 @@ tools/build_assets.py).  SURVEY.md Appendix B lists every constant.
 """
 from __future__ import annotations
 
+import dataclasses
 import json
 import math
 import os
@@ -168,20 +169,95 @@ def random_layout_host(cfg, layout: Layout, pose, goal, acc):
     return pose, goal, acc, status
 
 
+def relayout_host(cfg, layout: Layout, pose, goal, acc, meta, flags):
+    """rlca_layout_respawn_host (DESIGN.md §9k): the parking and re-layout after a tick of an env with auto_reset 0,
+    written into copies of the host arrays pose, goal, acc (N, 4) float32, meta (N, 4) int32 and flags (N, 4) uint8.
+    Returns (pose, goal, acc, meta, flags, live (N,) uint8, status (num_worlds,) int32)."""
+    import ctypes as C
+    from . import _lib
+    lib = _lib.load()
+    pose, goal, acc = (np.array(a, np.float32, order='C', copy=True) for a in (pose, goal, acc))
+    meta = np.array(meta, np.int32, order='C', copy=True)
+    flags = np.array(flags, np.uint8, order='C', copy=True)
+    n = int(cfg.robots_per_world) * int(cfg.num_worlds)
+    if any(a.shape != (n, 4) for a in (pose, goal, acc, meta, flags)):
+        raise ValueError(f'pose, goal, acc, meta and flags must be ({n}, 4)')
+    live = np.full(n, 0xFF, np.uint8)
+    status = np.full(int(cfg.num_worlds), -1, np.int32)
+    params = _lib.LayoutParams(layout.side, layout.separation, layout.min_travel)
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    _lib.check(lib.rlca_layout_respawn_host(C.byref(cfg), C.byref(params), vp(pose), vp(goal), vp(acc), vp(meta),
+                                            vp(flags), vp(live), vp(status)))
+    return pose, goal, acc, meta, flags, live, status
+
+
+def random_max_ticks(side):
+    """3 x the ticks the square's diagonal takes at v_max: the default tick budget of a random scenario, for an
+    evaluation run and for a training episode alike."""
+    return 3 * math.ceil(side * math.sqrt(2.0) / (COMMON['v_max'] * COMMON['dt']))
+
+
+RANDOM_FLAGS = ('--random-robots', '--random-side', '--random-separation', '--random-min-travel')
+
+
+def add_random_arguments(ap, timeout=False):
+    """The --random-* flags of a random scenario on an argparse parser; `timeout` adds --random-timeout (training)."""
+    ap.add_argument('--random-robots', type=int, default=None, metavar='K',
+                    help='random: robots per world, 2..64 (default %d)' % RANDOM_DEFAULTS['robots_per_world'])
+    ap.add_argument('--random-side', type=float, default=None, metavar='S',
+                    help='random: side of the square of starts and goals, m (default %g)' % RANDOM_DEFAULTS['side'])
+    ap.add_argument('--random-separation', type=float, default=None, metavar='D',
+                    help='random: least start-start and goal-goal distance, m (default %g)'
+                         % RANDOM_DEFAULTS['separation'])
+    ap.add_argument('--random-min-travel', type=float, default=None, metavar='L',
+                    help='random: least start-goal distance, m (default S / 2)')
+    if timeout:
+        ap.add_argument('--random-timeout', type=int, default=None, metavar='T',
+                        help='random: ticks after which an episode times out (default 3 ceil(S sqrt(2) / (v_max dt)), '
+                             '%d for the default square)' % random_max_ticks(RANDOM_DEFAULTS['side']))
+
+
+def check_random_arguments(ap, args):
+    """ap.error when a --random-* flag is given without --scenario random."""
+    flags = RANDOM_FLAGS + (('--random-timeout',) if hasattr(args, 'random_timeout') else ())
+    given = [getattr(args, f[2:].replace('-', '_')) for f in flags]
+    if args.scenario != 'random' and any(a is not None for a in given):
+        ap.error('%s apply to --scenario random only' % ' / '.join(flags))
+
+
+def random_scenario_from_arguments(ap, args):
+    """The random Scenario the --random-* flags describe; ap.error for values make_scenario rejects and for a
+    --random-timeout below 1.  With --random-timeout defined (a trainer) and not given, the timeout is
+    random_max_ticks(side); without it (evaluate.py) the scenario keeps make_scenario's default."""
+    timeout = getattr(args, 'random_timeout', None)
+    if timeout is not None and timeout < 1:
+        ap.error('--random-timeout must be >= 1, got %d' % timeout)
+    try:
+        sc = make_scenario('random', robots_per_world=args.random_robots, side=args.random_side,
+                           separation=args.random_separation, min_travel=args.random_min_travel, timeout=timeout)
+    except ValueError as e:
+        ap.error(str(e))
+    if hasattr(args, 'random_timeout') and timeout is None:
+        sc = dataclasses.replace(sc, timeout=random_max_ticks(sc.layout.side))
+    return sc
+
+
 def make_scenario(name: str, map_: WorldMap | None = None, robots_per_world: int | None = None,
                   radius: float | None = None, *, side: float | None = None, separation: float | None = None,
-                  min_travel: float | None = None) -> Scenario:
+                  min_travel: float | None = None, timeout: int | None = None) -> Scenario:
     """`robots_per_world` and `radius` shape the circle scenario (see circle_layout); both None, or 50 robots with no
     radius, keep the shipped 50-row table of the reference's circle.world.
 
     'random' (DESIGN.md §9i): `robots_per_world` robots (default 8) on circle.world's map with the circle's tick
     constants, whose starts and goals every world draws itself (StageWorld.random_layout) in a `side` m square (default
     10), starts and goals at least `separation` m apart (default 1), each goal at least `min_travel` m from its start
-    (default side / 2).  The tables are zero; ValueError for parameters rlca_layout_random rejects or a square that
-    leaves the map's free cells."""
+    (default side / 2).  `timeout` is the tick budget of an episode (default 10000, the circle's; a training run
+    passes random_max_ticks(side)).  The tables are zero; ValueError for parameters rlca_layout_random rejects or a
+    square that leaves the map's free cells."""
     name = name.lower()
-    if name != 'random' and (side is not None or separation is not None or min_travel is not None):
-        raise ValueError('side, separation and min_travel shape the random scenario only')
+    if name != 'random' and (side is not None or separation is not None or min_travel is not None or
+                             timeout is not None):
+        raise ValueError('side, separation, min_travel and timeout shape the random scenario only')
     if name == 'random':
         if radius is not None:
             raise ValueError('radius shapes the circle scenario only')
@@ -192,7 +268,10 @@ def make_scenario(name: str, map_: WorldMap | None = None, robots_per_world: int
         lay = random_layout_params(m, K, S, D, 0.5 * float(S) if min_travel is None else min_travel)
         K = int(K)
         zero = np.zeros((K, 4), np.float32)
-        return Scenario('random', 2, K, 10000, 0.7, 1, m, zero, zero.copy(), layout=lay)
+        if timeout is not None and not (int(timeout) == timeout and 1 <= timeout < 2 ** 31):
+            raise ValueError(f'random: timeout must be an integer >= 1, got {timeout}')
+        T = 10000 if timeout is None else int(timeout)
+        return Scenario('random', 2, K, T, 0.7, 1, m, zero, zero.copy(), layout=lay)
     if name == 'stage1':
         m = map_ or load_map(os.path.join(ASSETS, 'stage1_map.npz'))
         R = robots_per_world or 24

@@ -86,6 +86,12 @@ class StageWorld:
         self._host = None
         self._host_ptrs = None
         self._ticked = False
+        if self.sc.layout is not None:
+            # training on random layouts (relayout_finished): the next tick's live mask and the per-world status
+            self.live = torch.ones(N, dtype=torch.uint8, device=dev)
+            self._relayout_status = torch.zeros(self.num_worlds, dtype=torch.int32, device=dev)
+            self._layout_params = _lib.LayoutParams(self.sc.layout.side, self.sc.layout.separation,
+                                                    self.sc.layout.min_travel)
         self.reset_world()
 
     # ------------------------------------------------------------------ plumbing
@@ -193,11 +199,41 @@ class StageWorld:
         _lib.check(self.lib.rlca_layout_random(C.byref(self.cfg), C.byref(params), C.byref(st), _ptr(status),
                                                self._stream()))
         self._observe()
+        self.live.fill_(1)
+        self._relayout_status.zero_()
+        self._raise_layout_status(status)
+
+    def _raise_layout_status(self, status):
         bad = torch.nonzero(status).flatten().cpu()
         if len(bad):
             w = int(bad[0])
             raise ValueError(f'world {int(self.cfg.world_offset) + w}: robot {int(status[w]) - 1} not placed in '
                              f'{int(self.cfg.max_reject)} tries; lower the density')
+
+    def relayout_finished(self, stack_out, out=None):
+        """After a tick of a random scenario with auto_reset 0 (DESIGN.md §9k), on the env's stream with no
+        synchronisation: park the robots whose episode ended (last command 0, `live` 0), give every world whose robots
+        have all ended a new layout (rlca_layout_respawn), scan the new state (rlca_env_observe into the env's own obs /
+        gs), and make the re-laid robots' rows of stack_out (N, 3, beams) three copies of the new scan and their
+        out['gs'] rows the new local goal and speed (rlca_stack_refresh).  `out` holds the 'flags' and 'gs' buffers the
+        tick wrote (default the env's own); re-laid robots get flags[:, 3] (was_reset) = 1.  Pass `live` to the next
+        control_vel; check_relayout() reads the status."""
+        if self.sc.layout is None:
+            raise ValueError(f'scenario {self.sc.name} has no random layout')
+        o = out or {}
+        flags, gs = o.get('flags', self.flags), o.get('gs', self.gs)
+        st = self._state_struct(self._cur)
+        stream = self._stream()
+        _lib.check(self.lib.rlca_layout_respawn(C.byref(self.cfg), C.byref(self._layout_params), C.byref(st),
+                                                _ptr(flags), _ptr(self.live), _ptr(self._relayout_status), stream))
+        self._observe()
+        _lib.check(self.lib.rlca_stack_refresh(C.byref(self.cfg), _ptr(flags), _ptr(self.obs), _ptr(self.gs),
+                                               _ptr(stack_out), _ptr(gs), stream))
+
+    def check_relayout(self):
+        """One synchronisation: ValueError naming the first world a re-layout could not fill, in random_layout()'s
+        wording."""
+        self._raise_layout_status(self._relayout_status)
 
     def control_pose(self, pose, mask=None):
         """cmd_pose (stage_world1.py:237-249 -> stageros.cpp:282-296): teleport the masked agents (all when None) to

@@ -37,13 +37,22 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
         process_group=None, rank=0, save_every=20, generator=None, start_update=0):
     """hp: dict with HORIZON, GAMMA, LAMDA, BATCH_SIZE, EPOCH, COEFF_ENTROPY, CLIP_VALUE, NUM_ENV, OBS_SIZE, ACT_SIZE,
     LASER_HIST, MAX_EPISODES.  `start_update` continues the checkpoint numbering of a resumed run.
+    A random scenario (env.sc.layout, DESIGN.md §9k) trains with stage 2's update on per-world layouts: the env runs
+    with auto_reset 0, every tick passes env.live and is followed by env.relayout_finished, and a world whose robots
+    have all ended their episodes gets a new layout.
     Returns per-update stats (for tests / benchmarks)."""
+    relayout = env.sc.layout is not None
+    if relayout and (stage != 2 or int(env.cfg.auto_reset) != 0):
+        raise ValueError('a random scenario trains with stage 2 and auto_reset 0 (per-world re-layouts), got stage %d '
+                         'and auto_reset %d' % (stage, int(env.cfg.auto_reset)))
     H, N = hp['HORIZON'], env.N
     dev = env.device
     ro = Rollout(H, N, env.beam_mum, dev)
     env.reset_world()                                   # ppo_stage1.py:46-47
     env.reset_pose()                                    # :50
     env.generate_goal_point()                           # :52
+    if relayout:
+        env.random_layout()                             # the first layout, as evaluate() draws it
     obs = env.get_laser_observation()
     ro.stacks[0] = obs[:, None, :]                      # deque([obs, obs, obs]) (:60)
     ro.gs[0] = env.gs
@@ -57,8 +66,11 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
             generate_action(env=env, state_list=(ro.stacks[t], ro.gs[t]), policy=policy, action_bound=action_bound,
                             out={'value': ro.values[t], 'action': ro.actions[t], 'logprob': ro.logprobs[t],
                                  'scaled': ro.scaled})
-            env.control_vel(ro.scaled, stack_in=ro.stacks[t], stack_out=ro.stacks[t + 1],
+            env.control_vel(ro.scaled, live=env.live if relayout else None, stack_in=ro.stacks[t],
+                            stack_out=ro.stacks[t + 1],
                             out={'reward': ro.rewards[t], 'flags': ro.flags[t], 'gs': ro.gs[t + 1], 'eplog': ro.eplog[t]})
+            if relayout:
+                env.relayout_finished(ro.stacks[t + 1], out={'gs': ro.gs[t + 1], 'flags': ro.flags[t]})
         # last_v from the state after the horizon (ppo_stage1.py:94-97)
         last_v, _ = policy.forward_values(ro.stacks[H], ro.gs[H])
         dones = ro.flags[:, :, 0]
@@ -66,6 +78,8 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
                                                   last_value=last_v, dones=dones, lam=hp['LAMDA'])
         torch.cuda.synchronize(dev)
         t1 = time.perf_counter()
+        if relayout:
+            env.check_relayout()
         memory = (ro.stacks[:H], ro.gs[:H, :, 0:2], ro.gs[:H, :, 2:4], ro.actions, ro.logprobs, t_batch, ro.values,
                   ro.rewards, advs_batch)
         common = dict(policy=policy, optimizer=optimizer, batch_size=hp['BATCH_SIZE'], memory=memory, epoch=hp['EPOCH'],
