@@ -4,7 +4,8 @@
 Same hyper-parameters, log files and checkpoint names; `mpiexec -np 24` is replaced by one process per GPU:
     python ppo_stage1.py --num-worlds 43                       # 1 GPU, 43 x 24 = 1032 robots
     torchrun --nproc-per-node 8 --master-addr 127.0.0.1 ppo_stage1.py --num-worlds 43
-Fine-tuning on random layouts (DESIGN.md §9k) runs through ppo_stage2.py --scenario random.
+Fine-tuning on random layouts (DESIGN.md §9k) runs through ppo_stage2.py --scenario random, and on a mix of scenarios
+(DESIGN.md §9l) through ppo_stage2.py --mix.
 """
 import argparse
 import logging
@@ -14,6 +15,7 @@ import sys
 
 import torch
 
+from rl_collision_avoidance_b200.mix import MIX_AUTO_RESET, parse_mix, plan
 from rl_collision_avoidance_b200.model.net import Adam, CNNPolicy
 from rl_collision_avoidance_b200.model.ppo import setup_ppo_log
 from rl_collision_avoidance_b200.scenarios import add_random_arguments, check_random_arguments, \
@@ -55,10 +57,42 @@ def make_loggers():
     return logger, logger_cal
 
 
+def mix_components(mix, sc, rank):
+    """The Components of a parsed --mix on GPU `rank`: stage 2's 44 robots per world, the shipped circle's 50 and the
+    random scenario `sc`'s K (sc is None without a random component)."""
+    robots = {'stage2': 44, 'circle': 50, 'random': sc.robots_per_world if sc is not None else None}
+    return plan(mix, robots, rank)
+
+
+def make_component_env(c, sc, device, seed):
+    """The env handle of mix component `c`, built as a single-scenario run of that scenario builds it."""
+    kw = dict(num_worlds=c.worlds, device=device, seed=seed, auto_reset=MIX_AUTO_RESET[c.name],
+              world_offset=c.world_offset)
+    if c.name == 'stage2':
+        from rl_collision_avoidance_b200.stage_world2 import StageWorld as Stage2World
+        return Stage2World(LASER_BEAM, index=0, num_env=c.robots_per_world, **kw)
+    if c.name == 'circle':
+        from rl_collision_avoidance_b200.circle_world import StageWorld as CircleWorld
+        return CircleWorld(LASER_BEAM, index=0, num_env=c.robots_per_world, **kw)
+    return RandomWorld(LASER_BEAM, index=0, scenario=sc, **kw)
+
+
+def component_summary(c, stats):
+    """One line per mix component over every update of the run: episodes, successes, crashes, mean episode reward."""
+    rows = [s['by_scenario'][c.name] for s in stats]
+    n = sum(r['episodes'] for r in rows)
+    count = lambda key: sum(round(r[key] * r['episodes']) for r in rows if r['episodes'])
+    reward = sum(r['mean_ep_reward'] * r['episodes'] for r in rows if r['episodes'])
+    return ('  %s: %d worlds x %d robots, columns [%d, %d): %d episodes, %d reached the goal, %d crashed, '
+            'mean ep reward %.2f' % (c.name, c.worlds, c.robots_per_world, c.cols[0], c.cols[1], n,
+                                     count('success_rate'), count('crash_rate'), reward / n if n else float('nan')))
+
+
 def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, epoch=EPOCH, ckpt='stage1_2.pth',
          argv=None):
     ap = argparse.ArgumentParser()
-    ap.add_argument('--num-worlds', type=int, default=1, help='independent worlds per GPU (x %d robots each)' % num_env)
+    ap.add_argument('--num-worlds', type=int, default=None,
+                    help='independent worlds per GPU (x %d robots each; default 1)' % num_env)
     ap.add_argument('--updates', type=int, default=None, help='stop after this many PPO updates')
     ap.add_argument('--seed', type=int, default=0)
     ap.add_argument('--policy-path', default='policy')
@@ -67,11 +101,27 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     ap.add_argument('--scenario', default=None, choices=[None, 'stage1', 'stage2', 'circle', 'random'],
                     help='override the world (e.g. circle: BASELINE config 4 trains on circle.world; random: a new '
                          'layout in a world whenever all its robots have ended their episodes, stage 2 only)')
+    ap.add_argument('--mix', default=None, metavar='NAME:W,...',
+                    help='train on several scenarios in one run (stage 2 only; DESIGN.md §9l): world counts per GPU of '
+                         'stage2, circle and random, e.g. stage2:31,random:128,circle:14')
     add_random_arguments(ap, timeout=True)
     args = ap.parse_args(argv)
-    check_random_arguments(ap, args)
+    mix = None
+    if args.mix is not None:
+        if stage != 2:
+            ap.error('--mix trains with ppo_stage2.py: every component trains with stage 2\'s update')
+        if args.scenario is not None or args.num_worlds is not None:
+            ap.error('--mix gives the scenarios and their world counts: drop --scenario and --num-worlds')
+        try:
+            mix = parse_mix(args.mix)
+        except ValueError as e:
+            ap.error(str(e))
+    if args.num_worlds is None:
+        args.num_worlds = 1
+    random_in_mix = mix is not None and any(name == 'random' for name, _ in mix)
+    check_random_arguments(ap, args, random_component=random_in_mix)
     sc = None
-    if args.scenario == 'random':
+    if args.scenario == 'random' or random_in_mix:
         if stage != 2:
             ap.error('--scenario random trains with ppo_stage2.py: its layouts are per world, and stage 1 re-spawns '
                      'each robot on its own')
@@ -90,7 +140,11 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     if args.scenario == 'circle':
         from rl_collision_avoidance_b200.circle_world import StageWorld as world_cls   # noqa: N813
         num_env = 50
-    if sc is not None:
+    comps = None
+    if mix is not None:
+        comps = mix_components(mix, sc, rank)
+        env = [make_component_env(c, sc, device, args.seed) for c in comps]
+    elif sc is not None:
         env = RandomWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, device=device, seed=args.seed,
                           auto_reset=0, world_offset=rank * args.num_worlds)
         num_env = sc.robots_per_world
@@ -98,7 +152,8 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
         env = world_cls(LASER_BEAM, index=0, num_env=num_env, num_worlds=args.num_worlds, device=device,
                         seed=args.seed, auto_reset=1 if stage == 1 else 2, world_offset=rank * args.num_worlds)
     action_bound = [[0, -1], [1, 1]]
-    policy = CNNPolicy(frames=LASER_HIST, action_space=2, device=device, seed=args.seed, max_batch=max(batch_size, env.N))
+    n_agents = sum(e.N for e in env) if comps is not None else env.N
+    policy = CNNPolicy(frames=LASER_HIST, action_space=2, device=device, seed=args.seed, max_batch=max(batch_size, n_agents))
     policy.sample_seed = args.seed * 1000003 + rank              # every rank draws its own action noise
     opt = Adam(policy.parameters(), lr=LEARNING_RATE)
     if world_size > 1 and os.environ.get('RLCA_DP_PEER', '1') == '1':
@@ -145,6 +200,8 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
             s = stats[-1]
             print('update %d: rollout %.3fs update %.3fs -> %.0f agent-steps/s per GPU; mean ep reward %.2f' %
                   (s['update'], s['rollout_s'], s['update_s'], s['agent_steps_per_s'], s['mean_ep_reward']))
+            for c in comps or ():
+                print(component_summary(c, stats))
     except KeyboardInterrupt:
         pass
     finally:

@@ -8,6 +8,10 @@ S m square on circle.world's map, a new layout in a world whenever all its robot
 timing out after --random-timeout ticks (default 3 ceil(S sqrt(2) / (v_max dt)), 426 for the default 10 m square):
     mkdir -p policy && cp tests/golden/checkpoints/stage2.pth policy/stage2.pth
     python ppo_stage2.py --scenario random --random-robots 16 --num-worlds 256 --updates 100
+
+--mix trains on several scenarios in one run (DESIGN.md §9l): stage 2, the circle and random layouts side by side,
+world counts per GPU, every PPO update over all of them (the --random-* flags shape the random component):
+    python ppo_stage2.py --mix stage2:31,random:128,circle:14 --random-robots 16 --updates 100
 """
 from ppo_stage1 import main
 from rl_collision_avoidance_b200.stage_world2 import StageWorld

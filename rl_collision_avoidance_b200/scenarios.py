@@ -217,11 +217,14 @@ def add_random_arguments(ap, timeout=False):
                              '%d for the default square)' % random_max_ticks(RANDOM_DEFAULTS['side']))
 
 
-def check_random_arguments(ap, args):
-    """ap.error when a --random-* flag is given without --scenario random."""
+def check_random_arguments(ap, args, random_component=False):
+    """ap.error when a --random-* flag is given without --scenario random.  `random_component`: a trainer's --mix
+    holds a random component, which counts like --scenario random."""
     flags = RANDOM_FLAGS + (('--random-timeout',) if hasattr(args, 'random_timeout') else ())
     given = [getattr(args, f[2:].replace('-', '_')) for f in flags]
-    if args.scenario != 'random' and any(a is not None for a in given):
+    if args.scenario != 'random' and not random_component and any(a is not None for a in given):
+        if getattr(args, 'mix', None) is not None:
+            ap.error('%s apply to --scenario random or a random component of --mix only' % ' / '.join(flags))
         ap.error('%s apply to --scenario random only' % ' / '.join(flags))
 
 

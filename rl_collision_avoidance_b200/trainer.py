@@ -4,6 +4,7 @@
 One process per GPU.  Per tick: policy forward + sampling (librlca.so) -> fused env tick (librlca.so) with
 every output written straight into the rollout buffers; every HORIZON ticks: GAE, PPO update with an NCCL
 all-reduce of the flat gradient per optimizer step when launched under torchrun.  No mpi4py, no ROS.
+A stage-2 run may tick several env handles, one per scenario, on column slices of one rollout (DESIGN.md §9l).
 """
 from __future__ import annotations
 
@@ -13,9 +14,19 @@ import time
 import numpy as np
 import torch
 
+from .mix import MIX_AUTO_RESET, MIX_SCENARIOS, SLICE_ALIGN, check_aligned
 from .model.ppo import generate_action, generate_train_data, ppo_update_stage1, ppo_update_stage2
 from .model.utils import get_filter_index
 from .stage_world import RESULT_STRINGS
+
+
+def _episode_stats(ep):
+    """Episodes, success and crash rates and mean episode reward of eplog rows (E, 8)."""
+    n = len(ep)
+    nan = float('nan')
+    return {'episodes': n, 'success_rate': float((ep[:, 6] == 1).mean()) if n else nan,
+            'crash_rate': float((ep[:, 6] == 2).mean()) if n else nan,
+            'mean_ep_reward': float(ep[:, 2].mean()) if n else nan}
 
 
 class Rollout:
@@ -33,6 +44,85 @@ class Rollout:
         self.eplog = torch.zeros(horizon, n, 8, device=device)
 
 
+class _Component:
+    """One env handle of a run and its views of the rollout: agent columns [a, b), sliced once."""
+
+    def __init__(self, env, ro, a, b):
+        self.env, self.a, self.b = env, a, b
+        self.name = env.sc.name
+        self.relayout = env.sc.layout is not None
+        self.scaled = ro.scaled[a:b]
+        self.stacks = ro.stacks[:, a:b]
+        self.gs = ro.gs[:, a:b]
+        self.rewards = ro.rewards[:, a:b]
+        self.flags = ro.flags[:, a:b]
+        self.eplog = ro.eplog[:, a:b]
+
+    def check_aligned(self):
+        for name, view in (('action', self.scaled), ('stack', self.stacks), ('gs', self.gs),
+                           ('reward', self.rewards), ('flags', self.flags), ('eplog', self.eplog)):
+            check_aligned('%s[%d:%d] of %s' % (name, self.a, self.b, self.name), view, SLICE_ALIGN[name])
+
+    def start(self):
+        """The env's first episode, and slot 0 of its stacks and gs."""
+        e = self.env
+        e.reset_world()                                 # ppo_stage1.py:46-47
+        e.reset_pose()                                  # :50
+        e.generate_goal_point()                         # :52
+        if self.relayout:
+            e.random_layout()                           # the first layout, as evaluate() draws it
+        obs = e.get_laser_observation()
+        self.stacks[0] = obs[:, None, :]                # deque([obs, obs, obs]) (:60)
+        self.gs[0] = e.gs
+
+    def tick(self, t):
+        """Tick t on the component's slices, after the policy has written ro.scaled."""
+        e = self.env
+        e.control_vel(self.scaled, live=e.live if self.relayout else None, stack_in=self.stacks[t],
+                      stack_out=self.stacks[t + 1],
+                      out={'reward': self.rewards[t], 'flags': self.flags[t], 'gs': self.gs[t + 1],
+                           'eplog': self.eplog[t]})
+        if self.relayout:
+            e.relayout_finished(self.stacks[t + 1], out={'gs': self.gs[t + 1], 'flags': self.flags[t]})
+
+
+def compose(envs, ro):
+    """The components of `envs` on the rollout `ro`: env k owns the agent columns that follow env k - 1's.  With more
+    than one env, ValueError for a slice the kernels cannot read at its alignment (mix.SLICE_ALIGN)."""
+    comps, a = [], 0
+    for e in envs:
+        comps.append(_Component(e, ro, a, a + e.N))
+        a += e.N
+    if a != ro.scaled.shape[0]:
+        raise ValueError('the envs hold %d agents, the rollout %d' % (a, ro.scaled.shape[0]))
+    if len(comps) > 1:
+        for c in comps:
+            c.check_aligned()
+    return comps
+
+
+def _check_mix(envs, stage):
+    """ValueError unless `envs` can share one stage-2 rollout (DESIGN.md §9l)."""
+    if stage != 2:
+        raise ValueError('a mix of scenarios trains with stage 2, got stage %d' % stage)
+    seen = set()
+    for e in envs:
+        name, ar = e.sc.name, int(e.cfg.auto_reset)
+        if name == 'stage1':
+            raise ValueError("stage 1 cannot be mixed: it re-spawns each robot on its own and trains with stage 1's "
+                             'update')
+        if name not in MIX_SCENARIOS:
+            raise ValueError('scenario %r cannot be mixed (one of %s)' % (name, ', '.join(MIX_SCENARIOS)))
+        if name in seen:
+            raise ValueError('scenario %s appears more than once in the mix' % name)
+        seen.add(name)
+        if ar != MIX_AUTO_RESET[name]:
+            raise ValueError('%s trains with auto_reset %d in a mix, got %d' % (name, MIX_AUTO_RESET[name], ar))
+        if e.device != envs[0].device or e.beam_mum != envs[0].beam_mum:
+            raise ValueError('the envs of a mix must share the device and the beam count: %s has %s / %d, %s has %s / %d'
+                             % (envs[0].sc.name, envs[0].device, envs[0].beam_mum, name, e.device, e.beam_mum))
+
+
 def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logger_cal=None, stage=1, max_updates=None,
         process_group=None, rank=0, save_every=20, generator=None, start_update=0):
     """hp: dict with HORIZON, GAMMA, LAMDA, BATCH_SIZE, EPOCH, COEFF_ENTROPY, CLIP_VALUE, NUM_ENV, OBS_SIZE, ACT_SIZE,
@@ -40,22 +130,29 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     A random scenario (env.sc.layout, DESIGN.md §9k) trains with stage 2's update on per-world layouts: the env runs
     with auto_reset 0, every tick passes env.live and is followed by env.relayout_finished, and a world whose robots
     have all ended their episodes gets a new layout.
-    Returns per-update stats (for tests / benchmarks)."""
-    relayout = env.sc.layout is not None
-    if relayout and (stage != 2 or int(env.cfg.auto_reset) != 0):
-        raise ValueError('a random scenario trains with stage 2 and auto_reset 0 (per-world re-layouts), got stage %d '
-                         'and auto_reset %d' % (stage, int(env.cfg.auto_reset)))
-    H, N = hp['HORIZON'], env.N
-    dev = env.device
-    ro = Rollout(H, N, env.beam_mum, dev)
-    env.reset_world()                                   # ppo_stage1.py:46-47
-    env.reset_pose()                                    # :50
-    env.generate_goal_point()                           # :52
-    if relayout:
-        env.random_layout()                             # the first layout, as evaluate() draws it
-    obs = env.get_laser_observation()
-    ro.stacks[0] = obs[:, None, :]                      # deque([obs, obs, obs]) (:60)
-    ro.gs[0] = env.gs
+    `env` may be a sequence of envs, one per scenario (DESIGN.md §9l): stage 2 and the circle with auto_reset 2 and a
+    random scenario with auto_reset 0, each at most once, with stage 2.  Component k owns the rollout's agent columns
+    [a_k, b_k) in the order given; every tick runs one policy forward over all N = sum N_k columns, then each
+    component's tick (and re-layout) on its slices, and each update is stage 2's over the whole (H, N) batch.  A
+    one-element sequence is the single-env run.
+    Returns per-update stats (for tests / benchmarks); 'by_scenario' splits the episodes by component."""
+    envs = list(env) if isinstance(env, (list, tuple)) else [env]
+    if not envs:
+        raise ValueError('trainer.run needs at least one env')
+    mixed = len(envs) > 1
+    for e in envs:
+        if e.sc.layout is not None and (stage != 2 or int(e.cfg.auto_reset) != 0):
+            raise ValueError('a random scenario trains with stage 2 and auto_reset 0 (per-world re-layouts), got stage '
+                             '%d and auto_reset %d' % (stage, int(e.cfg.auto_reset)))
+    if mixed:
+        _check_mix(envs, stage)
+    H, N = hp['HORIZON'], sum(e.N for e in envs)
+    dev = envs[0].device
+    ro = Rollout(H, N, envs[0].beam_mum, dev)
+    comps = compose(envs, ro)
+    col_comp = np.repeat(np.arange(len(comps)), [e.N for e in envs])     # component of every agent column
+    for c in comps:
+        c.start()
     global_update = int(start_update)
     updates_done = 0
     episodes = 0
@@ -63,14 +160,11 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     while True:
         t0 = time.perf_counter()
         for t in range(H):
-            generate_action(env=env, state_list=(ro.stacks[t], ro.gs[t]), policy=policy, action_bound=action_bound,
+            generate_action(env=envs[0], state_list=(ro.stacks[t], ro.gs[t]), policy=policy, action_bound=action_bound,
                             out={'value': ro.values[t], 'action': ro.actions[t], 'logprob': ro.logprobs[t],
                                  'scaled': ro.scaled})
-            env.control_vel(ro.scaled, live=env.live if relayout else None, stack_in=ro.stacks[t],
-                            stack_out=ro.stacks[t + 1],
-                            out={'reward': ro.rewards[t], 'flags': ro.flags[t], 'gs': ro.gs[t + 1], 'eplog': ro.eplog[t]})
-            if relayout:
-                env.relayout_finished(ro.stacks[t + 1], out={'gs': ro.gs[t + 1], 'flags': ro.flags[t]})
+            for c in comps:
+                c.tick(t)
         # last_v from the state after the horizon (ppo_stage1.py:94-97)
         last_v, _ = policy.forward_values(ro.stacks[H], ro.gs[H])
         dones = ro.flags[:, :, 0]
@@ -78,8 +172,9 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
                                                   last_value=last_v, dones=dones, lam=hp['LAMDA'])
         torch.cuda.synchronize(dev)
         t1 = time.perf_counter()
-        if relayout:
-            env.check_relayout()
+        for c in comps:
+            if c.relayout:
+                c.env.check_relayout()
         memory = (ro.stacks[:H], ro.gs[:H, :, 0:2], ro.gs[:H, :, 2:4], ro.actions, ro.logprobs, t_batch, ro.values,
                   ro.rewards, advs_batch)
         common = dict(policy=policy, optimizer=optimizer, batch_size=hp['BATCH_SIZE'], memory=memory, epoch=hp['EPOCH'],
@@ -89,7 +184,10 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
         if stage == 1:
             rows = ppo_update_stage1(**common)
         else:
-            filter_index = get_filter_index(dones)            # ppo_stage2.py:112
+            # ppo_stage2.py:112.  The reference's run counter is not reset between columns, so a run of done carries
+            # from one robot's column into the next; in a mix it carries across the boundary between two components
+            # in the same way (§9l), exactly as for one env of N columns.
+            filter_index = get_filter_index(dones)
             rows = ppo_update_stage2(filter_index=filter_index, **common)
         torch.cuda.synchronize(dev)
         t2 = time.perf_counter()
@@ -104,13 +202,18 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
             episodes += 1
             if logger is not None and rank == 0:
                 res = RESULT_STRINGS.get(int(e[6]), 0)
+                c = comps[col_comp[i]]
+                robot = (i - c.a) % c.env.num_env           # the robot's index within its own component's world
                 if stage == 1:
                     dist = float(np.hypot(e[0] - e[4], e[1] - e[5]))
                     logger.info('Env %02d, Goal (%05.1f, %05.1f), Episode %05d, setp %03d, Reward %-5.1f, Distance %05.1f, %s' %
-                                (i % env.num_env, e[0], e[1], int(e[7]), int(e[3]) + 1, e[2], dist, res))
+                                (robot, e[0], e[1], int(e[7]), int(e[3]) + 1, e[2], dist, res))
+                elif mixed:
+                    logger.info('Env %02d, Goal (%05.1f, %05.1f), Episode %05d, setp %03d, Reward %-5.1f, %s, %s' %
+                                (robot, e[0], e[1], int(e[7]) - 1, int(e[3]), e[2], res, c.name))
                 else:
                     logger.info('Env %02d, Goal (%05.1f, %05.1f), Episode %05d, setp %03d, Reward %-5.1f, %s,' %
-                                (i % env.num_env, e[0], e[1], int(e[7]) - 1, int(e[3]), e[2], res))
+                                (robot, e[0], e[1], int(e[7]) - 1, int(e[3]), e[2], res))
             if logger_cal is not None and rank == 0:
                 logger_cal.info(float(e[2]))
         if rank == 0 and policy_path and global_update % save_every == 0:
@@ -121,11 +224,13 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
             if logger is not None:
                 logger.info('########################## model saved when update {} times#########'
                             '################'.format(global_update))
+        ep_comp = col_comp[idx[:, 1]]
         stats.append({'update': global_update, 'rollout_s': t1 - t0, 'update_s': t2 - t1,
                       'agent_steps_per_s': H * N / (t2 - t0), 'episodes': len(ep),
                       'mean_ep_reward': float(ep[:, 2].mean()) if len(ep) else float('nan'),
                       'success_rate': float((ep[:, 6] == 1).mean()) if len(ep) else float('nan'),
-                      'losses': rows[-1] if rows else None})
+                      'losses': rows[-1] if rows else None,
+                      'by_scenario': {c.name: _episode_stats(ep[ep_comp == k]) for k, c in enumerate(comps)}})
         # carry the state over the horizon boundary
         ro.stacks[0].copy_(ro.stacks[H])
         ro.gs[0].copy_(ro.gs[H])
