@@ -11,7 +11,10 @@ start at random positions in a --random-side S m square on circle.world's map, a
 with random goals at least --random-min-travel L m away (defaults 8, 10, 1 and S / 2; DESIGN.md §9i).  --hybrid switches
 the policy per robot by the nearest return of its newest scan: straight to the goal when it is beyond
 --hybrid-r-safe, the policy's action with v capped at --hybrid-v-safe when it is within --hybrid-r-risk, the policy's
-action otherwise, and prints the share of robot-ticks in each mode (DESIGN.md §9j).
+action otherwise, and prints the share of robot-ticks in each mode (DESIGN.md §9j).  --safety adds how closely the robots
+passed and why they crashed: crashes by cause (static map / another robot), and over the successful episodes the
+minimum separation between footprints, the minimum clearance and the near-miss rate, a near miss being a tick closer
+than --near-miss D m (default 0.1) to another robot (DESIGN.md §9m).
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -23,14 +26,17 @@ action otherwise, and prints the share of robot-ticks in each mode (DESIGN.md §
         --non-cooperative 5
     python evaluate.py --scenario random --baseline nh-orca --orca-map --num-worlds 1024 --random-robots 16
     python evaluate.py --scenario random --policy tests/golden/checkpoints/stage2.pth --num-worlds 1024 --hybrid
+    python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 --safety
 """
 import argparse
 import json
+import math
 import os
 
 import torch
 
-from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, evaluate, non_cooperative_mask
+from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, SAFETY_COLUMNS, evaluate, \
+    non_cooperative_mask
 from rl_collision_avoidance_b200.model.net import CNNPolicy
 from rl_collision_avoidance_b200.orca import HYBRID_DEFAULTS, Hybrid, NonCooperative, \
     add_arguments as add_controller_arguments, check_arguments as check_controller_arguments, check_hybrid, \
@@ -77,6 +83,11 @@ def main(argv=None):
                     help='hybrid: cap the speed when something is within R m (default %g)' % HYBRID_DEFAULTS['r_risk'])
     ap.add_argument('--hybrid-v-safe', type=float, default=None, metavar='V',
                     help='hybrid: the capped speed, m/s (default %g)' % HYBRID_DEFAULTS['v_safe'])
+    ap.add_argument('--safety', action='store_true',
+                    help='also report crashes by cause, minimum separation, minimum clearance and near misses '
+                         '(DESIGN.md §9m)')
+    ap.add_argument('--near-miss', type=float, default=None, metavar='D',
+                    help='a tick closer than D m to another robot is a near miss (default 0.1); implies --safety')
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -97,6 +108,9 @@ def main(argv=None):
         ap.error('--hybrid-r-safe / --hybrid-r-risk / --hybrid-v-safe apply with --hybrid only')
     if args.hybrid and args.baseline is not None:
         ap.error('--hybrid applies to --policy only')
+    if args.near_miss is not None and not (math.isfinite(args.near_miss) and args.near_miss >= 0.0):
+        ap.error('--near-miss must be finite and >= 0')
+    safety = args.near_miss if args.near_miss is not None else 0.1 if args.safety else None
     hybrid_params = None
     if args.hybrid:
         hybrid_params = dict(HYBRID_DEFAULTS)
@@ -136,7 +150,8 @@ def main(argv=None):
         nc = NonCooperative(env, non_cooperative_mask(sc.robots_per_world, args.num_worlds, args.non_cooperative),
                             speed=args.non_cooperative_speed)
     hy = Hybrid(env, **hybrid_params) if args.hybrid else None
-    out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy)
+    out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy,
+                   safety=safety)
 
     def line(m, robots, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -156,8 +171,24 @@ def main(argv=None):
         s = out['modes']
         print('hybrid modes over %d %srobot-ticks: policy %.4f  driver %.4f  safe %.4f'
               % (s['agent_ticks'], 'cooperative ' if nc is not None else '', s['policy'], s['driver'], s['safe']))
+
+    def safety_line(m, role=''):
+        f = lambda k: '%.3f +- %.3f' % m[k]
+        print('safety  %scrashes static %d  robot %d (both in range %d%s)  robot share %.4f  min separation %s m  '
+              'min clearance %s m  near-miss rate %.4f (< %g m)  least separation %.3f m'
+              % (role, m['crash_static'], m['crash_robot'], m['crash_both_in_range'],
+                 ', into non-cooperative %d' % m['crash_into_masked'] if nc is not None else '',
+                 m['crash_robot_share'], f('min_separation_reached'), f('min_clearance_reached'), m['near_miss_rate'],
+                 safety, m['min_separation']))
+
+    if safety is not None:
+        safety_line(out['safety'])
+        if nc is not None:
+            safety_line(out['safety_by_role']['cooperative'], 'cooperative  ')
+            safety_line(out['safety_by_role']['non_cooperative'], 'non-cooperative  ')
     if args.json:
-        res = {'args': vars(args), 'controller': controller or 'policy', 'robots': env.N,
+        shown = {k: v for k, v in vars(args).items() if safety is not None or k not in ('safety', 'near_miss')}
+        res = {'args': shown, 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
                'columns': list(COLUMNS), 'totals': out['totals'].tolist(),
                'partials': out['partials'].tolist()}
@@ -167,6 +198,12 @@ def main(argv=None):
         if hy is not None:
             res['modes'] = out['modes']
             res['mode_counts'] = out['mode_counts'].tolist()
+        if safety is not None:
+            res['safety'] = {'near_miss': safety, 'metrics': out['safety'], 'columns': list(SAFETY_COLUMNS),
+                             'totals': out['safety_totals'].tolist(), 'partials': out['safety_partials'].tolist()}
+            if nc is not None:
+                res['safety']['by_role'] = out['safety_by_role']
+                res['safety']['partials_split'] = out['safety_partials_split'].tolist()
         with open(args.json, 'w') as fh:
             json.dump(res, fh, indent=1)
     return out

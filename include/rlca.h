@@ -677,6 +677,97 @@ int rlca_layout_respawn_host(const rlca_env_config *cfg, const rlca_layout_param
 int rlca_stack_refresh(const rlca_env_config *cfg, const uint8_t *flags_dev, const float *obs_dev,
                        const float *gs_src_dev, float *stack_dev, float *gs_dev, void *stream);
 
+/* =====================================================================================
+ * Safety metrics (csrc/rlca_safety.cu, DESIGN.md §9m): how closely robots pass and why they crash, per episode of the
+ * evaluation tracker above.
+ *
+ * Footprint: the rectangle of half extents cfg->half_len, cfg->half_wid at the robot's pose (the tick's corners).
+ * Separation of a robot at a tick: the least distance between its footprint and the footprint of any other robot of
+ * its world, 0 when two intersect, +inf in a world of one robot; the partner is the robot that attains it (lowest
+ * index on ties).  Every other robot of the world counts, finished or not: the tick's collision test sees them all.
+ * Clearance of a robot at a tick: the nearest return of the scan the tick wrote, (min obs + 0.5) * range_max metres.
+ * Contact bound: sqrt(2) resolution + 2 dt (v_max + max(|w_min|, |w_max|) r_c), r_c = sqrt(half_len^2 + half_wid^2):
+ * two robots whose footprints come to share a cell within one tick started it no farther apart than that.
+ * ===================================================================================== */
+typedef struct rlca_safety_params {
+    float near_dist;             /* a tick whose separation is below this is a near-miss tick; finite, >= 0 */
+} rlca_safety_params;
+
+/* Per-agent state, N rows; before the first tick it tracks the caller sets min_sep, min_clear and last_clear to +inf,
+ * near to 0 and partner to -1.
+ *   min_sep, partner   running episode: least separation so far and the robot (index in its world) it was to
+ *   min_clear          running episode: least clearance so far
+ *   last_clear         clearance of the previous tick's scan, taken at the pose the next tick starts from
+ *   near               running episode: near-miss ticks
+ *   records            (N, episodes, 4), slot for slot the tracker's records: minimum separation, minimum clearance,
+ *                      near-miss ticks, and an integer held exactly by the float:
+ *                        bits 0-1   crash cause: 0 not a crash, 1 static map, 2 robot
+ *                        bit  2     cause robot, and last_clear was below the contact bound too ("both in range")
+ *                        bits 8-15  1 + the robot (index in its world) a cause-robot crash is charged to, else 0
+ *                        bits 16-23 1 + the partner of the minimum separation, 0 = none */
+typedef struct rlca_safety_state {
+    float *min_sep_dev;
+    float *min_clear_dev;
+    float *last_clear_dev;
+    int32_t *near_dev;
+    int32_t *partner_dev;
+    float *records_dev;
+    int32_t episodes;
+} rlca_safety_state;
+
+/* One launch after each rlca_env_step and BEFORE that tick's rlca_eval_track, with the same cfg, state buffers and
+ * io: reads the poses of state_in / state_out, the episode indices of state_in, io->flags_dev, io->obs_dev and the
+ * tracker's closed / count (never written), so a tick belongs to the episode the tracker assigns it to and a record
+ * goes into the slot the tracker fills next.  Per tracked robot the tick's separation is taken at the poses of
+ * state_out; for a robot the tick re-spawned (flags.w: state_out is the next episode's pose) at the poses of state_in,
+ * all robots', and its scan is not folded.  A tick that ends an episode writes the record and resets the running
+ * state, as does a re-spawn.  An episode that ends with result 2 gets its cause from the separation d0 of the robot at
+ * the poses of state_in: static when d0 exceeds the contact bound, otherwise robot, charged to the partner of d0.
+ * RLCA_ERR_INVALID for a NULL pointer, robots_per_world outside 1..64, episodes < 1 or different from the tracker's,
+ * near_dist not finite or < 0. */
+int rlca_safety_track(const rlca_env_config *cfg, const rlca_safety_params *params, const rlca_env_state *state_in,
+                      const rlca_env_state *state_out, const rlca_step_io *io, const rlca_eval_state *ev,
+                      const rlca_safety_state *ss, void *stream);
+/* The same from HOST buffers (pose (N,4) float; meta (N,4) int32; flags (N,4) uint8; obs (N,beams) float; the rest as
+ * the device state) by serial loops over the same code; the outputs equal rlca_safety_track's bit for bit. */
+int rlca_safety_track_host(const rlca_env_config *cfg, const rlca_safety_params *params, const float *pose_in_host,
+                           const int32_t *meta_in_host, const float *pose_out_host, const uint8_t *flags_host,
+                           const float *obs_host, const int32_t *closed_host, const int32_t *count_host,
+                           int32_t episodes, float *min_sep_host, float *min_clear_host, float *last_clear_host,
+                           int32_t *near_host, int32_t *partner_host, float *records_host);
+/* Separation of the footprints at pose_a_host[i] and pose_b_host[i] ((n,4) float x, y, theta, _), i < n, and the
+ * contact bound of cfg: the code the tracker runs, for tests and tools (no device needed). */
+int rlca_safety_separation_host(const rlca_env_config *cfg, const float *pose_a_host, const float *pose_b_host,
+                                int32_t n, float *separation_host);
+int rlca_safety_contact_host(const rlca_env_config *cfg, float *contact);
+
+/* Per-world float64 partials of the safety records of worlds [world_begin, world_begin + world_count), one thread per
+ * world in agent-then-record order, no atomics: partials_dev (world_count, RLCA_SAFETY_NPARTIALS).  The tracker's
+ * state gives the number of records per agent and each record's result code.  With role_mask_dev (N uint8) the
+ * partials are split as rlca_eval_reduce_split splits its own, partials_dev (world_count, 2, RLCA_SAFETY_NPARTIALS):
+ * row 0 over the agents with mask 0, row 1 over the others.  Every column but the last is a sum; totals add them in
+ * global world order and take the minimum of the last. */
+#define RLCA_SAFETY_CRASH_STATIC 0         /* crashes with cause static */
+#define RLCA_SAFETY_CRASH_ROBOT 1          /* cause robot */
+#define RLCA_SAFETY_CRASH_BOTH_IN_RANGE 2  /* cause robot with a scan return within the contact bound as well */
+#define RLCA_SAFETY_CRASH_INTO_MASKED 3    /* cause robot, charged to a robot with role mask != 0 (0 without a mask) */
+#define RLCA_SAFETY_REACHED 4              /* episodes that reached the goal; the columns up to 12 are over these */
+#define RLCA_SAFETY_REACHED_SEPARATION 5   /* ... with a finite minimum separation */
+#define RLCA_SAFETY_SUM_SEPARATION 6       /* sum, sum of squares (6, 7) of the finite minimum separations */
+#define RLCA_SAFETY_REACHED_CLEARANCE 8    /* ... with a finite minimum clearance */
+#define RLCA_SAFETY_SUM_CLEARANCE 9        /* sum, sum of squares (9, 10) of the finite minimum clearances */
+#define RLCA_SAFETY_NEAR_EPISODES 11       /* ... with at least one near-miss tick */
+#define RLCA_SAFETY_SUM_NEAR_TICKS 12      /* their near-miss ticks */
+#define RLCA_SAFETY_MIN_SEPARATION 13      /* least minimum separation of all recorded episodes, +inf when none */
+#define RLCA_SAFETY_NPARTIALS 14
+int rlca_safety_reduce(const rlca_env_config *cfg, const rlca_safety_state *ss, const rlca_eval_state *ev,
+                       const uint8_t *role_mask_dev, int32_t world_begin, int32_t world_count, double *partials_dev,
+                       void *stream);
+/* The same reduction from HOST buffers (no device needed; the code rlca_safety_reduce runs). */
+int rlca_safety_reduce_host(const rlca_env_config *cfg, const float *safety_records_host,
+                            const float *eval_records_host, const int32_t *count_host, const uint8_t *role_mask_host,
+                            int32_t episodes, int32_t world_begin, int32_t world_count, double *partials_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

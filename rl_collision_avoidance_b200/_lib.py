@@ -73,10 +73,27 @@ class HybridParams(C.Structure):
     _fields_ = [('r_safe', C.c_float), ('r_risk', C.c_float), ('v_safe', C.c_float), ('heading_gain', C.c_float)]
 
 
+class SafetyParams(C.Structure):
+    """Mirror of rlca_safety_params (include/rlca.h)."""
+    _fields_ = [('near_dist', C.c_float)]
+
+
+class SafetyState(C.Structure):
+    """Mirror of rlca_safety_state (include/rlca.h)."""
+    _fields_ = [('min_sep_dev', C.c_void_p), ('min_clear_dev', C.c_void_p), ('last_clear_dev', C.c_void_p),
+                ('near_dev', C.c_void_p), ('partner_dev', C.c_void_p), ('records_dev', C.c_void_p),
+                ('episodes', C.c_int32)]
+
+
 # rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
 EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
                  'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
                  'sum_straight', 'sum_path')
+
+# rlca_safety_reduce partials per world (the RLCA_SAFETY_* columns of include/rlca.h); the last one is a minimum
+SAFETY_PARTIALS = ('crash_static', 'crash_robot', 'crash_both_in_range', 'crash_into_masked', 'reached',
+                   'reached_separation', 'sum_separation', 'sum_separation_sq', 'reached_clearance', 'sum_clearance',
+                   'sum_clearance_sq', 'near_episodes', 'sum_near_ticks', 'min_separation')
 
 
 # every symbol include/rlca.h declares: (name, restype, argtypes)
@@ -174,6 +191,16 @@ SYMBOLS = {
     'rlca_layout_respawn_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), _P, _P, _P, _P, _P, _P,
                                            _P]),
     'rlca_stack_refresh': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, _P, _P]),
+    'rlca_safety_track': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(SafetyParams), C.POINTER(EnvState),
+                                    C.POINTER(EnvState), C.POINTER(StepIO), C.POINTER(EvalState),
+                                    C.POINTER(SafetyState), _P]),
+    'rlca_safety_track_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(SafetyParams), _P, _P, _P, _P, _P, _P, _P,
+                                         C.c_int32, _P, _P, _P, _P, _P, _P]),
+    'rlca_safety_separation_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, C.c_int32, _P]),
+    'rlca_safety_contact_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(C.c_float)]),
+    'rlca_safety_reduce': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(SafetyState), C.POINTER(EvalState), _P, C.c_int32,
+                                     C.c_int32, _P, _P]),
+    'rlca_safety_reduce_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

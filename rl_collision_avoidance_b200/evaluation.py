@@ -23,6 +23,8 @@ from .orca import NhOrcaController, OrcaController, mode_shares
 
 COLUMNS = _lib.EVAL_PARTIALS
 NPARTIALS = len(COLUMNS)
+SAFETY_COLUMNS = _lib.SAFETY_PARTIALS
+SAFETY_NPARTIALS = len(SAFETY_COLUMNS)
 ACTION_BOUND = [[0, -1], [1, 1]]
 # the reference's episode mechanics per scenario: stage 1 re-spawns a robot as soon as it is done
 # (ppo_stage1.py:51-65), stage 2 re-spawns a group when all of it is done (ppo_stage2.py:49-106), circle runs one
@@ -126,6 +128,158 @@ def reduce_split_host(cfg, records, count, open_, mask, world_begin=0, world_cou
     return out
 
 
+class SafetyTracker:
+    """Per-episode safety records next to an EpisodeTracker's (DESIGN.md §9m): minimum separation between footprints
+    and the robot it was to, minimum clearance (nearest scan return), near-miss ticks (separation below `near_dist`
+    metres) and the cause of a crash.  Call `track()` after each `env.control_vel` and BEFORE `tracker.track()`: the
+    episode a tick belongs to and the record slot are read from the tracker's state as its own call will see them."""
+
+    def __init__(self, env, tracker, near_dist=0.1):
+        near_dist = float(near_dist)
+        if not (math.isfinite(near_dist) and near_dist >= 0.0):
+            raise ValueError('near_dist must be finite and >= 0')
+        self.env, self.tracker, self.near_dist = env, tracker, near_dist
+        N, dev = env.N, env.device
+        self.min_sep = torch.empty(N, device=dev)
+        self.min_clear = torch.empty(N, device=dev)
+        self.last_clear = torch.empty(N, device=dev)
+        self.near = torch.empty(N, dtype=torch.int32, device=dev)
+        self.partner = torch.empty(N, dtype=torch.int32, device=dev)
+        self.records = torch.empty(N, tracker.episodes, 4, device=dev)
+        self._params = _lib.SafetyParams(near_dist)
+        self._st = _lib.SafetyState(_ptr(self.min_sep), _ptr(self.min_clear), _ptr(self.last_clear), _ptr(self.near),
+                                    _ptr(self.partner), _ptr(self.records), tracker.episodes)
+        self.reset()
+
+    def reset(self):
+        """Forget every record and the running episodes (with the tracker's own reset())."""
+        for t in (self.min_sep, self.min_clear, self.last_clear):
+            t.fill_(math.inf)
+        self.near.zero_()
+        self.partner.fill_(-1)
+        self.records.zero_()
+
+    def track(self):
+        """Safety records of the tick `env.control_vel` just ran (same stream, no synchronisation)."""
+        env = self.env
+        if not env._ticked:
+            raise RuntimeError('SafetyTracker.track() needs a tick: call env.control_vel first')
+        s_in, s_out = env._state_struct(1 - env._cur), env._state_struct(env._cur)
+        io = env._io(action=env._keep[0], out=env._last_out)
+        _lib.check(env.lib.rlca_safety_track(C.byref(env.cfg), C.byref(self._params), C.byref(s_in), C.byref(s_out),
+                                             C.byref(io), C.byref(self.tracker._st), C.byref(self._st),
+                                             env._stream()))
+
+    def partials(self, world_begin=0, world_count=None, role_mask=None):
+        """(world_count, SAFETY_NPARTIALS) float64 per-world partials, or (world_count, 2, SAFETY_NPARTIALS) split by
+        the agent mask `role_mask` (N): row 0 over the agents with mask 0, row 1 over the others, with the crashes
+        charged to a masked robot counted in 'crash_into_masked'."""
+        env = self.env
+        wc = env.num_worlds - world_begin if world_count is None else int(world_count)
+        m = None
+        if role_mask is not None:
+            m = torch.as_tensor(role_mask, device=env.device).to(torch.uint8).contiguous()
+            if m.shape != (env.N,):
+                raise ValueError(f'role_mask must have ({env.N},) entries')
+        shape = (wc, SAFETY_NPARTIALS) if m is None else (wc, 2, SAFETY_NPARTIALS)
+        out = torch.empty(shape, dtype=torch.float64, device=env.device)
+        _lib.check(env.lib.rlca_safety_reduce(C.byref(env.cfg), C.byref(self._st), C.byref(self.tracker._st), _ptr(m),
+                                              int(world_begin), wc, _ptr(out), env._stream()))
+        return out.cpu().numpy()
+
+
+def safety_contact(cfg):
+    """The contact bound of a config in metres (float32, as the library computes it)."""
+    out = C.c_float()
+    _lib.check(_lib.load().rlca_safety_contact_host(C.byref(cfg), C.byref(out)))
+    return np.float32(out.value)
+
+
+def safety_separation_host(cfg, pose_a, pose_b):
+    """Separation of the footprints at pose_a[i] and pose_b[i] ((n, 4) or (n, 3) x, y, theta), by the library's code."""
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    pad = lambda p: np.ascontiguousarray(np.concatenate(
+        (np.asarray(p, np.float32)[:, :3], np.zeros((len(p), 1), np.float32)), 1))
+    a, b = pad(pose_a), pad(pose_b)
+    if a.shape != b.shape:
+        raise ValueError('pose_a and pose_b must have the same number of rows')
+    out = np.zeros(len(a), np.float32)
+    _lib.check(_lib.load().rlca_safety_separation_host(C.byref(cfg), vp(a), vp(b), len(a), vp(out)))
+    return out
+
+
+def safety_track_host(cfg, near_dist, pose_in, meta_in, pose_out, flags, obs, closed, count, state):
+    """rlca_safety_track on host arrays (the same code, run by the CPU).  `state` is a dict of min_sep, min_clear,
+    last_clear (N) float32, near, partner (N) int32 and records (N, E, 4) float32, updated in place."""
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    f32 = lambda a: np.ascontiguousarray(a, np.float32)
+    i32 = lambda a: np.ascontiguousarray(a, np.int32)
+    for k, dt in (('min_sep', np.float32), ('min_clear', np.float32), ('last_clear', np.float32), ('near', np.int32),
+                  ('partner', np.int32), ('records', np.float32)):
+        if state[k].dtype != dt or not state[k].flags.c_contiguous:
+            raise ValueError(f'state[{k!r}] must be a contiguous {np.dtype(dt).name} array')
+    args = [f32(pose_in), i32(meta_in), f32(pose_out), np.ascontiguousarray(flags, np.uint8), f32(obs), i32(closed),
+            i32(count)]
+    _lib.check(_lib.load().rlca_safety_track_host(
+        C.byref(cfg), C.byref(_lib.SafetyParams(float(near_dist))), *(vp(a) for a in args), state['records'].shape[1],
+        *(vp(state[k]) for k in ('min_sep', 'min_clear', 'last_clear', 'near', 'partner', 'records'))))
+    return state
+
+
+def safety_reduce_host(cfg, safety_records, eval_records, count, role_mask=None, world_begin=0, world_count=None):
+    """rlca_safety_reduce on host arrays: (world_count, SAFETY_NPARTIALS), or (world_count, 2, ...) with a mask."""
+    vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
+    srec = np.ascontiguousarray(safety_records, np.float32)
+    erec = np.ascontiguousarray(eval_records, np.float32)
+    cnt = np.ascontiguousarray(count, np.int32)
+    msk = None if role_mask is None else np.ascontiguousarray(role_mask, np.uint8)
+    if msk is not None and msk.shape != cnt.shape:
+        raise ValueError('role_mask must have one entry per agent')
+    if srec.shape != erec.shape:
+        raise ValueError('the safety records and the tracker records must have the same shape')
+    wc = cfg.num_worlds - world_begin if world_count is None else int(world_count)
+    out = np.zeros((wc, SAFETY_NPARTIALS) if msk is None else (wc, 2, SAFETY_NPARTIALS), np.float64)
+    _lib.check(_lib.load().rlca_safety_reduce_host(C.byref(cfg), vp(srec), vp(erec), vp(cnt), vp(msk), srec.shape[1],
+                                                   int(world_begin), wc, vp(out)))
+    return out
+
+
+def safety_totals(partials):
+    """Per-world safety partials (rows in global world order): every column summed left to right except the last,
+    'min_separation', which is the minimum of the rows; the same bits however the rows were sharded."""
+    p = np.asarray(partials, np.float64).reshape(-1, SAFETY_NPARTIALS)
+    tot = np.zeros(SAFETY_NPARTIALS, np.float64)
+    tot[-1] = math.inf
+    for row in p:
+        tot[:-1] = tot[:-1] + row[:-1]
+        tot[-1] = min(tot[-1], row[-1])
+    return tot
+
+
+def safety_metrics(tot):
+    """Crashes by cause (counts, and shares of the crashes), and over the episodes that reached the goal the mean and
+    population std of the minimum separation and the minimum clearance (over those where it is finite), the share with
+    a near-miss tick and the mean near-miss ticks; 'min_separation' is the least of all recorded episodes."""
+    t = dict(zip(SAFETY_COLUMNS, np.asarray(tot, np.float64).tolist()))
+    crashes = t['crash_static'] + t['crash_robot']
+    n = t['reached']
+    out = {k: int(t[k]) for k in ('crash_static', 'crash_robot', 'crash_both_in_range', 'crash_into_masked', 'reached',
+                                  'near_episodes')}
+    out['crash_robot_share'] = t['crash_robot'] / crashes if crashes else math.nan
+    for name, cnt, col in (('min_separation_reached', 'reached_separation', 'separation'),
+                           ('min_clearance_reached', 'reached_clearance', 'clearance')):
+        k = t[cnt]
+        if k:
+            mean = t['sum_' + col] / k
+            out[name] = (mean, math.sqrt(max(t['sum_' + col + '_sq'] / k - mean * mean, 0.0)))
+        else:
+            out[name] = (math.nan, math.nan)
+    out['near_miss_rate'] = t['near_episodes'] / n if n else math.nan
+    out['mean_near_miss_ticks'] = t['sum_near_ticks'] / n if n else math.nan
+    out['min_separation'] = t['min_separation']
+    return out
+
+
 def non_cooperative_mask(robots_per_world, num_worlds, k):
     """(robots_per_world * num_worlds,) uint8 with robots floor(j R / k), j < k, of every world set: k robots spread
     evenly round the circle table (DESIGN.md §9h).  ValueError unless 1 <= k <= R."""
@@ -169,7 +323,7 @@ def metrics(tot):
     return out
 
 
-def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None):
+def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
@@ -188,13 +342,20 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     before the non-cooperative override, so masked robots still get the driver's action.  The result then also holds
     'mode_counts' (num_worlds, 3) int64, the ticks of tracked episodes each world's robots spent in each mode, and
     'modes' (orca.mode_shares: the share of those agent-ticks per mode and 'agent_ticks'); with `non_cooperative`
-    both cover the cooperative robots only."""
+    both cover the cooperative robots only.
+
+    With `safety` (a near-miss distance in metres) a SafetyTracker runs before the episode tracker on every tick and
+    the result also holds 'safety_partials' (num_worlds, SAFETY_NPARTIALS), 'safety_totals', 'safety'
+    (safety_metrics) and 'safety_tracker'; with `non_cooperative` also 'safety_partials_split' and 'safety_by_role',
+    where the cooperative row's 'crash_into_masked' counts its crashes into a non-cooperative robot.  With None nothing
+    of this is allocated or launched."""
     E = int(episodes)
     if int(check_every) < 1:
         raise ValueError('check_every must be >= 1')
     if hybrid is not None and isinstance(policy, (OrcaController, NhOrcaController)):
         raise ValueError('hybrid switches a policy; the ORCA baselines are not switched')
     tracker = EpisodeTracker(env, E)
+    safe = SafetyTracker(env, tracker, safety) if safety is not None else None
     N, dev = env.N, env.device
     circle = int(env.cfg.auto_reset) == 0
     env.reset_world()
@@ -225,6 +386,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         if circle:
             scaled = torch.stack((torch.where(terminal, 0.0, scaled[:, 0]), scaled[:, 1]), 1)
         env.control_vel(scaled, stack_in=stacks[k], stack_out=stacks[1 - k])
+        if safe is not None:
+            safe.track()
         tracker.track()
         if circle:
             terminal = env.flags[:, 0] != 0
@@ -242,4 +405,13 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     if hybrid is not None:
         out['mode_counts'] = hybrid.counts_per_world(None if non_cooperative is None else non_cooperative.mask)
         out['modes'] = mode_shares(out['mode_counts'])
+    if safe is not None:
+        sp = safe.partials()
+        out.update(safety_partials=sp, safety_totals=safety_totals(sp), safety_tracker=safe)
+        out['safety'] = safety_metrics(out['safety_totals'])
+        if non_cooperative is not None:
+            ss = safe.partials(role_mask=non_cooperative.mask)
+            out['safety_partials_split'] = ss
+            out['safety_by_role'] = {'cooperative': safety_metrics(safety_totals(ss[:, 0])),
+                                     'non_cooperative': safety_metrics(safety_totals(ss[:, 1]))}
     return out
