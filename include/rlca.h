@@ -312,6 +312,48 @@ int rlca_ppo_loss_fwd_bwd_weighted(rlca_policy *pol, const float *params_dev, co
                                    float coeff_entropy, float value_coef, float grad_weight, float *losses_dev,
                                    void *stream);
 
+/* PPO update diagnostics (DESIGN.md §9n): what an update did to the policy and the critic, accumulated on the device
+ * into rows of RLCA_PPO_DIAG_COLUMNS doubles, one row per epoch, read back once per update.  Every column has ONE merge
+ * rule - sum, max or min - by which minibatches, epochs and data-parallel ranks combine.  A fresh row holds 0 in the
+ * sum columns, -inf in the max columns and +inf in the min column.  With r = exp(new_lp - old_lp), A the advantage, t
+ * the value target, V the value and c the clip value: */
+#define RLCA_PPO_DIAG_N 0               /* rows */
+#define RLCA_PPO_DIAG_SUM_KL 1          /* sum of old_lp - new_lp */
+#define RLCA_PPO_DIAG_SUM_KL_K3 2       /* sum of (r - 1) - log r, with r - 1 as expm1(log r) */
+#define RLCA_PPO_DIAG_CLIPPED 3         /* rows with |r - 1| > c */
+#define RLCA_PPO_DIAG_CUT 4             /* rows whose surrogate gradient is cut: r > 1 + c with A > 0, r < 1 - c with A < 0 */
+#define RLCA_PPO_DIAG_SUM_RATIO 5       /* sum of r */
+#define RLCA_PPO_DIAG_SUM_ERR 6         /* sum, sum of squares (6, 7) of t - V */
+#define RLCA_PPO_DIAG_SUM_TARGET 8      /* sum, sum of squares (8, 9) of t */
+#define RLCA_PPO_DIAG_SUM_VALUE 10      /* sum of V */
+#define RLCA_PPO_DIAG_SUM_ADV 11        /* sum, sum of squares (11, 12) of A */
+#define RLCA_PPO_DIAG_MEAN_OUT 13       /* rows whose policy mean lies outside the action bound, per action dimension (13, 14) */
+#define RLCA_PPO_DIAG_ACTION_OUT 15     /* rows whose sampled action lies outside it (15, 16) */
+#define RLCA_PPO_DIAG_MAX_RATIO 17      /* MAX: largest r */
+#define RLCA_PPO_DIAG_MIN_RATIO 18      /* MIN: smallest r */
+#define RLCA_PPO_DIAG_GRAD_STEPS 19     /* rlca_grad_sumsq calls */
+#define RLCA_PPO_DIAG_GRAD_SUMSQ 20     /* sum of g^2 of each of the RLCA_POLICY_NTENSORS tensors (20 .. 42) */
+#define RLCA_PPO_DIAG_MAX_GRAD_SUMSQ 43 /* MAX: largest whole-buffer sum of g^2 of one call */
+#define RLCA_PPO_DIAG_COLUMNS 44
+
+/* One minibatch into the row acc_dev.  Inputs as rlca_ppo_loss_fwd_bwd_weighted gets them after the same
+ * rlca_policy_forward; new_lp and r are that kernel's own fp32 arithmetic, bit for bit (one device function).
+ * action_bound = {lo0, lo1, hi0, hi1}, a HOST array.  Per-row terms are fp32, sums float64; one CTA with a fixed
+ * reduction tree and one thread per column adding into acc_dev in stream order, no atomics: the same input gives the
+ * same bits.  1 <= nb <= max_batch of `pol`; a NULL pointer or another nb is RLCA_ERR_INVALID. */
+int rlca_ppo_diag_accumulate(rlca_policy *pol, const float *params_dev, const float *value_dev,
+                             const float *mean_dev, const float *action_dev, const float *old_logprob_dev,
+                             const float *adv_dev, const float *target_dev, int32_t nb, float clip_value,
+                             const float *action_bound, double *acc_dev, void *stream);
+
+/* Sum of g^2 of every tensor of the flat gradient buffer (the padding between tensors is not read) into the
+ * RLCA_PPO_DIAG_GRAD_* columns of the row acc_dev: the per-tensor sums are added, the whole-buffer sum is merged into
+ * the max column, and the step count goes up by one.  Two launches, fixed chunks and a fixed order of the partial sums
+ * in float64 (scratch in `pol`), no atomics.  Call it after rlca_policy_backward on the same stream and BEFORE the
+ * gradient exchange and the optimizer step: it measures the LOCAL gradient as the backward wrote it - scaled by
+ * grad_weight, and under data parallelism this rank's share of the step's gradient, not the all-reduced one. */
+int rlca_grad_sumsq(rlca_policy *pol, const float *grads_dev, double *acc_dev, void *stream);
+
 /* Behaviour-cloning loss of one minibatch and its gradient w.r.t. the network outputs (the SL-policy, DESIGN.md §9g):
  * loss = mean over rows of sum_k (mean_k - target_k)^2, target_action_dev (nb,2) the demonstrated action.
  * losses_dev[0] = loss.  The output gradients stay in the workspace for rlca_policy_backward: the value's is 0, so the

@@ -16,6 +16,7 @@ import sys
 import torch
 
 from rl_collision_avoidance_b200.mix import MIX_AUTO_RESET, parse_mix, plan
+from rl_collision_avoidance_b200.model.diagnostics import check_target_kl, setup_diag_log
 from rl_collision_avoidance_b200.model.net import Adam, CNNPolicy
 from rl_collision_avoidance_b200.model.ppo import setup_ppo_log
 from rl_collision_avoidance_b200.scenarios import add_random_arguments, check_random_arguments, \
@@ -104,8 +105,20 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     ap.add_argument('--mix', default=None, metavar='NAME:W,...',
                     help='train on several scenarios in one run (stage 2 only; DESIGN.md §9l): world counts per GPU of '
                          'stage2, circle and random, e.g. stage2:31,random:128,circle:14')
+    ap.add_argument('--diagnostics', action='store_true',
+                    help='write the health of every PPO update to log/<host>/diag.log (DESIGN.md §9n): approximate KL, '
+                         'clip fraction, explained variance, ratio extremes, action saturation, gradient norms')
+    ap.add_argument('--target-kl', type=float, default=None, metavar='X',
+                    help='skip the remaining epochs of an update once an epoch moved the policy by more than X '
+                         '(approx_kl_k3; finite and > 0; implies --diagnostics)')
     add_random_arguments(ap, timeout=True)
     args = ap.parse_args(argv)
+    if args.target_kl is not None:
+        try:
+            args.target_kl = check_target_kl(args.target_kl)
+        except ValueError as e:
+            ap.error('--target-kl: %s' % e)
+        args.diagnostics = True
     mix = None
     if args.mix is not None:
         if stage != 2:
@@ -136,6 +149,8 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
         dist.init_process_group('nccl', device_id=torch.device('cuda', local_rank))
         pg = True
     logger, logger_cal = make_loggers() if rank == 0 else (None, None)
+    if rank == 0 and args.diagnostics:
+        setup_diag_log()
     device = 'cuda:%d' % local_rank
     if args.scenario == 'circle':
         from rl_collision_avoidance_b200.circle_world import StageWorld as world_cls   # noqa: N813
@@ -195,7 +210,7 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     try:
         stats = run(env=env, policy=policy, policy_path=args.policy_path, action_bound=action_bound, optimizer=opt, hp=hp,
                     logger=logger, logger_cal=logger_cal, stage=stage, max_updates=args.updates, process_group=pg, rank=rank,
-                    start_update=start_update)
+                    start_update=start_update, diagnostics=args.diagnostics, target_kl=args.target_kl)
         if rank == 0 and stats:
             s = stats[-1]
             print('update %d: rollout %.3fs update %.3fs -> %.0f agent-steps/s per GPU; mean ep reward %.2f' %

@@ -133,6 +133,8 @@ SYMBOLS = {
                                         _P, _P]),
     'rlca_ppo_loss_fwd_bwd_weighted': (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_float, C.c_float,
                                                  C.c_float, C.c_float, _P, _P]),
+    'rlca_ppo_diag_accumulate': (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_float, _P, _P, _P]),
+    'rlca_grad_sumsq': (C.c_int, [_P, _P, _P, _P]),
     'rlca_bc_loss_fwd_bwd': (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P]),
     'rlca_policy_backward': (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P]),
     'rlca_adam_step': (C.c_int, [_P, _P, _P, _P, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32,

@@ -120,6 +120,7 @@ struct rlca_policy {
     cudaStream_t side[2];
     cudaEvent_t ev_fork, ev_heads, ev_dx, ev_split, ev_prep, ev_join[2];
     float *S2;                    // split-reduction scratch of the conv tower partials (the side streams use S meanwhile)
+    double *gsq_part;             // rlca_grad_sumsq partials [RLCA_POLICY_NTENSORS][GSQ_MAXCHUNKS]
     int64_t launches;
 };
 
@@ -842,6 +843,14 @@ __device__ __forceinline__ float block_sum_1024(float v, float *sh)
     return sh[32];
 }
 
+// New log-probability of a row's action from d = action - mean (log_normal_density, model/utils.py:90-97) and its ratio
+// to the rollout's.  One copy for the loss and for the diagnostics, which must see the loss's own bits.
+__device__ __forceinline__ float ppo_row_logprob(float d0, float d1, float ls0, float ls1, float var0, float var1)
+{
+    return (-(d0 * d0) / (2.0f * var0) - LOG_2PI_HALF - ls0) + (-(d1 * d1) / (2.0f * var1) - LOG_2PI_HALF - ls1);
+}
+__device__ __forceinline__ float ppo_row_ratio(float lp, float old_lp) { return expf(lp - old_lp); }
+
 __global__ void __launch_bounds__(1024) ppo_loss_kernel(const float *__restrict__ logstd, const float *__restrict__ value,
                                                         const float *__restrict__ mean, const float *__restrict__ action,
                                                         const float *__restrict__ old_lp, const float *__restrict__ adv,
@@ -859,8 +868,7 @@ __global__ void __launch_bounds__(1024) ppo_loss_kernel(const float *__restrict_
     for (int i = threadIdx.x; i < nb; i += 1024) {
         const float m0 = mean[2 * i], m1 = mean[2 * i + 1];
         const float d0 = action[2 * i] - m0, d1 = action[2 * i + 1] - m1;
-        const float lp = (-(d0 * d0) / (2.0f * var0) - LOG_2PI_HALF - ls0) + (-(d1 * d1) / (2.0f * var1) - LOG_2PI_HALF - ls1);
-        const float ratio = expf(lp - old_lp[i]);
+        const float ratio = ppo_row_ratio(ppo_row_logprob(d0, d1, ls0, ls1, var0, var1), old_lp[i]);
         const float A = adv[i];
         const float s1 = ratio * A;
         const float s2 = fminf(fmaxf(ratio, 1.0f - clip), 1.0f + clip) * A;
@@ -884,6 +892,141 @@ __global__ void __launch_bounds__(1024) ppo_loss_kernel(const float *__restrict_
         losses[2] = (0.5f + LOG_2PI_HALF + ls0) + (0.5f + LOG_2PI_HALF + ls1);   // dist_entropy (model/net.py:78-79)
         dlogstd[0] = g0 - coeff_entropy * weight;
         dlogstd[1] = g1 - coeff_entropy * weight;
+    }
+}
+
+// ------------------------------------------------------------------------------------ PPO update diagnostics
+// One minibatch into one accumulator row (the RLCA_PPO_DIAG_* columns of include/rlca.h, DESIGN.md §9n).  Single CTA:
+// per-row terms in fp32, per-thread sums in float64, a shuffle tree per warp, the warps in order, and one thread per
+// column merging into acc - a fixed order, so the same input gives the same bits.  "Outside the bound" counts a value
+// that is not strictly inside it: the mean is a sigmoid / tanh output and reaches the bound only by saturating in fp32.
+#define DIAG_THREADS 512
+
+__global__ void __launch_bounds__(DIAG_THREADS) ppo_diag_kernel(const float *__restrict__ logstd, const float *__restrict__ value,
+                                                                const float *__restrict__ mean, const float *__restrict__ action,
+                                                                const float *__restrict__ old_lp, const float *__restrict__ adv,
+                                                                const float *__restrict__ target, int nb, float clip,
+                                                                float lo0, float lo1, float hi0, float hi1,
+                                                                double *__restrict__ acc)
+{
+    __shared__ double sh[DIAG_THREADS / 32][RLCA_PPO_DIAG_MIN_RATIO + 1];
+    const float ls0 = logstd[0], ls1 = logstd[1];
+    const float var0 = expf(2.0f * ls0), var1 = expf(2.0f * ls1);
+    double s[RLCA_PPO_DIAG_MAX_RATIO];           // the sum columns, indexed as in acc
+#pragma unroll
+    for (int c = 0; c < RLCA_PPO_DIAG_MAX_RATIO; ++c) s[c] = 0.0;
+    float rmax = -INFINITY, rmin = INFINITY;
+    for (int i = threadIdx.x; i < nb; i += DIAG_THREADS) {
+        const float m0 = mean[2 * i], m1 = mean[2 * i + 1];
+        const float a0 = action[2 * i], a1 = action[2 * i + 1];
+        const float lp = ppo_row_logprob(a0 - m0, a1 - m1, ls0, ls1, var0, var1);
+        const float r = ppo_row_ratio(lp, old_lp[i]);
+        const float logr = lp - old_lp[i];
+        const float A = adv[i], t = target[i], V = value[i];
+        const float err = t - V;
+        s[RLCA_PPO_DIAG_N] += 1.0;
+        s[RLCA_PPO_DIAG_SUM_KL] += (double)(-logr);
+        s[RLCA_PPO_DIAG_SUM_KL_K3] += (double)(expm1f(logr) - logr);       // r - 1 without the cancellation near r = 1
+        s[RLCA_PPO_DIAG_CLIPPED] += fabsf(r - 1.0f) > clip ? 1.0 : 0.0;
+        s[RLCA_PPO_DIAG_CUT] += ((r > 1.0f + clip && A > 0.0f) || (r < 1.0f - clip && A < 0.0f)) ? 1.0 : 0.0;
+        s[RLCA_PPO_DIAG_SUM_RATIO] += (double)r;
+        s[RLCA_PPO_DIAG_SUM_ERR] += (double)err;
+        s[RLCA_PPO_DIAG_SUM_ERR + 1] += (double)err * (double)err;
+        s[RLCA_PPO_DIAG_SUM_TARGET] += (double)t;
+        s[RLCA_PPO_DIAG_SUM_TARGET + 1] += (double)t * (double)t;
+        s[RLCA_PPO_DIAG_SUM_VALUE] += (double)V;
+        s[RLCA_PPO_DIAG_SUM_ADV] += (double)A;
+        s[RLCA_PPO_DIAG_SUM_ADV + 1] += (double)A * (double)A;
+        s[RLCA_PPO_DIAG_MEAN_OUT] += (m0 > lo0 && m0 < hi0) ? 0.0 : 1.0;
+        s[RLCA_PPO_DIAG_MEAN_OUT + 1] += (m1 > lo1 && m1 < hi1) ? 0.0 : 1.0;
+        s[RLCA_PPO_DIAG_ACTION_OUT] += (a0 > lo0 && a0 < hi0) ? 0.0 : 1.0;
+        s[RLCA_PPO_DIAG_ACTION_OUT + 1] += (a1 > lo1 && a1 < hi1) ? 0.0 : 1.0;
+        rmax = fmaxf(rmax, r);
+        rmin = fminf(rmin, r);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+        for (int c = 0; c < RLCA_PPO_DIAG_MAX_RATIO; ++c) s[c] += __shfl_xor_sync(0xffffffffu, s[c], o);
+        rmax = fmaxf(rmax, __shfl_xor_sync(0xffffffffu, rmax, o));
+        rmin = fminf(rmin, __shfl_xor_sync(0xffffffffu, rmin, o));
+    }
+    if ((threadIdx.x & 31) == 0) {
+        double *row = sh[threadIdx.x >> 5];
+#pragma unroll
+        for (int c = 0; c < RLCA_PPO_DIAG_MAX_RATIO; ++c) row[c] = s[c];
+        row[RLCA_PPO_DIAG_MAX_RATIO] = (double)rmax;
+        row[RLCA_PPO_DIAG_MIN_RATIO] = (double)rmin;
+    }
+    __syncthreads();
+    const int c = threadIdx.x;
+    if (c <= RLCA_PPO_DIAG_MIN_RATIO) {
+        double v = sh[0][c];
+        for (int w = 1; w < DIAG_THREADS / 32; ++w)
+            v = c == RLCA_PPO_DIAG_MAX_RATIO ? fmax(v, sh[w][c]) : c == RLCA_PPO_DIAG_MIN_RATIO ? fmin(v, sh[w][c]) : v + sh[w][c];
+        acc[c] = c == RLCA_PPO_DIAG_MAX_RATIO ? fmax(acc[c], v) : c == RLCA_PPO_DIAG_MIN_RATIO ? fmin(acc[c], v) : acc[c] + v;
+    }
+}
+
+// Sum of g^2 per tensor of the flat gradient buffer: CTA (x, k) sums chunk x of tensor k in float64 into part[k][x]
+// (CTAs past the tensor's end leave), grad_sumsq_final_kernel adds a tensor's chunks in a fixed order and merges the row.
+#define GSQ_THREADS 256
+#define GSQ_CHUNK 8192
+#define GSQ_MAXCHUNKS 128
+static_assert((int64_t)GSQ_CHUNK * GSQ_MAXCHUNKS >= (int64_t)256 * FEAT, "fc1.weight, the largest tensor, must fit the grid");
+
+struct GradTensors {
+    int64_t off[RLCA_POLICY_NTENSORS];
+    int32_t size[RLCA_POLICY_NTENSORS];
+};
+
+__global__ void __launch_bounds__(GSQ_THREADS) grad_sumsq_kernel(const float *__restrict__ g, const GradTensors t,
+                                                                 double *__restrict__ part)
+{
+    __shared__ double sh[GSQ_THREADS / 32];
+    const int k = blockIdx.y;
+    const int start = blockIdx.x * GSQ_CHUNK;
+    if (start >= t.size[k]) return;
+    const float *p = g + t.off[k] + start;
+    const int len = min(GSQ_CHUNK, t.size[k] - start), n4 = len >> 2;
+    double s = 0.0;
+    for (int i = threadIdx.x; i < n4; i += GSQ_THREADS) {
+        const float4 v = reinterpret_cast<const float4 *>(p)[i];
+        s += (double)v.x * (double)v.x + (double)v.y * (double)v.y + (double)v.z * (double)v.z + (double)v.w * (double)v.w;
+    }
+    for (int i = 4 * n4 + threadIdx.x; i < len; i += GSQ_THREADS) s += (double)p[i] * (double)p[i];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < GSQ_THREADS / 32; ++w) s += sh[w];
+        part[k * GSQ_MAXCHUNKS + blockIdx.x] = s;
+    }
+}
+
+// One warp per tensor: lane l adds chunks l, l + 32, ... in order, then the shuffle tree; thread 0 adds the tensors in order.
+__global__ void __launch_bounds__(32 * RLCA_POLICY_NTENSORS) grad_sumsq_final_kernel(const double *__restrict__ part,
+                                                                                     const GradTensors t,
+                                                                                     double *__restrict__ acc)
+{
+    __shared__ double sh[RLCA_POLICY_NTENSORS];
+    const int k = threadIdx.x >> 5;
+    const int chunks = (t.size[k] + GSQ_CHUNK - 1) / GSQ_CHUNK;
+    double s = 0.0;
+    for (int x = threadIdx.x & 31; x < chunks; x += 32) s += part[k * GSQ_MAXCHUNKS + x];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) {
+        sh[k] = s;
+        acc[RLCA_PPO_DIAG_GRAD_SUMSQ + k] += s;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double total = 0.0;
+        for (int j = 0; j < RLCA_POLICY_NTENSORS; ++j) total += sh[j];
+        acc[RLCA_PPO_DIAG_GRAD_STEPS] += 1.0;
+        acc[RLCA_PPO_DIAG_MAX_GRAD_SUMSQ] = fmax(acc[RLCA_PPO_DIAG_MAX_GRAD_SUMSQ], total);
     }
 }
 
@@ -1213,6 +1356,7 @@ extern "C" int rlca_policy_create(int32_t max_batch, rlca_policy **out)
     RLCA_CUDA_TRY(cudaMalloc(&p->Wc, 2 * CONV_WBLK * sizeof(float)));
     RLCA_CUDA_TRY(cudaMalloc(&p->S, (size_t)RSPLIT * 2 * 128 * XLD * sizeof(float)));
     RLCA_CUDA_TRY(cudaMalloc(&p->S2, (size_t)RSPLIT * 2 * CONV_PART * sizeof(float)));
+    RLCA_CUDA_TRY(cudaMalloc(&p->gsq_part, (size_t)RLCA_POLICY_NTENSORS * GSQ_MAXCHUNKS * sizeof(double)));
     for (int i = 0; i < 2; ++i) {
         RLCA_CUDA_TRY(cudaStreamCreateWithFlags(&p->side[i], cudaStreamNonBlocking));
         RLCA_CUDA_TRY(cudaEventCreateWithFlags(&p->ev_join[i], cudaEventDisableTiming));
@@ -1265,7 +1409,7 @@ extern "C" int rlca_policy_destroy(rlca_policy *p)
     if (!p) return RLCA_OK;
     cudaFree(p->F); cudaFree(p->X); cudaFree(p->H2); cudaFree(p->dOut); cudaFree(p->dZ2); cudaFree(p->dX);
     cudaFree(p->dF); cudaFree(p->part); cudaFree(p->headpart); cudaFree(p->red); cudaFree(p->S); cudaFree(p->Wc);
-    cudaFree(p->S2);
+    cudaFree(p->S2); cudaFree(p->gsq_part);
     for (int i = 0; i < 2; ++i) { if (p->side[i]) cudaStreamDestroy(p->side[i]); if (p->ev_join[i]) cudaEventDestroy(p->ev_join[i]); }
     if (p->ev_fork) cudaEventDestroy(p->ev_fork);
     if (p->ev_heads) cudaEventDestroy(p->ev_heads);
@@ -1435,6 +1579,37 @@ extern "C" int rlca_ppo_loss_fwd_bwd_weighted(rlca_policy *pol, const float *par
                                                          old_logprob, adv, target, nb, clip_value, coeff_entropy,
                                                          value_coef, grad_weight, pol->dOut, losses, pol->red);
     pol->launches += 1;
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_ppo_diag_accumulate(rlca_policy *pol, const float *params, const float *value, const float *mean,
+                                        const float *action, const float *old_logprob, const float *adv,
+                                        const float *target, int32_t nb, float clip_value, const float *action_bound,
+                                        double *acc, void *stream)
+{
+    if (!pol || !params || !value || !mean || !action || !old_logprob || !adv || !target || !action_bound || !acc)
+        return rlca_set_err(RLCA_ERR_INVALID, "NULL argument");
+    if (nb < 1 || nb > pol->max_batch) return rlca_set_err(RLCA_ERR_INVALID, "nb exceeds the workspace max_batch");
+    ppo_diag_kernel<<<1, DIAG_THREADS, 0, (cudaStream_t)stream>>>(params + tensor_offset(T_LOGSTD), value, mean, action,
+                                                                  old_logprob, adv, target, nb, clip_value,
+                                                                  action_bound[0], action_bound[1], action_bound[2],
+                                                                  action_bound[3], acc);
+    pol->launches += 1;
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_grad_sumsq(rlca_policy *pol, const float *grads, double *acc, void *stream)
+{
+    if (!pol || !grads || !acc) return rlca_set_err(RLCA_ERR_INVALID, "NULL argument");
+    if ((uintptr_t)grads & 15) return rlca_set_err(RLCA_ERR_INVALID, "the gradient buffer must be 16-byte aligned");
+    GradTensors t;
+    for (int k = 0; k < RLCA_POLICY_NTENSORS; ++k) { t.off[k] = tensor_offset(k); t.size[k] = (int32_t)kTensorSize[k]; }
+    cudaStream_t s = (cudaStream_t)stream;
+    grad_sumsq_kernel<<<dim3(GSQ_MAXCHUNKS, RLCA_POLICY_NTENSORS), GSQ_THREADS, 0, s>>>(grads, t, pol->gsq_part);
+    grad_sumsq_final_kernel<<<1, 32 * RLCA_POLICY_NTENSORS, 0, s>>>(pol->gsq_part, t, acc);
+    pol->launches += 2;
     RLCA_CUDA_TRY(cudaGetLastError());
     return RLCA_OK;
 }

@@ -128,11 +128,20 @@ class _MinibatchGather:
 
 def _ppo_update(policy: CNNPolicy, optimizer, batch_size, memory, epoch, coeff_entropy, clip_value, num_step, num_env,
                 frames, obs_size, act_size, filter_index=None, drop_last=False, generator=None, process_group=None,
-                value_coef=20.0, permutations=None):
+                value_coef=20.0, permutations=None, diagnostics=None, target_kl=None):
     """Body shared by ppo_update_stage1/2.  `permutations` (optional, one index array per epoch into the KEPT rows)
     replays a recorded SubsetRandomSampler order instead of drawing one (parity tests against the reference).
     Under a process group the minibatch schedule is agreed across ranks first (parallel.plan_minibatches), so ranks
-    with different row counts issue the same number of all-reduces."""
+    with different row counts issue the same number of all-reduces.
+    `diagnostics` (a diagnostics.PPODiagnostics, DESIGN.md §9n) accumulates every minibatch and its local gradient into
+    the row of its epoch; losses, weights and ppo.log are the same with and without it.  With `target_kl` the finished
+    epoch's row is read at every epoch boundary - one synchronisation each - and the remaining epochs are skipped once
+    its approx_kl_k3 exceeds target_kl; under a process group the row is merged over the ranks first, so all of them
+    stop together.  diagnostics.epochs_run is the number of epochs run."""
+    if target_kl is not None and diagnostics is None:
+        raise ValueError('target_kl needs diagnostics: the stop rule reads their rows')
+    if diagnostics is not None and diagnostics.epochs < epoch:
+        raise ValueError('the diagnostics hold %d epochs, the update runs %d' % (diagnostics.epochs, epoch))
     lib = _lib.load()
     obss, goals, speeds, actions, logprobs, targets, values, rewards, advs = memory
     dev = policy.device
@@ -155,7 +164,8 @@ def _ppo_update(policy: CNNPolicy, optimizer, batch_size, memory, epoch, coeff_e
     if process_group is not None:
         import torch.distributed as dist
         world = dist.get_world_size(group)
-    from ..parallel import OverlappedGradSync, average_gradients, plan_minibatches
+    from ..parallel import OverlappedGradSync, allreduce_diagnostics, average_gradients, plan_minibatches
+    from .diagnostics import RULES, over_target_kl
     # gradient exchange of a data-parallel run, in order of preference: (1) optimizer.peer (parallel.PeerAdam): the sum
     # over the ranks is part of the fused Adam kernel, nothing to do here; (2) one NCCL all-reduce of the flat buffer
     # after the backward; (3) RLCA_DP_OVERLAP=1: the fc-side ranges all-reduced under the rest of the backward
@@ -182,6 +192,8 @@ def _ppo_update(policy: CNNPolicy, optimizer, batch_size, memory, epoch, coeff_e
     gather = _MinibatchGather(lib, (obss, gs, actions, logprobs, advs, targets), (b_obs, b_gs, b_act, b_lp, b_adv, b_tgt),
                               (frames * obs_size, 4, act_size, 1, 1, 1), dev)
     k = 0
+    if diagnostics is not None:
+        diagnostics.reset()
     for update in range(epoch):
         if permutations is not None:
             perm = keep[torch.as_tensor(permutations[update], device=dev, dtype=torch.long)]
@@ -197,7 +209,11 @@ def _ppo_update(policy: CNNPolicy, optimizer, batch_size, memory, epoch, coeff_e
                                                               _ptr(b_lp), _ptr(b_adv), _ptr(b_tgt), nb, clip_value,
                                                               coeff_entropy, value_coef, float(weights[bi]),
                                                               _ptr(log[k]), st))
+                if diagnostics is not None:
+                    diagnostics.accumulate(update, v, mean, b_act, b_lp, b_adv, b_tgt, nb, clip_value)
                 _lib.check(lib.rlca_policy_backward(ws, _ptr(policy.flat), _ptr(b_obs), _ptr(b_gs), nb, _ptr(policy.grad), st))
+                if diagnostics is not None:
+                    diagnostics.grads(update)
             else:
                 policy.grad.zero_()             # this rank ran out of rows: it still takes part in the all-reduce
                 if sync is not None:
@@ -208,6 +224,16 @@ def _ppo_update(policy: CNNPolicy, optimizer, batch_size, memory, epoch, coeff_e
                 average_gradients(policy.grad, group)
             optimizer.step(grad_scale=1.0 / world)
             k += 1
+        if diagnostics is not None:
+            diagnostics.epochs_run = update + 1
+        if target_kl is not None and update + 1 < epoch:
+            row = diagnostics.acc[update].clone()
+            if process_group is not None:
+                allreduce_diagnostics(row, RULES, group)
+            if over_target_kl(row.cpu().numpy(), target_kl):
+                break
+    if diagnostics is not None and process_group is not None:
+        allreduce_diagnostics(diagnostics.acc, RULES, group)    # every rank reports the update of all ranks
     rows = log[:k].cpu().tolist()
     for pl, vl, ent in rows:
         logger_ppo.info('{}, {}, {}'.format(pl, vl, ent))
@@ -216,20 +242,21 @@ def _ppo_update(policy: CNNPolicy, optimizer, batch_size, memory, epoch, coeff_e
 
 def ppo_update_stage1(policy, optimizer, batch_size, memory, epoch, coeff_entropy=0.02, clip_value=0.2, num_step=2048,
                       num_env=12, frames=1, obs_size=24, act_size=4, generator=None, process_group=None,
-                      permutations=None):
+                      permutations=None, diagnostics=None, target_kl=None):
     """model/ppo.py:143-194 (drop_last=False)."""
     rows = _ppo_update(policy, optimizer, batch_size, memory, epoch, coeff_entropy, clip_value, num_step, num_env,
-                       frames, obs_size, act_size, None, False, generator, process_group, permutations=permutations)
+                       frames, obs_size, act_size, None, False, generator, process_group, permutations=permutations,
+                       diagnostics=diagnostics, target_kl=target_kl)
     print('update')
     return rows
 
 
 def ppo_update_stage2(policy, optimizer, batch_size, memory, filter_index, epoch, coeff_entropy=0.02, clip_value=0.2,
                       num_step=2048, num_env=12, frames=1, obs_size=24, act_size=4, generator=None, process_group=None,
-                      permutations=None):
+                      permutations=None, diagnostics=None, target_kl=None):
     """model/ppo.py:197-259 (filtered transitions deleted, drop_last=True)."""
     rows = _ppo_update(policy, optimizer, batch_size, memory, epoch, coeff_entropy, clip_value, num_step, num_env,
                        frames, obs_size, act_size, filter_index, True, generator, process_group,
-                       permutations=permutations)
+                       permutations=permutations, diagnostics=diagnostics, target_kl=target_kl)
     print('filter {} transitions; update'.format(len(filter_index)))
     return rows

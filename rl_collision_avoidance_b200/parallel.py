@@ -25,6 +25,23 @@ def allreduce_moments(moments: torch.Tensor, group=None):
     return moments
 
 
+def allreduce_diagnostics(acc: torch.Tensor, rules, group=None):
+    """Accumulator rows (..., columns) merged over ranks in place, column c by rules[c]: 'sum' columns with SUM, 'max'
+    columns with MAX and 'min' columns, negated, with the same MAX (model/diagnostics.py).  Every rank ends with the
+    same rows, so a decision taken from them is the same everywhere."""
+    import torch.distributed as dist
+    idx = lambda rule: torch.tensor([c for c, r in enumerate(rules) if r == rule], dtype=torch.long, device=acc.device)
+    isum, imax, imin = idx('sum'), idx('max'), idx('min')
+    sums = acc[..., isum].contiguous()
+    dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=group)
+    ext = torch.cat((acc[..., imax], -acc[..., imin]), dim=-1).contiguous()
+    dist.all_reduce(ext, op=dist.ReduceOp.MAX, group=group)
+    acc[..., isum] = sums
+    acc[..., imax] = ext[..., :imax.numel()]
+    acc[..., imin] = -ext[..., imax.numel():]
+    return acc
+
+
 def normalize_from_moments(x: torch.Tensor, moments: torch.Tensor):
     """(x - mean) / std with numpy semantics (ddof = 0) from global moments (model/ppo.py:148)."""
     cnt = moments[2]

@@ -124,7 +124,7 @@ def _check_mix(envs, stage):
 
 
 def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logger_cal=None, stage=1, max_updates=None,
-        process_group=None, rank=0, save_every=20, generator=None, start_update=0):
+        process_group=None, rank=0, save_every=20, generator=None, start_update=0, diagnostics=False, target_kl=None):
     """hp: dict with HORIZON, GAMMA, LAMDA, BATCH_SIZE, EPOCH, COEFF_ENTROPY, CLIP_VALUE, NUM_ENV, OBS_SIZE, ACT_SIZE,
     LASER_HIST, MAX_EPISODES.  `start_update` continues the checkpoint numbering of a resumed run.
     A random scenario (env.sc.layout, DESIGN.md §9k) trains with stage 2's update on per-world layouts: the env runs
@@ -135,6 +135,9 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     [a_k, b_k) in the order given; every tick runs one policy forward over all N = sum N_k columns, then each
     component's tick (and re-layout) on its slices, and each update is stage 2's over the whole (H, N) batch.  A
     one-element sequence is the single-env run.
+    `diagnostics` (DESIGN.md §9n) adds stats[k]['diagnostics'], the metrics of model.diagnostics.metrics plus
+    'epochs_run' and 'logstd', and rank 0 writes one line per update to the diag.log logger; `target_kl` (finite and
+    > 0, implies diagnostics) skips the remaining epochs of an update once an epoch's approx_kl_k3 exceeds it.
     Returns per-update stats (for tests / benchmarks); 'by_scenario' splits the episodes by component."""
     envs = list(env) if isinstance(env, (list, tuple)) else [env]
     if not envs:
@@ -153,6 +156,12 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     col_comp = np.repeat(np.arange(len(comps)), [e.N for e in envs])     # component of every agent column
     for c in comps:
         c.start()
+    diag = None
+    if diagnostics or target_kl is not None:
+        from .model.diagnostics import PPODiagnostics, check_target_kl, format_line, logger_diag
+        if target_kl is not None:
+            target_kl = check_target_kl(target_kl)
+        diag = PPODiagnostics(policy, hp['EPOCH'], action_bound)
     global_update = int(start_update)
     updates_done = 0
     episodes = 0
@@ -180,7 +189,7 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
         common = dict(policy=policy, optimizer=optimizer, batch_size=hp['BATCH_SIZE'], memory=memory, epoch=hp['EPOCH'],
                       coeff_entropy=hp['COEFF_ENTROPY'], clip_value=hp['CLIP_VALUE'], num_step=H, num_env=N,
                       frames=hp['LASER_HIST'], obs_size=hp['OBS_SIZE'], act_size=hp['ACT_SIZE'], generator=generator,
-                      process_group=process_group)
+                      process_group=process_group, diagnostics=diag, target_kl=target_kl)
         if stage == 1:
             rows = ppo_update_stage1(**common)
         else:
@@ -231,6 +240,10 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
                       'success_rate': float((ep[:, 6] == 1).mean()) if len(ep) else float('nan'),
                       'losses': rows[-1] if rows else None,
                       'by_scenario': {c.name: _episode_stats(ep[ep_comp == k]) for k, c in enumerate(comps)}})
+        if diag is not None:
+            stats[-1]['diagnostics'] = diag.metrics()
+            if rank == 0:
+                logger_diag.info(format_line(global_update, stats[-1]['diagnostics']))
         # carry the state over the horizon boundary
         ro.stacks[0].copy_(ro.stacks[H])
         ro.gs[0].copy_(ro.gs[H])
