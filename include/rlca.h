@@ -287,8 +287,13 @@ int rlca_policy_forward(rlca_policy *pol, const float *params_dev, const float *
 /* action ~ N(mean, exp(logstd)) with a counter-based generator (replaces torch.normal,
  * model/net.py:53-55), logprob = log_normal_density summed over the 2 dims
  * (model/utils.py:90-97), scaled = clip(action, [v_min,w_min], [v_max,w_max]) (model/ppo.py:75).
+ * deterministic == 0 -> row i draws Philox4x32-10 of counter (i, counter lo, counter hi, 0x5A17) under key
+ *   (seed lo, seed hi); u1 = ((w0 >> 8) + 1) * 2^-24, u2 = (w1 >> 8) * 2^-24, Box-Muller z = sqrt(-2 ln u1) *
+ *   (cos, sin)(2 pi u2) and action = mean + exp(logstd) * z.  A row's draw depends on (seed, counter, i) only;
  * deterministic == 1 -> action = mean (generate_action_no_sampling, model/ppo.py:84-107);
- * deterministic == 2 -> action_dev is an INPUT and only its logprob is evaluated (evaluate_actions, model/net.py:72-80). */
+ * deterministic == 2 -> action_dev is an INPUT and only its logprob is evaluated (evaluate_actions, model/net.py:72-80).
+ * Any other deterministic, nb < 1 or a NULL params, mean, action or logprob -> RLCA_ERR_INVALID, nothing launched.
+ * scaled_dev may be NULL. */
 int rlca_policy_sample(const float *params_dev, const float *mean_dev, int32_t nb, uint64_t seed, uint64_t counter,
                        int32_t deterministic, float *action_dev, float *logprob_dev, float *scaled_dev, void *stream);
 

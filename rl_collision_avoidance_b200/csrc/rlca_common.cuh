@@ -56,7 +56,8 @@ __host__ __device__ __forceinline__ void dev_philox(uint32_t (&c)[4], uint32_t k
 }
 
 // Four uniforms in [0, 1) (24 bits each) keyed by (seed, agent, episode, draw, purpose).  Purposes: 1 spawn and
-// heading, 2 goal (rlca_env.cu); 3 start, 4 goal, 5 heading of a random layout (rlca_layout.cu).
+// heading, 2 goal (rlca_env.cu); 3 start, 4 goal, 5 heading of a random layout (rlca_layout.cu).  The action sampler
+// (sample_kernel, rlca_policy.cu) calls dev_philox directly with purpose word 0x5A17 and counter (row, call counter).
 __host__ __device__ __forceinline__ void dev_rand4(uint64_t seed, uint32_t agent, uint32_t episode, uint32_t draw,
                                                    uint32_t purpose, float (&u)[4])
 {

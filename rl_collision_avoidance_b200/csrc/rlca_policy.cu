@@ -776,18 +776,6 @@ __global__ void __launch_bounds__(256) colsum_kernel(const ColsumArgs a)
 }
 
 // ------------------------------------------------------------------------------------ sampling
-__device__ __forceinline__ void philox4(uint32_t (&c)[4], uint32_t k0, uint32_t k1)
-{
-#pragma unroll
-    for (int i = 0; i < 10; ++i) {
-        uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
-        uint32_t hi1 = __umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
-        uint32_t n0 = hi1 ^ c[1] ^ k0, n2 = hi0 ^ c[3] ^ k1;
-        c[0] = n0; c[1] = lo1; c[2] = n2; c[3] = lo0;
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-}
-
 #define LOG_2PI_HALF 0.91893853320467274178f
 
 __global__ void sample_kernel(const float *__restrict__ logstd, const float *__restrict__ mean, int nb, uint64_t seed,
@@ -802,7 +790,7 @@ __global__ void sample_kernel(const float *__restrict__ logstd, const float *__r
     if (deterministic == 2) { a0 = action[2 * i]; a1 = action[2 * i + 1]; }   // evaluate a given action
     if (!deterministic) {
         uint32_t c[4] = {(uint32_t)i, (uint32_t)counter, (uint32_t)(counter >> 32), 0x5A17u};
-        philox4(c, (uint32_t)seed, (uint32_t)(seed >> 32));
+        dev_philox(c, (uint32_t)seed, (uint32_t)(seed >> 32));
         // Box-Muller on two 24-bit uniforms in (0,1]
         const float u1 = ((float)(c[0] >> 8) + 1.0f) * 5.9604644775390625e-08f;
         const float u2 = (float)(c[1] >> 8) * 5.9604644775390625e-08f;
@@ -1552,6 +1540,8 @@ extern "C" int rlca_policy_sample(const float *params, const float *mean, int32_
                                   int32_t deterministic, float *action, float *logprob, float *scaled, void *stream)
 {
     if (!params || !mean || !action || !logprob || nb < 1) return rlca_set_err(RLCA_ERR_INVALID, "NULL argument");
+    if (deterministic < 0 || deterministic > 2)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_policy_sample: deterministic must be 0, 1 or 2");
     sample_kernel<<<(nb + 127) / 128, 128, 0, (cudaStream_t)stream>>>(params + tensor_offset(T_LOGSTD), mean, nb, seed,
                                                                       counter, deterministic, action, logprob, scaled);
     RLCA_CUDA_TRY(cudaGetLastError());
