@@ -14,7 +14,11 @@ the policy per robot by the nearest return of its newest scan: straight to the g
 action otherwise, and prints the share of robot-ticks in each mode (DESIGN.md §9j).  --safety adds how closely the robots
 passed and why they crashed: crashes by cause (static map / another robot), and over the successful episodes the
 minimum separation between footprints, the minimum clearance and the near-miss rate, a near miss being a tick closer
-than --near-miss D m (default 0.1) to another robot (DESIGN.md §9m).
+than --near-miss D m (default 0.1) to another robot (DESIGN.md §9m).  --timeouts adds why robots timed out or never
+finished: each time-out and each unfinished episode is called frozen (its centre has not moved for --stall-window W
+ticks, default 50), stalled (it moves but has not come 0.1 m closer to its goal in W ticks) or slow (still getting
+closer), and marked when another robot stood within 1 m; with the closest distance to the goal left, the share of
+still ticks and the rotation per successful episode (DESIGN.md §9o).
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -27,6 +31,8 @@ than --near-miss D m (default 0.1) to another robot (DESIGN.md §9m).
     python evaluate.py --scenario random --baseline nh-orca --orca-map --num-worlds 1024 --random-robots 16
     python evaluate.py --scenario random --policy tests/golden/checkpoints/stage2.pth --num-worlds 1024 --hybrid
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 --safety
+    python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3 \\
+        --timeouts
 """
 import argparse
 import json
@@ -35,8 +41,8 @@ import os
 
 import torch
 
-from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, SAFETY_COLUMNS, evaluate, \
-    non_cooperative_mask
+from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, PROGRESS_COLUMNS, PROGRESS_DEFAULTS, \
+    SAFETY_COLUMNS, evaluate, non_cooperative_mask
 from rl_collision_avoidance_b200.model.net import CNNPolicy
 from rl_collision_avoidance_b200.orca import HYBRID_DEFAULTS, Hybrid, NonCooperative, \
     add_arguments as add_controller_arguments, check_arguments as check_controller_arguments, check_hybrid, \
@@ -88,6 +94,12 @@ def main(argv=None):
                          '(DESIGN.md §9m)')
     ap.add_argument('--near-miss', type=float, default=None, metavar='D',
                     help='a tick closer than D m to another robot is a near miss (default 0.1); implies --safety')
+    ap.add_argument('--timeouts', action='store_true',
+                    help='also report why robots timed out or never finished: frozen, stalled or slow, with a robot '
+                         'near or not (DESIGN.md §9o)')
+    ap.add_argument('--stall-window', type=int, default=None, metavar='W',
+                    help='a robot still for W ticks is frozen, one without progress for W ticks stalled (default %d); '
+                         'implies --timeouts' % PROGRESS_DEFAULTS['window'])
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -111,6 +123,11 @@ def main(argv=None):
     if args.near_miss is not None and not (math.isfinite(args.near_miss) and args.near_miss >= 0.0):
         ap.error('--near-miss must be finite and >= 0')
     safety = args.near_miss if args.near_miss is not None else 0.1 if args.safety else None
+    if args.stall_window is not None and args.stall_window < 1:
+        ap.error('--stall-window must be >= 1')
+    progress = None
+    if args.timeouts or args.stall_window is not None:
+        progress = {} if args.stall_window is None else {'window': args.stall_window}
     hybrid_params = None
     if args.hybrid:
         hybrid_params = dict(HYBRID_DEFAULTS)
@@ -151,7 +168,7 @@ def main(argv=None):
                             speed=args.non_cooperative_speed)
     hy = Hybrid(env, **hybrid_params) if args.hybrid else None
     out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy,
-                   safety=safety)
+                   safety=safety, progress=progress)
 
     def line(m, robots, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -186,8 +203,25 @@ def main(argv=None):
         if nc is not None:
             safety_line(out['safety_by_role']['cooperative'], 'cooperative  ')
             safety_line(out['safety_by_role']['non_cooperative'], 'non-cooperative  ')
+
+    def progress_line(m, role=''):
+        f = lambda k: '%.3f +- %.3f' % m[k]
+        group = lambda g, name, n: ('%s %d: frozen %d  stalled %d  slow %d  robot near %d  closest %s m'
+                                    % (name, n, m[g + '_frozen'], m[g + '_stalled'], m[g + '_slow'],
+                                       m[g + '_robot_near'], f(g + '_closest')))
+        print('progress  %s%s  |  %s  |  still share %.4f  rotation per reached %s rad  (window %d ticks)'
+              % (role, group('timeout', 'time-outs', m['timeouts']), group('unfinished', 'unfinished', m['unfinished']),
+                 m['still_share'], f('rotation_reached'), out['progress_tracker'].params['window']))
+
+    if progress is not None:
+        progress_line(out['progress'])
+        if nc is not None:
+            progress_line(out['progress_by_role']['cooperative'], 'cooperative  ')
+            progress_line(out['progress_by_role']['non_cooperative'], 'non-cooperative  ')
     if args.json:
-        shown = {k: v for k, v in vars(args).items() if safety is not None or k not in ('safety', 'near_miss')}
+        hidden = (() if safety is not None else ('safety', 'near_miss')) + \
+            (() if progress is not None else ('timeouts', 'stall_window'))
+        shown = {k: v for k, v in vars(args).items() if k not in hidden}
         res = {'args': shown, 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
                'columns': list(COLUMNS), 'totals': out['totals'].tolist(),
@@ -204,6 +238,13 @@ def main(argv=None):
             if nc is not None:
                 res['safety']['by_role'] = out['safety_by_role']
                 res['safety']['partials_split'] = out['safety_partials_split'].tolist()
+        if progress is not None:
+            res['progress'] = {'params': out['progress_tracker'].params, 'metrics': out['progress'],
+                               'columns': list(PROGRESS_COLUMNS), 'totals': out['progress_totals'].tolist(),
+                               'partials': out['progress_partials'].tolist()}
+            if nc is not None:
+                res['progress']['by_role'] = out['progress_by_role']
+                res['progress']['partials_split'] = out['progress_partials_split'].tolist()
         with open(args.json, 'w') as fh:
             json.dump(res, fh, indent=1)
     return out

@@ -815,6 +815,102 @@ int rlca_safety_reduce_host(const rlca_env_config *cfg, const float *safety_reco
                             const float *eval_records_host, const int32_t *count_host, const uint8_t *role_mask_host,
                             int32_t episodes, int32_t world_begin, int32_t world_count, double *partials_host);
 
+/* =====================================================================================
+ * Progress metrics (csrc/rlca_progress.cu, DESIGN.md §9o): why robots time out or never finish, per episode of the
+ * evaluation tracker above.
+ *
+ * A tick of a tracked episode (closed != meta_in.y) is folded unless it re-spawned the robot (flags.w).  A folded tick
+ * takes d = pose_out.w (the distance to the goal the tick computed), the centre displacement
+ * s = |(x, y)_out - (x, y)_in| and the heading change |wrap(theta_out - theta_in)|, and keeps per running episode:
+ *   closest     the least d
+ *   reference   the first folded tick sets ref = d and since = 0; a later one with d <= ref - progress_dist sets
+ *               ref = d and since = 0, any other adds 1 to since (ticks since progress)
+ *   still       a tick with s < still_dist is still; run counts consecutive still ticks (0 after a moving tick),
+ *               still all still ticks of the episode
+ *   rotation    the sum of the heading changes, radians
+ *   near        another robot of the world, any, finished or parked included, had its centre strictly within
+ *               block_dist of this robot's at the poses the tick ended at, on the last folded tick
+ * Cause of an episode that ends with result 3 (time-out), and of an unfinished episode at the reduction:
+ * 1 frozen (run >= window), else 2 stalled (since >= window), else 3 slow; + 4 when near is set.
+ * ===================================================================================== */
+typedef struct rlca_progress_params {
+    int32_t window;              /* ticks; >= 1 */
+    float progress_dist;         /* metres; finite, >= 0 */
+    float still_dist;            /* metres per tick; finite, >= 0 */
+    float block_dist;            /* metres; finite, >= 0 */
+} rlca_progress_params;
+
+/* Per-agent state, N rows; the caller zeroes running and counters before the first tick it tracks (all zero = no
+ * folded tick yet: the next folded tick starts the episode's state).
+ *   running    (N, 4) float  closest, progress reference, rotation, near (0 or 1) of the running episode
+ *   counters   (N, 4) int32  ticks since progress, still run, still ticks, folded ticks of the running episode
+ *   records    (N, episodes, 4) float, slot for slot the tracker's records: closest, rotation, still ticks, folded
+ *              ticks (the counts held exactly below 2^24 ticks)
+ *   causes     (N, episodes) uint8: the cause of a record whose episode timed out, 0 for every other record */
+typedef struct rlca_progress_state {
+    float *running_dev;
+    int32_t *counters_dev;
+    float *records_dev;
+    uint8_t *causes_dev;
+    int32_t episodes;
+} rlca_progress_state;
+
+/* One launch after each rlca_env_step and BEFORE that tick's rlca_eval_track, with the same cfg, state buffers and
+ * io: reads the poses of state_in / state_out, the episode indices of state_in, io->flags_dev and the tracker's
+ * closed / count (never written), so a tick belongs to the episode the tracker assigns it to and a record goes into
+ * the slot the tracker fills next.  A tick that ends an episode writes the record (on a re-spawn tick from the state
+ * the previous tick left) and zeroes the running state, as does any re-spawn.  It reads and writes nothing
+ * rlca_safety_track does, so the two may run in either order.  RLCA_ERR_INVALID for a NULL pointer, robots_per_world
+ * outside 1..64, episodes < 1 or different from the tracker's, a distance not finite or < 0, window < 1. */
+int rlca_progress_track(const rlca_env_config *cfg, const rlca_progress_params *params,
+                        const rlca_env_state *state_in, const rlca_env_state *state_out, const rlca_step_io *io,
+                        const rlca_eval_state *ev, const rlca_progress_state *ps, void *stream);
+/* The same from HOST buffers (pose (N,4) float; meta (N,4) int32; flags (N,4) uint8; the rest as the device state) by
+ * serial loops over the same code; the outputs equal rlca_progress_track's bit for bit. */
+int rlca_progress_track_host(const rlca_env_config *cfg, const rlca_progress_params *params,
+                             const float *pose_in_host, const int32_t *meta_in_host, const float *pose_out_host,
+                             const uint8_t *flags_host, const int32_t *closed_host, const int32_t *count_host,
+                             int32_t episodes, float *running_host, int32_t *counters_host, float *records_host,
+                             uint8_t *causes_host);
+
+/* Per-world float64 partials of worlds [world_begin, world_begin + world_count), one thread per world in
+ * agent-then-record order, no atomics: partials_dev (world_count, RLCA_PROGRESS_NPARTIALS).  The tracker's state gives
+ * the number of records per agent, each record's result code and which agents are unfinished (fewer than `episodes`
+ * records and open); an unfinished episode is classified from the running state with params->window.  With
+ * role_mask_dev (N uint8) the partials are split as rlca_eval_reduce_split splits its own, partials_dev (world_count,
+ * 2, RLCA_PROGRESS_NPARTIALS): row 0 over the agents with mask 0, row 1 over the others.  Every column is a sum;
+ * totals add them in global world order. */
+#define RLCA_PROGRESS_TIMEOUT_FROZEN 0          /* time-outs with cause frozen */
+#define RLCA_PROGRESS_TIMEOUT_STALLED 1         /* ... stalled */
+#define RLCA_PROGRESS_TIMEOUT_SLOW 2            /* ... slow */
+#define RLCA_PROGRESS_TIMEOUT_ROBOT_NEAR 3      /* time-outs with robot near (+4) */
+#define RLCA_PROGRESS_TIMEOUT_FOLDED 4          /* time-outs with at least one folded tick: the next two are over these */
+#define RLCA_PROGRESS_TIMEOUT_SUM_CLOSEST 5     /* sum of closest */
+#define RLCA_PROGRESS_TIMEOUT_SUM_CLOSEST_SQ 6  /* sum of closest squared */
+#define RLCA_PROGRESS_UNFINISHED_FROZEN 7       /* the same seven over unfinished episodes */
+#define RLCA_PROGRESS_UNFINISHED_STALLED 8
+#define RLCA_PROGRESS_UNFINISHED_SLOW 9
+#define RLCA_PROGRESS_UNFINISHED_ROBOT_NEAR 10
+#define RLCA_PROGRESS_UNFINISHED_FOLDED 11
+#define RLCA_PROGRESS_UNFINISHED_SUM_CLOSEST 12
+#define RLCA_PROGRESS_UNFINISHED_SUM_CLOSEST_SQ 13
+#define RLCA_PROGRESS_SUM_STILL_TICKS 14        /* over every recorded episode: still ticks */
+#define RLCA_PROGRESS_SUM_TICKS 15              /* ... folded ticks */
+#define RLCA_PROGRESS_REACHED 16                /* recorded episodes that reached the goal */
+#define RLCA_PROGRESS_SUM_ROTATION 17           /* their rotation, radians */
+#define RLCA_PROGRESS_SUM_ROTATION_SQ 18        /* ... squared */
+#define RLCA_PROGRESS_NPARTIALS 19
+int rlca_progress_reduce(const rlca_env_config *cfg, const rlca_progress_params *params,
+                         const rlca_progress_state *ps, const rlca_eval_state *ev, const uint8_t *role_mask_dev,
+                         int32_t world_begin, int32_t world_count, double *partials_dev, void *stream);
+/* The same reduction from HOST buffers (no device needed; the code rlca_progress_reduce runs). */
+int rlca_progress_reduce_host(const rlca_env_config *cfg, const rlca_progress_params *params,
+                              const float *progress_records_host, const uint8_t *causes_host,
+                              const float *running_host, const int32_t *counters_host,
+                              const float *eval_records_host, const int32_t *count_host, const int32_t *open_host,
+                              const uint8_t *role_mask_host, int32_t episodes, int32_t world_begin,
+                              int32_t world_count, double *partials_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

@@ -85,6 +85,18 @@ class SafetyState(C.Structure):
                 ('episodes', C.c_int32)]
 
 
+class ProgressParams(C.Structure):
+    """Mirror of rlca_progress_params (include/rlca.h)."""
+    _fields_ = [('window', C.c_int32), ('progress_dist', C.c_float), ('still_dist', C.c_float),
+                ('block_dist', C.c_float)]
+
+
+class ProgressState(C.Structure):
+    """Mirror of rlca_progress_state (include/rlca.h)."""
+    _fields_ = [('running_dev', C.c_void_p), ('counters_dev', C.c_void_p), ('records_dev', C.c_void_p),
+                ('causes_dev', C.c_void_p), ('episodes', C.c_int32)]
+
+
 # rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
 EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
                  'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
@@ -94,6 +106,12 @@ EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 's
 SAFETY_PARTIALS = ('crash_static', 'crash_robot', 'crash_both_in_range', 'crash_into_masked', 'reached',
                    'reached_separation', 'sum_separation', 'sum_separation_sq', 'reached_clearance', 'sum_clearance',
                    'sum_clearance_sq', 'near_episodes', 'sum_near_ticks', 'min_separation')
+
+# rlca_progress_reduce partials per world (the RLCA_PROGRESS_* columns of include/rlca.h), all sums
+PROGRESS_PARTIALS = tuple(g + '_' + k for g in ('timeout', 'unfinished')
+                          for k in ('frozen', 'stalled', 'slow', 'robot_near', 'folded', 'sum_closest',
+                                    'sum_closest_sq')) + \
+    ('sum_still_ticks', 'sum_ticks', 'reached', 'sum_rotation', 'sum_rotation_sq')
 
 
 # every symbol include/rlca.h declares: (name, restype, argtypes)
@@ -203,6 +221,15 @@ SYMBOLS = {
     'rlca_safety_reduce': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(SafetyState), C.POINTER(EvalState), _P, C.c_int32,
                                      C.c_int32, _P, _P]),
     'rlca_safety_reduce_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
+    'rlca_progress_track': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(ProgressParams), C.POINTER(EnvState),
+                                      C.POINTER(EnvState), C.POINTER(StepIO), C.POINTER(EvalState),
+                                      C.POINTER(ProgressState), _P]),
+    'rlca_progress_track_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(ProgressParams), _P, _P, _P, _P, _P, _P,
+                                           C.c_int32, _P, _P, _P, _P]),
+    'rlca_progress_reduce': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(ProgressParams), C.POINTER(ProgressState),
+                                       C.POINTER(EvalState), _P, C.c_int32, C.c_int32, _P, _P]),
+    'rlca_progress_reduce_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(ProgressParams), _P, _P, _P, _P, _P, _P,
+                                            _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

@@ -25,6 +25,10 @@ COLUMNS = _lib.EVAL_PARTIALS
 NPARTIALS = len(COLUMNS)
 SAFETY_COLUMNS = _lib.SAFETY_PARTIALS
 SAFETY_NPARTIALS = len(SAFETY_COLUMNS)
+PROGRESS_COLUMNS = _lib.PROGRESS_PARTIALS
+PROGRESS_NPARTIALS = len(PROGRESS_COLUMNS)
+# DESIGN.md §9o: a third of stage 1's 150-tick budget; 10 cm of progress; 5 mm per tick (0.05 m/s at dt 0.1); 1 m
+PROGRESS_DEFAULTS = {'window': 50, 'progress_dist': 0.1, 'still_dist': 0.005, 'block_dist': 1.0}
 ACTION_BOUND = [[0, -1], [1, 1]]
 # the reference's episode mechanics per scenario: stage 1 re-spawns a robot as soon as it is done
 # (ppo_stage1.py:51-65), stage 2 re-spawns a group when all of it is done (ppo_stage2.py:49-106), circle runs one
@@ -280,6 +284,150 @@ def safety_metrics(tot):
     return out
 
 
+def progress_params(params=None):
+    """_lib.ProgressParams from a dict of any of PROGRESS_DEFAULTS' keys (the others take their defaults); ValueError
+    unless window is an integer >= 1 and the distances are finite and >= 0."""
+    p = dict(PROGRESS_DEFAULTS)
+    unknown = set(params or ()) - set(p)
+    if unknown:
+        raise ValueError(f'unknown progress parameters: {sorted(unknown)}')
+    p.update(params or {})
+    if int(p['window']) != p['window'] or int(p['window']) < 1:
+        raise ValueError('window must be an integer >= 1')
+    for k in ('progress_dist', 'still_dist', 'block_dist'):
+        if not (math.isfinite(float(p[k])) and float(p[k]) >= 0.0):
+            raise ValueError(f'{k} must be finite and >= 0')
+    return _lib.ProgressParams(int(p['window']), float(p['progress_dist']), float(p['still_dist']),
+                               float(p['block_dist']))
+
+
+class ProgressTracker:
+    """Per-episode progress records next to an EpisodeTracker's (DESIGN.md §9o): closest distance to the goal, ticks
+    since the last `progress_dist` of progress, still ticks (centre moved less than `still_dist`), rotation, whether
+    another robot stood within `block_dist`, and the cause of a time-out: frozen, stalled or slow, + 4 with a robot
+    near.  `params` is a dict of any of PROGRESS_DEFAULTS' keys.  Call `track()` after each `env.control_vel` and
+    BEFORE `tracker.track()`: the episode a tick belongs to and the record slot are read from the tracker's state as
+    its own call will see them."""
+
+    def __init__(self, env, tracker, params=None):
+        self._params = progress_params(params)
+        self.params = dict(PROGRESS_DEFAULTS, **(params or {}))
+        self.env, self.tracker = env, tracker
+        N, E, dev = env.N, tracker.episodes, env.device
+        self.running = torch.zeros(N, 4, device=dev)
+        self.counters = torch.zeros(N, 4, dtype=torch.int32, device=dev)
+        self.records = torch.zeros(N, E, 4, device=dev)
+        self.causes = torch.zeros(N, E, dtype=torch.uint8, device=dev)
+        self._st = _lib.ProgressState(_ptr(self.running), _ptr(self.counters), _ptr(self.records), _ptr(self.causes),
+                                      E)
+
+    def reset(self):
+        """Forget every record and the running episodes (with the tracker's own reset())."""
+        for t in (self.running, self.counters, self.records, self.causes):
+            t.zero_()
+
+    def track(self):
+        """Progress records of the tick `env.control_vel` just ran (same stream, no synchronisation)."""
+        env = self.env
+        if not env._ticked:
+            raise RuntimeError('ProgressTracker.track() needs a tick: call env.control_vel first')
+        s_in, s_out = env._state_struct(1 - env._cur), env._state_struct(env._cur)
+        io = env._io(action=env._keep[0], out=env._last_out)
+        _lib.check(env.lib.rlca_progress_track(C.byref(env.cfg), C.byref(self._params), C.byref(s_in),
+                                               C.byref(s_out), C.byref(io), C.byref(self.tracker._st),
+                                               C.byref(self._st), env._stream()))
+
+    def partials(self, world_begin=0, world_count=None, role_mask=None):
+        """(world_count, PROGRESS_NPARTIALS) float64 per-world partials, or (world_count, 2, PROGRESS_NPARTIALS) split
+        by the agent mask `role_mask` (N): row 0 over the agents with mask 0, row 1 over the others."""
+        env = self.env
+        wc = env.num_worlds - world_begin if world_count is None else int(world_count)
+        m = None
+        if role_mask is not None:
+            m = torch.as_tensor(role_mask, device=env.device).to(torch.uint8).contiguous()
+            if m.shape != (env.N,):
+                raise ValueError(f'role_mask must have ({env.N},) entries')
+        shape = (wc, PROGRESS_NPARTIALS) if m is None else (wc, 2, PROGRESS_NPARTIALS)
+        out = torch.empty(shape, dtype=torch.float64, device=env.device)
+        _lib.check(env.lib.rlca_progress_reduce(C.byref(env.cfg), C.byref(self._params), C.byref(self._st),
+                                                C.byref(self.tracker._st), _ptr(m), int(world_begin), wc, _ptr(out),
+                                                env._stream()))
+        return out.cpu().numpy()
+
+
+def progress_track_host(cfg, params, pose_in, meta_in, pose_out, flags, closed, count, state):
+    """rlca_progress_track on host arrays (the same code, run by the CPU).  `params` as ProgressTracker's; `state` is a
+    dict of running (N, 4) float32, counters (N, 4) int32, records (N, E, 4) float32 and causes (N, E) uint8, updated
+    in place."""
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    for k, dt in (('running', np.float32), ('counters', np.int32), ('records', np.float32), ('causes', np.uint8)):
+        if state[k].dtype != dt or not state[k].flags.c_contiguous:
+            raise ValueError(f'state[{k!r}] must be a contiguous {np.dtype(dt).name} array')
+    args = [np.ascontiguousarray(pose_in, np.float32), np.ascontiguousarray(meta_in, np.int32),
+            np.ascontiguousarray(pose_out, np.float32), np.ascontiguousarray(flags, np.uint8),
+            np.ascontiguousarray(closed, np.int32), np.ascontiguousarray(count, np.int32)]
+    _lib.check(_lib.load().rlca_progress_track_host(
+        C.byref(cfg), C.byref(progress_params(params)), *(vp(a) for a in args), state['records'].shape[1],
+        *(vp(state[k]) for k in ('running', 'counters', 'records', 'causes'))))
+    return state
+
+
+def progress_reduce_host(cfg, params, state, eval_records, count, open_, role_mask=None, world_begin=0,
+                         world_count=None):
+    """rlca_progress_reduce on host arrays (`state` as progress_track_host's; the tracker's records, count and open):
+    (world_count, PROGRESS_NPARTIALS), or (world_count, 2, ...) with a mask."""
+    vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
+    prec = np.ascontiguousarray(state['records'], np.float32)
+    causes = np.ascontiguousarray(state['causes'], np.uint8)
+    running = np.ascontiguousarray(state['running'], np.float32)
+    counters = np.ascontiguousarray(state['counters'], np.int32)
+    erec = np.ascontiguousarray(eval_records, np.float32)
+    cnt = np.ascontiguousarray(count, np.int32)
+    opn = np.ascontiguousarray(open_, np.int32)
+    msk = None if role_mask is None else np.ascontiguousarray(role_mask, np.uint8)
+    if msk is not None and msk.shape != cnt.shape:
+        raise ValueError('role_mask must have one entry per agent')
+    if prec.shape != erec.shape or causes.shape != prec.shape[:2]:
+        raise ValueError('the progress records, causes and the tracker records must have matching shapes')
+    wc = cfg.num_worlds - world_begin if world_count is None else int(world_count)
+    out = np.zeros((wc, PROGRESS_NPARTIALS) if msk is None else (wc, 2, PROGRESS_NPARTIALS), np.float64)
+    _lib.check(_lib.load().rlca_progress_reduce_host(
+        C.byref(cfg), C.byref(progress_params(params)), vp(prec), vp(causes), vp(running), vp(counters), vp(erec),
+        vp(cnt), vp(opn), vp(msk), prec.shape[1], int(world_begin), wc, vp(out)))
+    return out
+
+
+def progress_totals(partials):
+    """Per-world progress partials (rows in global world order) summed left to right: the same bits however the rows
+    were sharded."""
+    p = np.asarray(partials, np.float64).reshape(-1, PROGRESS_NPARTIALS)
+    tot = np.zeros(PROGRESS_NPARTIALS, np.float64)
+    for row in p:
+        tot = tot + row
+    return tot
+
+
+def progress_metrics(tot):
+    """For the time-outs and for the unfinished episodes: their number, the counts and shares of each cause (frozen,
+    stalled, slow) and of those with a robot near, and the mean and population std of the closest distance to the
+    goal (over those with a folded tick); the share of still ticks among all ticks of the recorded episodes; the mean
+    and std of the rotation of the episodes that reached the goal.  NaN where there is nothing to average."""
+    t = dict(zip(PROGRESS_COLUMNS, np.asarray(tot, np.float64).tolist()))
+    ms = lambda s, s2, n: (s / n, math.sqrt(max(s2 / n - (s / n) ** 2, 0.0))) if n else (math.nan, math.nan)
+    out = {}
+    for g, count in (('timeout', 'timeouts'), ('unfinished', 'unfinished')):
+        n = t[g + '_frozen'] + t[g + '_stalled'] + t[g + '_slow']
+        out[count] = int(n)
+        for k in ('frozen', 'stalled', 'slow', 'robot_near'):
+            out[g + '_' + k] = int(t[g + '_' + k])
+            out[g + '_' + k + '_share'] = t[g + '_' + k] / n if n else math.nan
+        out[g + '_closest'] = ms(t[g + '_sum_closest'], t[g + '_sum_closest_sq'], t[g + '_folded'])
+    out['still_share'] = t['sum_still_ticks'] / t['sum_ticks'] if t['sum_ticks'] else math.nan
+    out['reached'] = int(t['reached'])
+    out['rotation_reached'] = ms(t['sum_rotation'], t['sum_rotation_sq'], t['reached'])
+    return out
+
+
 def non_cooperative_mask(robots_per_world, num_worlds, k):
     """(robots_per_world * num_worlds,) uint8 with robots floor(j R / k), j < k, of every world set: k robots spread
     evenly round the circle table (DESIGN.md §9h).  ValueError unless 1 <= k <= R."""
@@ -323,7 +471,8 @@ def metrics(tot):
     return out
 
 
-def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None):
+def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None,
+             progress=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
@@ -348,7 +497,12 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     the result also holds 'safety_partials' (num_worlds, SAFETY_NPARTIALS), 'safety_totals', 'safety'
     (safety_metrics) and 'safety_tracker'; with `non_cooperative` also 'safety_partials_split' and 'safety_by_role',
     where the cooperative row's 'crash_into_masked' counts its crashes into a non-cooperative robot.  With None nothing
-    of this is allocated or launched."""
+    of this is allocated or launched.
+
+    With `progress` (a dict of any of PROGRESS_DEFAULTS' keys, {} for the defaults) a ProgressTracker runs before the
+    episode tracker on every tick and the result also holds 'progress_partials' (num_worlds, PROGRESS_NPARTIALS),
+    'progress_totals', 'progress' (progress_metrics) and 'progress_tracker'; with `non_cooperative` also
+    'progress_partials_split' and 'progress_by_role'.  With None nothing of this is allocated or launched."""
     E = int(episodes)
     if int(check_every) < 1:
         raise ValueError('check_every must be >= 1')
@@ -356,6 +510,7 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         raise ValueError('hybrid switches a policy; the ORCA baselines are not switched')
     tracker = EpisodeTracker(env, E)
     safe = SafetyTracker(env, tracker, safety) if safety is not None else None
+    prog = ProgressTracker(env, tracker, progress) if progress is not None else None
     N, dev = env.N, env.device
     circle = int(env.cfg.auto_reset) == 0
     env.reset_world()
@@ -388,6 +543,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         env.control_vel(scaled, stack_in=stacks[k], stack_out=stacks[1 - k])
         if safe is not None:
             safe.track()
+        if prog is not None:
+            prog.track()
         tracker.track()
         if circle:
             terminal = env.flags[:, 0] != 0
@@ -414,4 +571,13 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             out['safety_partials_split'] = ss
             out['safety_by_role'] = {'cooperative': safety_metrics(safety_totals(ss[:, 0])),
                                      'non_cooperative': safety_metrics(safety_totals(ss[:, 1]))}
+    if prog is not None:
+        pp = prog.partials()
+        out.update(progress_partials=pp, progress_totals=progress_totals(pp), progress_tracker=prog)
+        out['progress'] = progress_metrics(out['progress_totals'])
+        if non_cooperative is not None:
+            ps = prog.partials(role_mask=non_cooperative.mask)
+            out['progress_partials_split'] = ps
+            out['progress_by_role'] = {'cooperative': progress_metrics(progress_totals(ps[:, 0])),
+                                       'non_cooperative': progress_metrics(progress_totals(ps[:, 1]))}
     return out
