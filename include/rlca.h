@@ -216,6 +216,9 @@ int rlca_env_set_host_zero_copy(rlca_env *env, int32_t mode);
 int rlca_env_set_ctas_per_world(rlca_env *env, int32_t ctas_per_world);
 /* Number of kernels the library launched on behalf of this handle so far. */
 int64_t rlca_env_launch_count(const rlca_env *env);
+/* Small maps: CTAs of the tick's lidar launch that one SM holds at once (its shared memory and registers at the
+ * map's tables); 0 for a big map.  The launch is sized for 8. */
+int rlca_env_lidar_ctas_per_sm(const rlca_env *env, int32_t *ctas);
 
 
 /* =====================================================================================

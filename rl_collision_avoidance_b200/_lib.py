@@ -133,6 +133,7 @@ SYMBOLS = {
     'rlca_env_set_host_chunks': (C.c_int, [_P, C.c_int32]),
     'rlca_env_set_host_zero_copy': (C.c_int, [_P, C.c_int32]),
     'rlca_env_launch_count': (C.c_int64, [_P]),
+    'rlca_env_lidar_ctas_per_sm': (C.c_int, [_P, C.POINTER(C.c_int32)]),
     'rlca_sizeof_env_config': (C.c_int, []),
     'rlca_policy_param_offset': (C.c_int64, [C.c_int32]),
     'rlca_policy_param_size': (C.c_int64, [C.c_int32]),
