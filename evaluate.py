@@ -18,7 +18,10 @@ than --near-miss D m (default 0.1) to another robot (DESIGN.md §9m).  --timeout
 finished: each time-out and each unfinished episode is called frozen (its centre has not moved for --stall-window W
 ticks, default 50), stalled (it moves but has not come 0.1 m closer to its goal in W ticks) or slow (still getting
 closer), and marked when another robot stood within 1 m; with the closest distance to the goal left, the share of
-still ticks and the rotation per successful episode (DESIGN.md §9o).
+still ticks and the rotation per successful episode (DESIGN.md §9o).  --scan-noise SIGMA_M, --beam-dropout P and
+--action-noise SIGMA_V[,SIGMA_W] evaluate under sensor and actuation noise: Gaussian range error on every beam with a
+return, beams that read no return, and a relative gain error on the executed v and w, drawn from --noise-seed
+(default --seed; DESIGN.md §9p).  The ORCA baselines do not read the scan, so only --action-noise applies to them.
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -33,6 +36,8 @@ still ticks and the rotation per successful episode (DESIGN.md §9o).
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 --safety
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3 \\
         --timeouts
+    python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
+        --scan-noise 0.05 --beam-dropout 0.1 --action-noise 0.1
 """
 import argparse
 import json
@@ -44,6 +49,7 @@ import torch
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, PROGRESS_COLUMNS, PROGRESS_DEFAULTS, \
     SAFETY_COLUMNS, evaluate, non_cooperative_mask
 from rl_collision_avoidance_b200.model.net import CNNPolicy
+from rl_collision_avoidance_b200.noise import NOISE_FLAGS, Noise, add_noise_arguments, noise_from_arguments
 from rl_collision_avoidance_b200.orca import HYBRID_DEFAULTS, Hybrid, NonCooperative, \
     add_arguments as add_controller_arguments, check_arguments as check_controller_arguments, check_hybrid, \
     from_arguments as controller_from_arguments
@@ -100,6 +106,7 @@ def main(argv=None):
     ap.add_argument('--stall-window', type=int, default=None, metavar='W',
                     help='a robot still for W ticks is frozen, one without progress for W ticks stalled (default %d); '
                          'implies --timeouts' % PROGRESS_DEFAULTS['window'])
+    add_noise_arguments(ap)
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -128,6 +135,9 @@ def main(argv=None):
     progress = None
     if args.timeouts or args.stall_window is not None:
         progress = {} if args.stall_window is None else {'window': args.stall_window}
+    if args.baseline is not None and (args.scan_noise is not None or args.beam_dropout is not None):
+        ap.error('--scan-noise / --beam-dropout apply to --policy only: the ORCA baselines do not read the scan')
+    noise_params = noise_from_arguments(ap, args)
     hybrid_params = None
     if args.hybrid:
         hybrid_params = dict(HYBRID_DEFAULTS)
@@ -167,8 +177,9 @@ def main(argv=None):
         nc = NonCooperative(env, non_cooperative_mask(sc.robots_per_world, args.num_worlds, args.non_cooperative),
                             speed=args.non_cooperative_speed)
     hy = Hybrid(env, **hybrid_params) if args.hybrid else None
+    noise = Noise(env, noise_params) if noise_params is not None else None
     out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy,
-                   safety=safety, progress=progress)
+                   safety=safety, progress=progress, noise=noise)
 
     def line(m, robots, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -179,6 +190,10 @@ def main(argv=None):
                  m['timeout_rate'], m['unfinished'], f('extra_time'), f('extra_distance'), f('average_speed')))
 
     m = out['metrics']
+    if noise is not None:
+        ns = out['noise']
+        print('noise  range sigma %g m  beam dropout %g  v gain sigma %g  w gain sigma %g  seed %d'
+              % (ns['range_sigma'], ns['dropout'], ns['v_gain_sigma'], ns['w_gain_sigma'], ns['seed']))
     line(m, env.N)
     if nc is not None:
         k = args.non_cooperative * args.num_worlds
@@ -220,12 +235,15 @@ def main(argv=None):
             progress_line(out['progress_by_role']['non_cooperative'], 'non-cooperative  ')
     if args.json:
         hidden = (() if safety is not None else ('safety', 'near_miss')) + \
-            (() if progress is not None else ('timeouts', 'stall_window'))
+            (() if progress is not None else ('timeouts', 'stall_window')) + \
+            (() if noise is not None else tuple(f[2:].replace('-', '_') for f in NOISE_FLAGS))
         shown = {k: v for k, v in vars(args).items() if k not in hidden}
         res = {'args': shown, 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
                'columns': list(COLUMNS), 'totals': out['totals'].tolist(),
                'partials': out['partials'].tolist()}
+        if noise is not None:
+            res['noise'] = out['noise']
         if nc is not None:
             res['by_role'] = out['by_role']
             res['partials_split'] = out['partials_split'].tolist()

@@ -914,6 +914,55 @@ int rlca_progress_reduce_host(const rlca_env_config *cfg, const rlca_progress_pa
                               const uint8_t *role_mask_host, int32_t episodes, int32_t world_begin,
                               int32_t world_count, double *partials_host);
 
+/* =====================================================================================
+ * Sensor and actuation noise (csrc/rlca_noise.cu, DESIGN.md §9p): separate launches around the tick, issued only when
+ * a run asks for noise; the tick itself and its outputs are untouched.
+ *
+ * Draws: Philox-4x32-10 under the key (seed lo, seed hi) of the counter
+ *   (global agent = (world_offset + w) R + r, draw, element group, purpose | stream_id << 8)
+ * with purposes 0xE1 range noise, 0xE2 dropout, 0xE3 action noise (one byte, so that no stream id shifted by 8 can
+ * overlap them; the environment uses 1-5, the sampler 0x5A17).  `draw` is the caller's tick counter; `stream_id` tells
+ * apart several env handles of one run (a mix component's index).  A uniform is the top 24 bits of a word times
+ * 2^-24; a normal pair is Box-Muller on the words (w0, w1) or (w2, w3): u1 = ((w >> 8) + 1) 2^-24 in (0, 1],
+ * u2 = (w >> 8) 2^-24, z = sqrt(-2 ln u1) (cos, sin)(2 pi u2), with the contract ln / sin / cos of rlca_common.cuh.
+ * No draw depends on num_worlds, the launch shape or anything but the key and the counter.
+ *
+ * Scan (the newest frame of an (N, 3, beams) observation stack, normalised o = r / 6 - 0.5): element group g holds
+ * beams 4g .. 4g + 3, one Philox call per group and purpose.  Per beam, r = (o + 0.5) range_max:
+ *   dropout     u < dropout (float32 compare): the beam reads range_max (no return)
+ *   range noise otherwise, a beam with a return (r < range_max) and range_sigma > 0 gets
+ *               r' = clamp(fma(range_sigma, z, r), 0, range_max), written back as fma(r', 1/6, -0.5); a beam without a
+ *               return stays as it is, so noise never makes a return
+ * Action (N, 2): clip (v, w) to [v_min, v_max] x [w_min, w_max], multiply by max(fma(sigma, z, 1), 0) (z from group 0,
+ * purpose 0xE3: z1 for v, z2 for w), clip again.  A gain never reverses a command, and a zero command stays zero.
+ * ===================================================================================== */
+typedef struct rlca_noise_params {
+    float range_sigma;           /* metres; finite, >= 0 */
+    float dropout;               /* probability a beam reads no return; in [0, 1] */
+    float v_gain_sigma;          /* relative; finite, >= 0 */
+    float w_gain_sigma;          /* relative; finite, >= 0 */
+    uint64_t seed;
+    uint32_t stream_id;          /* < 2^24 */
+} rlca_noise_params;
+
+/* In place on stack_dev (N, 3, beams) float, after a tick: perturbs the newest frame (slot 2) of every row, the two
+ * older frames having been perturbed when they were newest.  A row whose flags_dev[4 a + 3] (was_reset) is set gets the
+ * perturbed frame in all three slots, as the tick gives a re-spawned row three copies of its scan; flags_dev NULL means
+ * every row is fresh (the first stack after a reset).  RLCA_ERR_INVALID for a NULL cfg, params or stack,
+ * robots_per_world outside 1..64, num_worlds or beams < 1, world_offset < 0, a sigma negative or not finite, dropout
+ * outside [0, 1] or stream_id >= 2^24. */
+int rlca_noise_scan(const rlca_env_config *cfg, const rlca_noise_params *p, uint32_t draw,
+                    const unsigned char *flags_dev, float *stack_dev, void *stream);
+/* Before a tick: the command the robots execute, action_out_dev (N, 2), from the command action_in_dev (N, 2), which is
+ * never written.  The same argument checks, and action_in_dev / action_out_dev not NULL. */
+int rlca_noise_action(const rlca_env_config *cfg, const rlca_noise_params *p, uint32_t draw,
+                      const float *action_in_dev, float *action_out_dev, void *stream);
+/* The same from HOST buffers by serial loops over the same code; the outputs equal the kernels' bit for bit. */
+int rlca_noise_scan_host(const rlca_env_config *cfg, const rlca_noise_params *p, uint32_t draw,
+                         const unsigned char *flags_host, float *stack_host);
+int rlca_noise_action_host(const rlca_env_config *cfg, const rlca_noise_params *p, uint32_t draw,
+                           const float *action_in_host, float *action_out_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

@@ -5,7 +5,8 @@ Same hyper-parameters, log files and checkpoint names; `mpiexec -np 24` is repla
     python ppo_stage1.py --num-worlds 43                       # 1 GPU, 43 x 24 = 1032 robots
     torchrun --nproc-per-node 8 --master-addr 127.0.0.1 ppo_stage1.py --num-worlds 43
 Fine-tuning on random layouts (DESIGN.md §9k) runs through ppo_stage2.py --scenario random, and on a mix of scenarios
-(DESIGN.md §9l) through ppo_stage2.py --mix.
+(DESIGN.md §9l) through ppo_stage2.py --mix.  --scan-noise SIGMA_M, --beam-dropout P and --action-noise SIGMA_V[,SIGMA_W]
+train under lidar and actuation noise (DESIGN.md §9p), with any scenario or mix.
 """
 import argparse
 import logging
@@ -19,6 +20,7 @@ from rl_collision_avoidance_b200.mix import MIX_AUTO_RESET, parse_mix, plan
 from rl_collision_avoidance_b200.model.diagnostics import check_target_kl, setup_diag_log
 from rl_collision_avoidance_b200.model.net import Adam, CNNPolicy
 from rl_collision_avoidance_b200.model.ppo import setup_ppo_log
+from rl_collision_avoidance_b200.noise import add_noise_arguments, noise_from_arguments
 from rl_collision_avoidance_b200.scenarios import add_random_arguments, check_random_arguments, \
     random_scenario_from_arguments
 from rl_collision_avoidance_b200.stage_world import StageWorld as RandomWorld
@@ -112,7 +114,9 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
                     help='skip the remaining epochs of an update once an epoch moved the policy by more than X '
                          '(approx_kl_k3; finite and > 0; implies --diagnostics)')
     add_random_arguments(ap, timeout=True)
+    add_noise_arguments(ap)
     args = ap.parse_args(argv)
+    noise = noise_from_arguments(ap, args)
     if args.target_kl is not None:
         try:
             args.target_kl = check_target_kl(args.target_kl)
@@ -210,7 +214,7 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     try:
         stats = run(env=env, policy=policy, policy_path=args.policy_path, action_bound=action_bound, optimizer=opt, hp=hp,
                     logger=logger, logger_cal=logger_cal, stage=stage, max_updates=args.updates, process_group=pg, rank=rank,
-                    start_update=start_update, diagnostics=args.diagnostics, target_kl=args.target_kl)
+                    start_update=start_update, diagnostics=args.diagnostics, target_kl=args.target_kl, noise=noise)
         if rank == 0 and stats:
             s = stats[-1]
             print('update %d: rollout %.3fs update %.3fs -> %.0f agent-steps/s per GPU; mean ep reward %.2f' %

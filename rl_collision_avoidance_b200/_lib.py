@@ -97,6 +97,12 @@ class ProgressState(C.Structure):
                 ('causes_dev', C.c_void_p), ('episodes', C.c_int32)]
 
 
+class NoiseParams(C.Structure):
+    """Mirror of rlca_noise_params (include/rlca.h)."""
+    _fields_ = [('range_sigma', C.c_float), ('dropout', C.c_float), ('v_gain_sigma', C.c_float),
+                ('w_gain_sigma', C.c_float), ('seed', C.c_uint64), ('stream_id', C.c_uint32)]
+
+
 # rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
 EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
                  'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
@@ -231,6 +237,10 @@ SYMBOLS = {
                                        C.POINTER(EvalState), _P, C.c_int32, C.c_int32, _P, _P]),
     'rlca_progress_reduce_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(ProgressParams), _P, _P, _P, _P, _P, _P,
                                             _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
+    'rlca_noise_scan': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(NoiseParams), C.c_uint32, _P, _P, _P]),
+    'rlca_noise_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(NoiseParams), C.c_uint32, _P, _P, _P]),
+    'rlca_noise_scan_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(NoiseParams), C.c_uint32, _P, _P]),
+    'rlca_noise_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(NoiseParams), C.c_uint32, _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

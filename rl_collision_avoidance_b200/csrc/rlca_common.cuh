@@ -115,3 +115,40 @@ __host__ __device__ __forceinline__ float dev_atan2f(float y, float x)
     if (x < 0.0f) a = pi - a;
     return y < 0.0f ? -a : a;
 }
+
+// natural logarithm of a positive normal x under the same contract: the cephes logf polynomial on the mantissa reduced
+// to [sqrt(1/2), sqrt(2)), explicit FMAs only, so host and device round alike (about 1 ulp from the exact value).
+#include <string.h>
+__host__ __device__ __forceinline__ float dev_logf(float x)
+{
+    uint32_t b;
+#ifdef __CUDA_ARCH__
+    b = __float_as_uint(x);
+#else
+    memcpy(&b, &x, sizeof(b));
+#endif
+    int e = (int)(b >> 23) - 127;
+    b = (b & 0x007FFFFFu) | 0x3F800000u;
+    float m;
+#ifdef __CUDA_ARCH__
+    m = __uint_as_float(b);
+#else
+    memcpy(&m, &b, sizeof(m));
+#endif
+    if (m > 1.41421356237309505f) {
+        m *= 0.5f;
+        e += 1;
+    }
+    const float f = m - 1.0f, z = f * f, fe = (float)e;
+    float p = fmaf(7.0376836292e-2f, f, -1.1514610310e-1f);
+    p = fmaf(p, f, 1.1676998740e-1f);
+    p = fmaf(p, f, -1.2420140846e-1f);
+    p = fmaf(p, f, 1.4249322787e-1f);
+    p = fmaf(p, f, -1.6668057665e-1f);
+    p = fmaf(p, f, 2.0000714765e-1f);
+    p = fmaf(p, f, -2.4999993993e-1f);
+    p = fmaf(p, f, 3.3333331174e-1f);
+    float y = fmaf(p * f, z, fe * -2.12194440e-4f);
+    y = fmaf(-0.5f, z, y);
+    return fmaf(fe, 0.693359375f, f + y);
+}

@@ -472,7 +472,7 @@ def metrics(tot):
 
 
 def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None,
-             progress=None):
+             progress=None, noise=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
@@ -502,12 +502,23 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     With `progress` (a dict of any of PROGRESS_DEFAULTS' keys, {} for the defaults) a ProgressTracker runs before the
     episode tracker on every tick and the result also holds 'progress_partials' (num_worlds, PROGRESS_NPARTIALS),
     'progress_totals', 'progress' (progress_metrics) and 'progress_tracker'; with `non_cooperative` also
-    'progress_partials_split' and 'progress_by_role'.  With None nothing of this is allocated or launched."""
+    'progress_partials_split' and 'progress_by_role'.  With None nothing of this is allocated or launched.
+
+    With `noise` (a noise.Noise on `env`, DESIGN.md §9p) the robots sense and act under noise: the first stack and,
+    after every tick, the stack the tick wrote get `noise.scan` (with env.flags), and the command, after the
+    non-cooperative override and the circle rule, becomes `noise.action`'s executed command before control_vel.
+    env.obs, env.gs and the state are never perturbed, so the trackers keep measuring the true scan and poses.  The
+    result then also holds 'noise' (the settings).  Scan noise needs a policy: the ORCA baselines do not read the scan."""
     E = int(episodes)
     if int(check_every) < 1:
         raise ValueError('check_every must be >= 1')
     if hybrid is not None and isinstance(policy, (OrcaController, NhOrcaController)):
         raise ValueError('hybrid switches a policy; the ORCA baselines are not switched')
+    if noise is not None:
+        if noise.env is not env:
+            raise ValueError('the noise belongs to another env')
+        if noise.params.scan_on and isinstance(policy, (OrcaController, NhOrcaController)):
+            raise ValueError('scan noise perturbs what a policy reads; the ORCA baselines do not read the scan')
     tracker = EpisodeTracker(env, E)
     safe = SafetyTracker(env, tracker, safety) if safety is not None else None
     prog = ProgressTracker(env, tracker, progress) if progress is not None else None
@@ -523,6 +534,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         hybrid.reset()
     obs = env.get_laser_observation()
     stacks = [obs[:, None, :].repeat(1, 3, 1).contiguous(), torch.empty(N, 3, env.beam_mum, device=dev)]
+    if noise is not None:
+        noise.scan(stacks[0])
     terminal = torch.zeros(N, dtype=torch.bool, device=dev)
     goal_done = 1 if circle else E
     ticks = 0
@@ -540,7 +553,11 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             non_cooperative.apply(scaled)
         if circle:
             scaled = torch.stack((torch.where(terminal, 0.0, scaled[:, 0]), scaled[:, 1]), 1)
+        if noise is not None:
+            scaled = noise.action(scaled)
         env.control_vel(scaled, stack_in=stacks[k], stack_out=stacks[1 - k])
+        if noise is not None:
+            noise.scan(stacks[1 - k], env.flags)
         if safe is not None:
             safe.track()
         if prog is not None:
@@ -580,4 +597,6 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             out['progress_partials_split'] = ps
             out['progress_by_role'] = {'cooperative': progress_metrics(progress_totals(ps[:, 0])),
                                        'non_cooperative': progress_metrics(progress_totals(ps[:, 1]))}
+    if noise is not None:
+        out['noise'] = noise.settings()
     return out
