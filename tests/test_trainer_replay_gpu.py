@@ -1,0 +1,640 @@
+"""trainer.run replayed on the host: two PPO updates of the unmodified trainer, recorded through wrappers of the names
+trainer imports and of the optimizer instance, then every update replayed against independent references.
+
+a. The environment, bit for bit: one CPU oracle per component, driven by the executed commands, with the scan deque of
+   tests/trainer_ref.py, the re-layout host twin (random layouts) and the noise host twins.  Stacks, goal | speed,
+   rewards, flags and the eplog rows of ended episodes equal the device rollout's.
+b. The policy per tick, at the weights of the update's start: values against the float64 forward within
+   learner_ref.check_forward's bound for the tensor-core mode, means within the bound at _forward64; actions,
+   log-probabilities and the clip against sample_ref (test_sample_gpu's bounds); the stored action is the sampled,
+   un-noised one; last_v is the float64 value of the replayed state after the horizon.
+c. The update: GAE targets and advantages against the float64 recurrence on the replayed rewards and dones (1 float32
+   ulp, test_learner_shapes_gpu.test_gae_vs_float64_recurrence); filter_index exactly; the epochs' permutations drawn
+   again from the generator state at entry give the restated minibatch schedule (a ragged last minibatch in stage 1,
+   the tail dropped in stage 2); then per optimizer step, teacher-forced from the device's parameters at that step, on
+   the rows of the replayed minibatch with the restated advantage normalisation (before np.delete): the ppo.log row
+   against learner_ref.ref_losses, all 23 gradients against float64 autograd relative to their layer's scale, and the
+   Adam step against trainer_ref.adam_step in float64 from the device's gradient (bounds at step_checks and
+   adam_bounds).  Every replayed PPO ratio is asserted to be learner_ref.MARGIN away from 1 +- clip.
+d. The Env log lines against the replay's own episode bookkeeping.
+
+Real rollouts are not decisive batches (learner_ref): a pre-activation within fp32 rounding of zero can flip its ReLU
+mask between the kernels and float64, which moves that tower's gradients by ~1e-3 of their scale.  A tower's tensors are
+therefore held to test_learner_gpu's bound for undecided conv masks, 3e-3 of the layer scale, in a minibatch where one
+of its conv pre-activations is within learner_ref.MARGIN of its layer's max of zero in float64.  An undecided fc1 / fc2
+mask moves its row's whole contribution, so that side's tensors may also differ by twice the float64 gradient of the
+rows holding one.  Elsewhere the tight bounds hold.
+"""
+import dataclasses
+import logging
+import math
+import os
+import time
+
+import numpy as np
+import pytest
+import torch
+
+import sample_ref
+import trainer_ref as ref
+from learner_ref import (CLIP, COEFF, MARGIN, VCOEF, Checks, layer_scale, maxabs, ref_forward, ref_logprob, ref_losses)
+from test_sample_gpu import action_bound, lp_bound
+
+pytestmark = pytest.mark.gpu
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CKPT = os.path.join(ROOT, 'tests', 'golden', 'checkpoints')
+U = 2.0 ** -24
+NOISE = dict(range_sigma=0.05, dropout=0.1, v_gain_sigma=0.2, w_gain_sigma=0.2, seed=2 ** 33 + 5)
+LR = 5e-5
+B1, B2 = float(np.float32(0.9)), float(np.float32(0.999))      # the betas as the fused Adam kernel receives them
+TINY = 2.0 ** -148        # two float32 subnormal steps: the absolute floor of a rounding near zero
+
+# (scenario, worlds, auto_reset, timeout, extra make_scenario arguments) per component
+CASES = {
+    # 2 x 24 robots; episodes time out after 20 ticks, so the first ones end on tick 19 and 39 = the horizon's last;
+    # H N = 1920 is 7.5 minibatches of 256: a ragged last minibatch
+    'stage1': dict(stage=1, comps=[('stage1', 2, 1, 19, {})], H=40, batch=256, ckpt='stage1_2.pth', noise=False),
+    # one stage-2 world with a 25-tick time-out: every group re-spawns inside the horizon, early finishers idle
+    'stage2': dict(stage=2, comps=[('stage2', 1, 2, 25, {})], H=52, batch=256, ckpt='stage2.pth', noise=False),
+    # random layouts under noise: a re-laid row's stack is refreshed before it is perturbed
+    'random': dict(stage=2, comps=[('random', 8, 0, 25, dict(robots_per_world=8, side=6.0))], H=52, batch=128,
+                   ckpt='stage2.pth', noise=True),
+    # stage 2 | circle | random in mix.MIX_SCENARIOS order; the stage-2 groups end together on tick 51 = H - 1, and
+    # circle and random robots that finished early idle on update 2's first tick: filter runs cross the boundaries
+    'mix': dict(stage=2, comps=[('stage2', 1, 2, 25, {}), ('circle', 2, 2, 100, dict(robots_per_world=8, radius=1.5)),
+                                ('random', 4, 0, 60, dict(robots_per_world=8, side=6.0))],
+                H=52, batch=256, ckpt='stage2.pth', noise=False),
+    'noise': dict(stage=1, comps=[('stage1', 2, 1, 19, {})], H=40, batch=256, ckpt='stage1_2.pth', noise=True),
+}
+SEED = 3
+
+
+def _scenario(name, timeout, extra):
+    from rl_collision_avoidance_b200.scenarios import make_scenario
+    sc = make_scenario(name, **extra)
+    return dataclasses.replace(sc, timeout=timeout)
+
+
+class _Lines(logging.Handler):
+    def __init__(self):
+        super().__init__()
+        self.records = []
+
+    def emit(self, record):
+        self.records.append(record.msg if not isinstance(record.msg, str) else record.getMessage())
+
+
+def _np(t):
+    return t.detach().cpu().numpy().copy()
+
+
+# ------------------------------------------------------------------------------------------------ recording
+class Recorder:
+    def __init__(self, monkeypatch, policy, optimizer, generator):
+        from rl_collision_avoidance_b200 import noise as noise_mod
+        from rl_collision_avoidance_b200 import trainer
+        self.policy, self.opt, self.gen = policy, optimizer, generator
+        self.ticks, self.fv, self.noise_cmds, self.gtd, self.updates = [], [], [], [], []
+        self.ro = self.comps = None
+        rec = self
+
+        compose0 = trainer.compose
+
+        def compose(envs, ro, noise=None):
+            rec.ro = ro
+            rec.comps = compose0(envs, ro, noise)
+            return rec.comps
+        monkeypatch.setattr(trainer, 'compose', compose)
+
+        fv0 = policy.forward_values
+
+        def forward_values(x, gs, v_out=None, mean_out=None):
+            v, mean = fv0(x, gs, v_out, mean_out)
+            rec.fv.append((x.data_ptr(), v.clone(), mean.clone()))
+            return v, mean
+        monkeypatch.setattr(policy, 'forward_values', forward_values)
+
+        ga0 = trainer.generate_action
+
+        def generate_action(env, state_list, policy, action_bound, out=None):
+            r = ga0(env=env, state_list=state_list, policy=policy, action_bound=action_bound, out=out)
+            slot = (state_list[0].data_ptr() - rec.ro.stacks.data_ptr()) // rec.ro.stacks[0].nbytes
+            rec.ticks.append(dict(slot=slot, seed=policy.sample_seed, counter=policy.sample_counter,
+                                  mean=rec.fv[-1][2], scaled=r[3].clone()))
+            return r
+        monkeypatch.setattr(trainer, 'generate_action', generate_action)
+
+        act0 = noise_mod.Noise.action
+
+        def action(self_, scaled):
+            draw = self_.action_draws
+            out = act0(self_, scaled)
+            rec.noise_cmds.append((self_.stream_id, draw, scaled.clone(), out.clone()))
+            return out
+        monkeypatch.setattr(noise_mod.Noise, 'action', action)
+
+        gtd0 = trainer.generate_train_data
+
+        def generate_train_data(rewards, gamma, values, last_value, dones, lam):
+            tg, adv = gtd0(rewards=rewards, gamma=gamma, values=values, last_value=last_value, dones=dones, lam=lam)
+            rec.gtd.append(dict(rewards=_np(rewards), values=_np(values), last_value=_np(last_value), dones=_np(dones),
+                                gamma=gamma, lam=lam, targets=_np(tg), advs=_np(adv)))
+            return tg, adv
+        monkeypatch.setattr(trainer, 'generate_train_data', generate_train_data)
+
+        def wrap_update(f0):
+            def update(**kw):
+                ro = rec.ro
+                u = dict(snap={k: _np(getattr(ro, k)) for k in ('stacks', 'gs', 'actions', 'logprobs', 'values',
+                                                                 'rewards', 'flags', 'eplog')},
+                         filter_index=list(kw.get('filter_index') or []), flat=rec.policy.flat.clone(),
+                         m=rec.opt.exp_avg.clone(), v=rec.opt.exp_avg_sq.clone(), steps=[],
+                         gen_state=rec.gen.get_state(), step_count=rec.opt.step_count,
+                         ticks=rec.ticks[-ro.actions.shape[0]:])
+                rec.updates.append(u)
+                u['rows'] = f0(**kw)
+                return u['rows']
+            return update
+        monkeypatch.setattr(trainer, 'ppo_update_stage1', wrap_update(trainer.ppo_update_stage1))
+        monkeypatch.setattr(trainer, 'ppo_update_stage2', wrap_update(trainer.ppo_update_stage2))
+
+        step0 = optimizer.step
+
+        def step(grad_scale=1.0):
+            p = rec.policy
+            before = dict(p=p.flat.clone(), g=p.grad.clone(), m=optimizer.exp_avg.clone(),
+                          v=optimizer.exp_avg_sq.clone(),
+                          t=optimizer.step_count + 1, grad_scale=grad_scale)
+            step0(grad_scale=grad_scale)
+            before.update(p1=p.flat.clone(), m1=optimizer.exp_avg.clone(), v1=optimizer.exp_avg_sq.clone())
+            rec.updates[-1]['steps'].append(before)
+        monkeypatch.setattr(optimizer, 'step', step)
+
+
+def _train(case, monkeypatch):
+    from rl_collision_avoidance_b200.model.net import Adam, CNNPolicy
+    from rl_collision_avoidance_b200.noise import NoiseParams
+    from rl_collision_avoidance_b200.stage_world import StageWorld
+    from rl_collision_avoidance_b200.trainer import run
+    c = CASES[case]
+    envs, scs = [], []
+    for name, W, ar, timeout, extra in c['comps']:
+        sc = _scenario(name, timeout, extra)
+        scs.append((sc, W, ar))
+        envs.append(StageWorld(512, scenario=sc, num_worlds=W, seed=SEED, auto_reset=ar))
+    N = sum(e.N for e in envs)
+    policy = CNNPolicy(frames=3, action_space=2, seed=SEED, max_batch=max(c['batch'], N))
+    policy.load_state_dict(torch.load(os.path.join(CKPT, c['ckpt']), map_location='cuda'))
+    opt = Adam(policy.parameters(), lr=LR)
+    gen = torch.Generator(device='cuda').manual_seed(SEED)
+    hp = dict(HORIZON=c['H'], GAMMA=0.99, LAMDA=0.95, BATCH_SIZE=c['batch'], EPOCH=2, COEFF_ENTROPY=COEFF,
+              CLIP_VALUE=CLIP, NUM_ENV=N, OBS_SIZE=512, ACT_SIZE=2, LASER_HIST=3, MAX_EPISODES=5000)
+    noise = NoiseParams(**NOISE) if c['noise'] else None
+    rec = Recorder(monkeypatch, policy, opt, gen)
+    lg, lc = logging.getLogger(f'replay_{case}'), logging.getLogger(f'replay_cal_{case}')
+    hl, hc = _Lines(), _Lines()
+    for l, h in ((lg, hl), (lc, hc)):
+        l.setLevel(logging.INFO)
+        l.propagate = False
+        l.addHandler(h)
+    try:
+        run(env=envs if len(envs) > 1 else envs[0], policy=policy, policy_path=None, action_bound=[[0, -1], [1, 1]],
+            optimizer=opt, hp=hp, logger=lg, logger_cal=lc, stage=c['stage'], max_updates=2, generator=gen,
+            noise=noise)
+    finally:
+        lg.removeHandler(hl)
+        lc.removeHandler(hc)
+    torch.cuda.synchronize()
+    return rec, envs, scs, noise, hl.records, hc.records
+
+
+# ------------------------------------------------------------------------------------------------ a. environment
+class OracleComponent:
+    """The CPU oracle of one component, the restated scan deque and the episode bookkeeping of its robots."""
+
+    def __init__(self, k, comp, sc, W, ar, noise):
+        from oracle.oracle import OracleWorld, OrcConfig
+        from rl_collision_avoidance_b200.noise import scan_host
+        from rl_collision_avoidance_b200.scenarios import fill_config, random_layout_host
+        self.k, self.c, self.sc, self.noise = k, comp, sc, noise
+        self.cfg = comp.env.cfg                      # the product's config struct, for the host twins
+        ocfg = fill_config(OrcConfig(), sc, num_worlds=W, beams=512, auto_reset=ar, seed=SEED)
+        o = self.o = OracleWorld(ocfg, sc.map.cells, sc.init_tab, sc.goal_tab)
+        self.relayout = sc.layout is not None
+        o.reset_world()
+        o.reset_pose()
+        o.generate_goal_point()
+        if self.relayout:
+            o.pose[...], o.goal[...], o.acc[...], status = random_layout_host(self.cfg, sc.layout, o.pose, o.goal,
+                                                                              o.acc)
+            assert not status.any()
+            o.observe()
+        n = o.N
+        self.live = np.ones(n, np.uint8)
+        self.stacks = ref.Stacks(o.obs)
+        self.scan_draws = 0
+        if noise is not None:
+            self.stacks.load(scan_host(self.cfg, noise, 0, self.stacks.array(), None, stream_id=k))
+        self.scan_draws = 1
+        self.gs = o.gs.copy()
+        # episode bookkeeping (ppo_stage1.py:51-57, 127-131; ppo_stage2.py:49-56, 136-137)
+        self.episode = np.zeros(n, np.int64)
+        self.steps = np.zeros(n, np.int64)
+        self.ep_reward = np.zeros(n)
+        self.ep_abs = np.zeros(n)
+        self.goal = o.goal[:, 0:2].copy()
+        self.init = o.pose[:, 0:2].copy()
+        self.idle = np.zeros(n, bool)                 # stage 2's liveflag false / a parked random robot
+        self.last_r = np.zeros(n, np.float32)
+
+    def state(self):
+        return self.stacks.array(), self.gs.copy()
+
+    def tick(self, cmd, g):
+        """one tick at global tick g: reward, flags, eplog, the rows that were idle on it and those that ended"""
+        from rl_collision_avoidance_b200.noise import scan_host
+        from rl_collision_avoidance_b200.scenarios import relayout_host
+        o = self.o
+        idle = self.idle | (self.live == 0)
+        o.step(cmd, live=self.live if self.relayout else None)
+        reward, flags, eplog = o.reward.copy(), o.flags.copy(), o.eplog.copy()
+        obs, gs = o.obs.copy(), o.gs.copy()
+        ended = (flags[:, 0] != 0) & ~idle
+        restart = flags[:, 3] != 0
+        self.stacks.tick(obs, restart)
+        if self.relayout:
+            o.pose[...], o.goal[...], o.acc[...], o.meta[...], flags, self.live, status = relayout_host(
+                self.cfg, self.sc.layout, o.pose, o.goal, o.acc, o.meta, flags)
+            assert not status.any()
+            o.observe()
+            relaid = flags[:, 3] != 0
+            arr = self.stacks.array()
+            arr[relaid] = o.obs[relaid][:, None, :]
+            self.stacks.load(arr)
+            gs[relaid] = o.gs[relaid]
+            restart = relaid
+        if self.noise is not None:
+            self.stacks.load(scan_host(self.cfg, self.noise, self.scan_draws, self.stacks.array(), flags,
+                                       stream_id=self.k))
+        self.scan_draws += 1
+        self.gs = gs
+        # bookkeeping
+        lines = []
+        live_now = ~idle
+        self.steps[live_now] += 1
+        self.ep_reward[live_now] += reward[live_now].astype(np.float64)
+        self.ep_abs[live_now] += np.abs(reward[live_now].astype(np.float64))
+        for i in np.nonzero(ended)[0]:
+            lines.append((i, self.episode[i], self.steps[i], self.ep_reward[i], self.ep_abs[i], self.goal[i].copy(),
+                          self.init[i].copy(), int(flags[i, 2])))
+        self.idle = (self.idle | ended) & ~restart
+        for i in np.nonzero(restart)[0]:
+            self.episode[i] += 1
+            self.steps[i] = 0
+            self.ep_reward[i] = self.ep_abs[i] = 0.0
+            self.goal[i] = o.goal[i, 0:2]
+            self.init[i] = o.pose[i, 0:2]
+        out = dict(reward=reward, flags=flags, eplog=eplog, idle=idle, ended=ended, lines=lines,
+                   last_r=self.last_r.copy())
+        self.last_r = reward.copy()
+        return out
+
+
+def _bits_equal(a, b):
+    a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
+    return a.shape == b.shape and np.array_equal(a.view(np.uint8), b.view(np.uint8))
+
+
+# ------------------------------------------------------------------------------------------------ float64 pieces
+def _params64(policy, flat):
+    from rl_collision_avoidance_b200.model.net import TENSORS
+    out = {}
+    for i, (name, shape) in enumerate(TENSORS):
+        o = policy.offsets[i]
+        out[name] = flat[o:o + math.prod(shape)].view(shape).double().clone()
+    return out
+
+
+def _forward64(P, x, gs, chunk=1024):
+    """float64 value (n,), mean (n, 2) and, per row and head, the magnitude of the actor head's terms
+    sum_k |w_k h_k| + |b| (n, 2): check_forward's mean bound (1e-5) holds for the synthetic weights of learner_ref; the
+    checkpoints' heads sum larger terms, so the mean is held to the value's relative bound, 2e-5 of that magnitude
+    (sigmoid and tanh have slope <= 1), and never below 1e-5"""
+    vs, ms, zs = [], [], []
+    W = torch.cat((P['actor1.weight'], P['actor2.weight'])).abs()
+    b = torch.cat((P['actor1.bias'], P['actor2.bias'])).abs()
+    with torch.no_grad():
+        for r0 in range(0, x.shape[0], chunk):
+            pre = []
+            v, m, _ = ref_forward(P, x[r0:r0 + chunk].double(), gs[r0:r0 + chunk].double(), pre)
+            h = torch.relu(dict(pre)['act_fc2'])
+            vs.append(v)
+            ms.append(m)
+            zs.append(h @ W.T + b)
+    return torch.cat(vs), torch.cat(ms), torch.cat(zs)
+
+
+def _mean_bound(P, pre):
+    """the bound on the device's mean per row and head (n, 2): see _forward64"""
+    W = torch.cat((P['actor1.weight'], P['actor2.weight'])).detach().abs()
+    b = torch.cat((P['actor1.bias'], P['actor2.bias'])).detach().abs()
+    h = torch.relu(dict(pre)['act_fc2'].detach())
+    return torch.clamp(2e-5 * (h @ W.T + b), min=1e-5)
+
+
+ADV_U = 4 * U             # the device's normalised advantage: (x - mean) / std in float32, from float64 moments
+ACTOR_SIDE = ('act_', 'actor', 'logstd')
+CRITIC_SIDE = ('crt_', 'critic')
+
+
+def _flip_rows_grad(policy, st, ii, x, gsx, act_all, lp_all, adv_n, tgt_all, pre, tower):
+    """The float64 gradient of the minibatch loss's share from the rows with an undecided fc1 / fc2 ReLU mask in
+    `tower` (a pre-activation within learner_ref.MARGIN of its layer's max of zero), or None when there is none.  A
+    flipped mask changes only its own row's contribution to the sum over the minibatch, so the device's gradient may
+    differ from float64 by up to twice that share."""
+    rows = torch.zeros(len(ii), dtype=torch.bool, device=ii.device)
+    for layer, z in pre:
+        if layer in (tower + '_fc1', tower + '_fc2'):
+            rows |= (z.detach().abs() < MARGIN * float(z.detach().abs().max())).any(1)
+    if not rows.any():
+        return None
+    with torch.enable_grad():
+        P = {n: t.requires_grad_(True) for n, t in _params64(policy, st['p']).items()}
+        jj = ii[rows]
+        v, mean, _ = ref_forward(P, x[jj].double(), gsx[jj].double())
+        (pl, vl, _), _ = ref_losses(P, v, mean, act_all[jj], lp_all[jj], adv_n[jj], tgt_all[jj])
+        ((pl + VCOEF * vl) * (len(jj) / len(ii))).backward()
+    return {n: t.grad for n, t in P.items()}
+
+
+def step_checks(check, what, policy, st, row, ii, x, gsx, act_all, lp_all, adv_n, tgt_all, ev):
+    """One optimizer step, teacher-forced from the device's parameters at the step (st['p']) on the minibatch rows ii
+    of the replayed schedule.
+
+    Loss row.  The float64 losses (learner_ref.ref_losses) differ from the device's through the device's forward
+    (its value within dv = 2e-5 max(1, |v|), check_forward's bound; its mean within dm, _mean_bound) and through the
+    float32 loss reduction (check_step's 1e-5 of the loss, at least 1e-7).  First order:
+      policy: |d ratio| = ratio |d logprob| <= ratio sum_d |a - mean| / sigma^2 dm, the advantage within ADV_U, so
+              the policy loss moves by <= mean(ratio (|adv| |d logprob| + ADV_U |adv|));
+      value:  mean((v - tgt)^2) moves by <= mean(2 |v - tgt| dv + dv^2) (the targets are the device's own);
+      entropy: a function of logstd alone.
+    Gradients.  check_step's 5e-5 of the layer scale holds where the forward is within check_forward's bounds for
+    |v| <= 1: the mean within 1e-5, the value within 2e-5.  A gradient is first order in the error of the output its
+    loss term reads, so the actor side (its towers, heads and logstd) is held to 5e-5 times this minibatch's
+    max(dm) / 1e-5 and the critic side to 5e-5 times dv / 2e-5.  A tower's conv tensors with an undecided conv mask
+    are held to at least 3e-3 (module docstring); an undecided fc mask adds twice its rows' share (_flip_rows_grad).
+    Adam.  ref.adam_step in float64 from the device's p, g, m, v and step, with the float32 betas the kernel receives,
+    against the bound of adam_bounds."""
+    P = {n: t.requires_grad_(True) for n, t in _params64(policy, st['p']).items()}
+    pre = []
+    v, mean, _ = ref_forward(P, x[ii].double(), gsx[ii].double(), pre)
+    act, old_lp, adv, tgt = act_all[ii], lp_all[ii], adv_n[ii], tgt_all[ii]
+    (pl, vl, ent), loss = ref_losses(P, v, mean, act, old_lp, adv, tgt)
+    loss.backward()
+    with torch.no_grad():
+        ratio = torch.exp(ref_logprob(P, mean, act) - old_lp)
+        near = ((ratio - (1 - CLIP)).abs() < MARGIN) | ((ratio - (1 + CLIP)).abs() < MARGIN)
+        assert not near.any(), f'{what}: a PPO ratio within {MARGIN} of 1 +- clip: choose another seed'
+        ev['clipped'] += int(((ratio < 1 - CLIP) | (ratio > 1 + CLIP)).sum())
+        dm = _mean_bound(P, pre)
+        dv = 2e-5 * max(1.0, maxabs(v))
+        dlp = ((act - mean).abs() / torch.exp(2 * P['logstd']) * dm).sum(1)
+        bounds = (float((ratio * adv.abs() * (dlp + ADV_U)).mean()) + 1e-5 * max(abs(float(pl)), 1e-2),
+                  float((2 * (v - tgt).abs() * dv + dv * dv).mean()) + 1e-5 * max(abs(float(vl)), 1e-2),
+                  1e-5 * max(abs(float(ent)), 1e-2))
+        for i, name in enumerate(('policy', 'value', 'entropy')):
+            check(f'{what} {name} loss', abs(row[i] - float((pl, vl, ent)[i])), bounds[i])
+        undecided = {layer: int((z.abs() < MARGIN * float(z.abs().max())).sum()) for layer, z in pre}
+        factor = float(dm.max()) / 1e-5
+        ev['worst_mean_factor'] = max(ev['worst_mean_factor'], factor)
+        ev['worst_value_factor'] = max(ev['worst_value_factor'], dv / 2e-5)
+        grads = {n: t.grad for n, t in P.items()}
+        gdev = _params64(policy, st['g'])
+        for tower in ('act', 'crt'):
+            ev['undecided_conv'] += int(bool(undecided[tower + '_cv1'] or undecided[tower + '_cv2']))
+            ev['undecided_fc'] += int(bool(undecided[tower + '_fc1'] or undecided[tower + '_fc2']))
+        flip = {side: _flip_rows_grad(policy, st, ii, x, gsx, act_all, lp_all, adv_n, tgt_all, pre, tower)
+                for side, tower in ((ACTOR_SIDE, 'act'), (CRITIC_SIDE, 'crt'))}
+        for name, r in grads.items():
+            side = ACTOR_SIDE if name.startswith(ACTOR_SIDE) else CRITIC_SIDE
+            tower = 'act' if side is ACTOR_SIDE else 'crt'
+            conv = '_fea_cv' in name and (undecided[tower + '_cv1'] or undecided[tower + '_cv2'])
+            tol = 5e-5 * (factor if side is ACTOR_SIDE else dv / 2e-5)
+            tol = max(tol, 3e-3) if conv else tol
+            extra = 2 * maxabs(flip[side][name]) if flip[side] is not None else 0.0
+            check(f'{what} grad {name}', maxabs(gdev[name] - r), tol * layer_scale(grads, name) + extra)
+    p0, g0, m0, v0 = (_np(st[key]).astype(np.float64) for key in ('p', 'g', 'm', 'v'))
+    p64, m64, v64 = ref.adam_step(p0, g0, m0, v0, st['t'], LR, (B1, B2), 1e-8)
+    p1, m1, v1 = (_np(st[key]).astype(np.float64) for key in ('p1', 'm1', 'v1'))
+    bm, bv, bp = adam_bounds(p0, g0, m0, v0, p1, p64, st['t'])
+    for name, got, want, bound in (('exp_avg', m1, m64, bm), ('exp_avg_sq', v1, v64, bv), ('parameters', p1, p64, bp)):
+        r = np.abs(got - want) / bound
+        i = int(np.argmax(r))
+        check(f'{what} Adam {name} (error / bound; worst at {i}: p {p0[i]:.9g} g {g0[i]:.9g} m {m0[i]:.9g} '
+              f'v {v0[i]:.9g} got {got[i]:.9g} want {want[i]:.9g})', float(r[i]), 1.0)
+
+
+def adam_bounds(p0, g0, m0, v0, p1, p64, step):
+    """Error model of the fused Adam step (csrc/rlca_policy.cu, adam_update_one) against ref.adam_step with the same
+    float32 betas, u = 2^-24 the unit roundoff (every float32 rounding is within u of its result):
+      m = fmaf(b1, m, (1 - b1) g): 1 - b1 is exact (Sterbenz); the product and the fma round once each:
+          <= 2u (b1 |m| + (1 - b1) |g|);
+      v = fmaf(b2, v, (1 - b2) g g): two products and the fma: <= 3u (b2 v + (1 - b2) g^2);
+      the step d = lr / bc1 * m / (sqrtf(v) / sqrt(bc2) + eps) carries m's error relative to m (bm / |m|: large where
+          b1 m and (1 - b1) g cancel, as they do when the gradient changes sign) and half of v's relative error (the
+          square root); lr's float32 rounding and eight float32 operations add <= 9u, taken as 16u;
+          bc1 = 1 - powf(b1, t) and bc2 = 1 - powf(b2, t) are formed in float32 on the host, and powf's error
+          (<= 1 ulp, 2u) is amplified by the cancellation b^t / (1 - b^t): 2u k1 for bc1, u k2 for bc2 under the
+          square root;
+      p - d rounds to within half an ulp of the result.
+    Returns the bounds on m, v and p."""
+    k1 = B1 ** step / (1 - B1 ** step)
+    k2 = B2 ** step / (1 - B2 ** step)
+    bm = 2 * U * (B1 * np.abs(m0) + (1 - B1) * np.abs(g0)) + TINY
+    bv = 3 * U * (B2 * v0 + (1 - B2) * g0 * g0) + TINY
+    mv = np.abs(B1 * m0 + (1 - B1) * g0)
+    vv = B2 * v0 + (1 - B2) * g0 * g0
+    rel = (16 * U + 2 * U * k1 + U * k2 + np.divide(bm, mv, out=np.zeros_like(mv), where=mv > 0)
+           + 0.5 * np.divide(bv, vv, out=np.zeros_like(vv), where=vv > 0))
+    bp = 0.5 * np.spacing(np.abs(p1).astype(np.float32)).astype(np.float64) + rel * np.abs(p64 - p0) + TINY
+    return bm, bv, bp
+
+
+# ------------------------------------------------------------------------------------------------ the test
+@pytest.mark.parametrize('case', list(CASES))
+def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
+    t_start = time.perf_counter()
+    c = CASES[case]
+    stage, H = c['stage'], c['H']
+    rec, envs, scs, noise, lines, cal = _train(case, monkeypatch)
+    t_train = time.perf_counter() - t_start
+    policy = rec.policy
+    comps = rec.comps
+    N = sum(e.N for e in envs)
+    assert len(rec.updates) == 2 and len(rec.gtd) == 2 and len(rec.ticks) == 2 * H
+    oc = [OracleComponent(k, comp, sc, W, ar, noise) for k, (comp, (sc, W, ar)) in enumerate(zip(comps, scs))]
+    check = Checks()
+    ev = dict(ended=0, ended_last_tick=0, idle=0, respawn=0, relaid=0, filtered=0, boundary_runs=0, noised_rows=0,
+              steps=0, clipped=0, undecided_conv=0, undecided_fc=0, worst_mean_factor=0.0,
+              worst_value_factor=0.0)
+    expected_lines = []
+    for u, up in enumerate(rec.updates):
+        snap = up['snap']
+        # ---- a. the environment, bit for bit, and the episode bookkeeping
+        st0 = [o.state() for o in oc]
+        for o, (s, g) in zip(oc, st0):
+            a, b = o.c.a, o.c.b
+            assert _bits_equal(snap['stacks'][0, a:b], s), f'update {u}: stacks[0] of {o.c.name} (carry-over)'
+            assert _bits_equal(snap['gs'][0, a:b], g), f'update {u}: gs[0] of {o.c.name} (carry-over)'
+        dones = np.zeros((H, N), bool)
+        rewards = np.zeros((H, N), np.float32)
+        upd_lines = []
+        for t in range(H):
+            g = u * H + t
+            tk = up['ticks'][t]
+            assert tk['slot'] == t, f'update {u} tick {t}: the policy read stack slot {tk["slot"]}'
+            scaled = _np(tk['scaled'])
+            for o in oc:
+                a, b = o.c.a, o.c.b
+                cmd = scaled[a:b]
+                if noise is not None and noise.action_on:
+                    from rl_collision_avoidance_b200.noise import action_host
+                    sid, draw, inp, out = [x for x in rec.noise_cmds if x[0] == o.k][g]
+                    assert draw == g and _bits_equal(_np(inp), cmd), f'tick {g}: the noised command\'s input'
+                    want = action_host(o.cfg, noise, g, cmd, stream_id=o.k)
+                    assert _bits_equal(_np(out), want), f'tick {g}: executed command of {o.c.name}'
+                    ev['noised_rows'] += int((want != cmd).any(1).sum())
+                    cmd = want
+                r = o.tick(cmd, g)
+                s, gsn = o.state()
+                what = f'update {u} tick {t} {o.c.name}'
+                assert _bits_equal(snap['stacks'][t + 1, a:b], s), f'{what}: stack'
+                assert _bits_equal(snap['gs'][t + 1, a:b], gsn), f'{what}: gs'
+                assert _bits_equal(snap['rewards'][t, a:b], r['reward']), f'{what}: reward'
+                assert _bits_equal(snap['flags'][t, a:b], r['flags']), f'{what}: flags'
+                e = r['ended']
+                assert _bits_equal(snap['eplog'][t, a:b][e], r['eplog'][e]), f'{what}: eplog of ended episodes'
+                # stage 2's liveflag: an idle robot's row repeats its last reward and stays terminal, result 0
+                idle = r['idle']
+                if idle.any():
+                    assert _bits_equal(r['reward'][idle], r['last_r'][idle]), f'{what}: stale reward of idle rows'
+                    assert (r['flags'][idle, 0] == 1).all() and (r['flags'][idle, 2] == 0).all(), f'{what}: idle flags'
+                ev['idle'] += int(idle.sum())
+                ev['ended'] += int(e.sum())
+                ev['ended_last_tick'] += int(e.sum()) if t == H - 1 else 0
+                ev['respawn' if not o.relayout else 'relaid'] += int((r['flags'][:, 3] != 0).sum())
+                dones[t, a:b] = r['flags'][:, 0] != 0
+                rewards[t, a:b] = r['reward']
+                for (i, epi, steps, rsum, rabs, goal, init, res) in r['lines']:
+                    upd_lines.append((t, a + i, o, i, epi, steps, rsum, rabs, goal, init, res))
+        # ---- b. the policy per tick, at the weights of the update's start
+        P = _params64(policy, up['flat'])
+        logstd = _np(up['flat'][policy.offsets[0]:policy.offsets[0] + 2])
+        x = torch.from_numpy(snap['stacks'][:H].reshape(H * N, 3, 512)).cuda()
+        gsx = torch.from_numpy(snap['gs'][:H].reshape(H * N, 4)).cuda()
+        v64, m64, zs = _forward64(P, x, gsx)
+        mean_dev = torch.stack([tk['mean'] for tk in up['ticks']]).reshape(H * N, 2)
+        vs = max(1.0, maxabs(v64))
+        check(f'update {u} rollout value', maxabs(torch.from_numpy(snap['values']).cuda().reshape(-1).double() - v64),
+              2e-5 * vs)
+        check(f'update {u} rollout mean (error / bound)',
+              float(((mean_dev.double() - m64).abs() / torch.clamp(2e-5 * zs, min=1e-5)).max()), 1.0)
+        mean_np = _np(mean_dev).reshape(H, N, 2)
+        wa, wl = 0.0, 0.0
+        for t, tk in enumerate(up['ticks']):
+            assert tk['seed'] == policy.sample_seed
+            act64, z = sample_ref.sample(mean_np[t], logstd, tk['seed'], tk['counter'])
+            act = snap['actions'][t]
+            sz = sample_ref.sigma(logstd) * np.abs(z)
+            wa = max(wa, float((np.abs(act - act64) / action_bound(act, sz)).max()))
+            lp = sample_ref.log_prob(act, mean_np[t], logstd)
+            wl = max(wl, float((np.abs(snap['logprobs'][t] - lp) / lp_bound(act, mean_np[t], logstd)).max()))
+            assert _bits_equal(_np(tk['scaled']), sample_ref.scaled(act)), f'update {u} tick {t}: scaled action'
+        check(f'update {u} stored actions = sample_ref draws (error / bound)', wa, 1.0)
+        check(f'update {u} stored log-probabilities (error / bound)', wl, 1.0)
+        # last_v: the value of the replayed state after the horizon
+        gt = rec.gtd[u]
+        sH = np.concatenate([o.state()[0] for o in oc])
+        gH = np.concatenate([o.state()[1] for o in oc])
+        lv64, _, _ = _forward64(P, torch.from_numpy(sH).cuda(), torch.from_numpy(gH).cuda())
+        check(f'update {u} last_v', maxabs(torch.from_numpy(gt['last_value']).cuda().double() - lv64),
+              2e-5 * max(1.0, maxabs(lv64)))
+        # ---- c. the update
+        assert _bits_equal(gt['rewards'], rewards), f'update {u}: GAE rewards'
+        assert _bits_equal(gt['values'], snap['values']), f'update {u}: GAE values'
+        assert np.array_equal(gt['dones'] != 0, dones), f'update {u}: GAE dones are not flag 0 (done)'
+        # the C ABI takes gamma and lambda as float32 (test_gae_vs_float64_recurrence)
+        tg64, adv64 = ref.gae(rewards, snap['values'], gt['last_value'], dones, float(np.float32(gt['gamma'])),
+                              float(np.float32(gt['lam'])))
+        for name, got, want in (('targets', gt['targets'], tg64), ('advantages', gt['advs'], adv64)):
+            ulp = np.spacing(np.abs(want).astype(np.float32)).astype(np.float64)
+            check(f'update {u} GAE {name} (ulps)', float((np.abs(got - want) / ulp).max()), 1.0)
+        fi = ref.filter_index(dones) if stage == 2 else []
+        assert up['filter_index'] == fi, f'update {u}: filter_index'
+        ev['filtered'] += len(fi)
+        starts = {o.c.a for o in oc if o.c.a > 0}
+        ev['boundary_runs'] += sum(1 for j in fi if j < N and j in starts)
+        keep = ref.kept_rows(H * N, fi)
+        gen = torch.Generator(device='cuda')
+        gen.set_state(up['gen_state'])
+        batches = []
+        for _ in range(2):
+            perm = torch.randperm(len(keep), device='cuda', generator=gen).cpu().numpy()
+            batches += ref.minibatches(keep[perm], c['batch'], drop_last=stage == 2)
+        assert len(batches) == len(up['steps']) == len(up['rows']), (len(batches), len(up['steps']), len(up['rows']))
+        if stage == 1:
+            assert len(batches[-1]) < c['batch'] or (H * N) % c['batch'] == 0
+        # the restated normalisation of the device's GAE output: over all H N rows, before np.delete (model/ppo.py:148,
+        # 202, 212-218); the device forms it in float32 from float64 moments, a few u of each value (ADV_U below)
+        adv_n = torch.from_numpy(ref.normalise(gt['advs'].astype(np.float64)).reshape(-1)).cuda()
+        tgt_all = torch.from_numpy(gt['targets'].reshape(-1).astype(np.float64)).cuda()
+        act_all = torch.from_numpy(snap['actions'].reshape(-1, 2)).cuda().double()
+        lp_all = torch.from_numpy(snap['logprobs'].reshape(-1)).cuda().double()
+        for k, (idx, st) in enumerate(zip(batches, up['steps'])):
+            what = f'update {u} step {k} (nb {len(idx)})'
+            assert st['grad_scale'] == 1.0 and st['t'] == up['step_count'] + k + 1, what
+            assert _bits_equal(_np(st['p']), _np(up['flat'] if k == 0 else up['steps'][k - 1]['p1'])), \
+                f'{what}: the parameters the step starts from'
+            ev['steps'] += 1
+            step_checks(check, what, policy, st, up['rows'][k], torch.from_numpy(idx).cuda(), x, gsx, act_all,
+                        lp_all, adv_n, tgt_all, ev)
+        # ---- d. the episode log lines of this update, in the trainer's (tick, column) order
+        upd_lines.sort(key=lambda x: (x[0], x[1]))
+        expected_lines += upd_lines
+    # ---- d. log lines against the bookkeeping
+    from rl_collision_avoidance_b200.stage_world import RESULT_STRINGS
+    env_lines = [l for l in lines if isinstance(l, str) and l.startswith('Env ')]
+    assert len(env_lines) == len(expected_lines) == len(cal), (len(env_lines), len(expected_lines), len(cal))
+    mixed = len(oc) > 1
+    for line, calv, (t, col, o, i, epi, steps, rsum, rabs, goal, init, res) in zip(env_lines, cal, expected_lines):
+        robot = i % o.c.env.num_env
+        head = 'Env %02d, Goal (%05.1f, %05.1f), Episode %05d, setp %03d, Reward ' % (
+            robot, goal[0], goal[1], epi + 1 if stage == 1 else epi, steps + 1 if stage == 1 else steps)
+        assert line.startswith(head), (line, head)
+        rest = line[len(head):].split(', ')
+        got_r = float(rest[0])
+        if stage == 1:
+            dist = float(np.hypot(np.float32(goal[0]) - np.float32(init[0]), np.float32(goal[1]) - np.float32(init[1])))
+            assert rest[1:] == ['Distance %05.1f' % dist, RESULT_STRINGS[res]], line
+        elif mixed:
+            assert rest[1:] == [RESULT_STRINGS[res], o.c.name], line
+        else:
+            assert rest[1:] == [RESULT_STRINGS[res] + ','], line
+        # float32 running sum of `steps` terms: <= steps u sum |r| from the float64 sum
+        tol = steps * U * rabs
+        assert abs(float(calv) - rsum) <= tol + 1e-30, (line, float(calv), rsum, tol)
+        assert abs(got_r - rsum) <= 0.05 + tol + 1e-9, (line, rsum)
+    check.done()
+    # ---- the events each case exists for
+    print(f'[events] {case}: {ev}, train {t_train:.1f} s, total {time.perf_counter() - t_start:.1f} s')
+    assert ev['ended'] > 0 and len(env_lines) > 0 and ev['steps'] > 0
+    if case in ('stage1', 'noise'):
+        assert ev['ended_last_tick'] > 0 and ev['respawn'] > 0
+    if noise is not None:
+        assert ev['noised_rows'] > 0
+    if case in ('stage2', 'mix'):
+        assert ev['filtered'] > 0 and ev['idle'] > 0 and ev['respawn'] > 0
+    if case in ('random', 'mix'):
+        assert ev['relaid'] > 0
+    if case == 'mix':
+        assert ev['boundary_runs'] > 0, 'no filter run crossed a component boundary'
