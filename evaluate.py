@@ -22,6 +22,9 @@ still ticks and the rotation per successful episode (DESIGN.md §9o).  --scan-no
 --action-noise SIGMA_V[,SIGMA_W] evaluate under sensor and actuation noise: Gaussian range error on every beam with a
 return, beams that read no return, and a relative gain error on the executed v and w, drawn from --noise-seed
 (default --seed; DESIGN.md §9p).  The ORCA baselines do not read the scan, so only --action-noise applies to them.
+--scan-delay T[,T_MAX] and --command-delay T[,T_MAX] evaluate under sensing and command latency: each robot reads the
+scan of T ticks (0.1 s each) earlier and executes the command issued T ticks earlier, or a delay drawn in T..T_MAX per
+robot and episode from --latency-seed (default --seed; DESIGN.md §9q).  Only --command-delay applies to the baselines.
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -38,6 +41,8 @@ return, beams that read no return, and a relative gain error on the executed v a
         --timeouts
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
         --scan-noise 0.05 --beam-dropout 0.1 --action-noise 0.1
+    python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
+        --scan-delay 2 --command-delay 1,3
 """
 import argparse
 import json
@@ -48,6 +53,8 @@ import torch
 
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, PROGRESS_COLUMNS, PROGRESS_DEFAULTS, \
     SAFETY_COLUMNS, evaluate, non_cooperative_mask
+from rl_collision_avoidance_b200.latency import LATENCY_FLAGS, Latency, add_latency_arguments, \
+    latency_from_arguments
 from rl_collision_avoidance_b200.model.net import CNNPolicy
 from rl_collision_avoidance_b200.noise import NOISE_FLAGS, Noise, add_noise_arguments, noise_from_arguments
 from rl_collision_avoidance_b200.orca import HYBRID_DEFAULTS, Hybrid, NonCooperative, \
@@ -107,6 +114,7 @@ def main(argv=None):
                     help='a robot still for W ticks is frozen, one without progress for W ticks stalled (default %d); '
                          'implies --timeouts' % PROGRESS_DEFAULTS['window'])
     add_noise_arguments(ap)
+    add_latency_arguments(ap)
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -138,6 +146,9 @@ def main(argv=None):
     if args.baseline is not None and (args.scan_noise is not None or args.beam_dropout is not None):
         ap.error('--scan-noise / --beam-dropout apply to --policy only: the ORCA baselines do not read the scan')
     noise_params = noise_from_arguments(ap, args)
+    if args.baseline is not None and args.scan_delay is not None:
+        ap.error('--scan-delay applies to --policy only: the ORCA baselines do not read the scan')
+    latency_params = latency_from_arguments(ap, args)
     hybrid_params = None
     if args.hybrid:
         hybrid_params = dict(HYBRID_DEFAULTS)
@@ -178,8 +189,9 @@ def main(argv=None):
                             speed=args.non_cooperative_speed)
     hy = Hybrid(env, **hybrid_params) if args.hybrid else None
     noise = Noise(env, noise_params) if noise_params is not None else None
+    latency = Latency(env, latency_params) if latency_params is not None else None
     out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy,
-                   safety=safety, progress=progress, noise=noise)
+                   safety=safety, progress=progress, noise=noise, latency=latency)
 
     def line(m, robots, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -194,6 +206,10 @@ def main(argv=None):
         ns = out['noise']
         print('noise  range sigma %g m  beam dropout %g  v gain sigma %g  w gain sigma %g  seed %d'
               % (ns['range_sigma'], ns['dropout'], ns['v_gain_sigma'], ns['w_gain_sigma'], ns['seed']))
+    if latency is not None:
+        ls = out['latency']
+        print('latency  scan delay %d..%d ticks  command delay %d..%d ticks  (tick %g s)  seed %d'
+              % (*ls['scan_delay'], *ls['command_delay'], env.cfg.dt, ls['seed']))
     line(m, env.N)
     if nc is not None:
         k = args.non_cooperative * args.num_worlds
@@ -236,7 +252,8 @@ def main(argv=None):
     if args.json:
         hidden = (() if safety is not None else ('safety', 'near_miss')) + \
             (() if progress is not None else ('timeouts', 'stall_window')) + \
-            (() if noise is not None else tuple(f[2:].replace('-', '_') for f in NOISE_FLAGS))
+            (() if noise is not None else tuple(f[2:].replace('-', '_') for f in NOISE_FLAGS)) + \
+            (() if latency is not None else tuple(f[2:].replace('-', '_') for f in LATENCY_FLAGS))
         shown = {k: v for k, v in vars(args).items() if k not in hidden}
         res = {'args': shown, 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
@@ -244,6 +261,8 @@ def main(argv=None):
                'partials': out['partials'].tolist()}
         if noise is not None:
             res['noise'] = out['noise']
+        if latency is not None:
+            res['latency'] = out['latency']
         if nc is not None:
             res['by_role'] = out['by_role']
             res['partials_split'] = out['partials_split'].tolist()

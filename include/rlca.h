@@ -963,6 +963,71 @@ int rlca_noise_scan_host(const rlca_env_config *cfg, const rlca_noise_params *p,
 int rlca_noise_action_host(const rlca_env_config *cfg, const rlca_noise_params *p, uint32_t draw,
                            const float *action_in_host, float *action_out_host);
 
+/* =====================================================================================
+ * Sensing and command latency (csrc/rlca_latency.cu, DESIGN.md §9q): separate launches around the tick, issued only
+ * when a run asks for latency; the tick itself and its outputs are untouched.  One tick is dt = 0.1 s and every delay
+ * is a whole number of ticks in 0 .. RLCA_LATENCY_MAX_DELAY.
+ *
+ * Delays: an agent draws its scan delay d in [scan_lo, scan_hi] and its command delay l in [cmd_lo, cmd_hi] when it
+ * starts an episode (a row whose flags[4 a + 3], was_reset, is set, or every row when flags is NULL), and holds them
+ * until its next one.  The draw is lo + (((hi - lo + 1) * (uint64)w0) >> 32), w0 the first word of Philox-4x32-10
+ * under the key (seed lo, seed hi) of the counter
+ *   (global agent = (world_offset + w) R + r, draw, 0, purpose | stream_id << 8)
+ * with purposes 0xE4 scan, 0xE5 command (one byte; the environment uses 1-5, the sampler 0x5A17, noise 0xE1-0xE3).
+ * `draw` is the caller's own counter of calls of that kind, 0, 1, 2, ...; it also picks the ring slot, draw mod
+ * (hi + 1), so it must advance by one per call.  Everything is integer arithmetic and copies: the host twins equal the
+ * kernels bit for bit, and no delay depends on num_worlds, the launch shape or anything but the key and the counter.
+ *
+ * Scan (after a tick and any re-layout, before scan noise): a ring of D = scan_hi + 1 frames per agent.  A fresh row
+ * puts its newest frame in all D slots and redraws d; its stack, three copies of that frame, is left as it is.  Any
+ * other row stores its newest frame in slot draw mod D and then reads slot (draw - d) mod D into the newest frame.  The
+ * robot therefore reads the true frame of d calls earlier, or its episode's first frame while fewer than d calls have
+ * passed; the stack's two older frames are what the tick shifted in, the frames delivered on the calls before.
+ * Command (before noise and the tick, with the flags of the PREVIOUS tick, NULL on a run's first tick): a ring of
+ * C = cmd_hi + 1 (v, w) pairs per agent.  A fresh row puts the issued command in all C slots and redraws l; then every
+ * row stores the issued command (bit for bit, unclipped) in slot draw mod C and executes slot (draw - l) mod C: the
+ * robot executes the command issued l calls earlier, or its episode's first command while fewer than l calls have
+ * passed.  (Not a zero command: the tick's collision latch is cleared only by a move, so a re-spawned robot held still
+ * would crash again on every tick.)
+ * A kind whose hi is 0 is the identity: no launch, its ring and delay pointers may be NULL, and the action entry copies
+ * the command to action_out (nothing when the two are the same buffer).
+ * ===================================================================================== */
+#define RLCA_LATENCY_MAX_DELAY 8
+typedef struct rlca_latency_params {
+    int32_t scan_lo, scan_hi;    /* ticks; 0 <= lo <= hi <= RLCA_LATENCY_MAX_DELAY */
+    int32_t cmd_lo, cmd_hi;      /* ticks; the same */
+    uint64_t seed;
+    uint32_t stream_id;          /* < 2^24 */
+} rlca_latency_params;
+
+/* The state of one env handle's latency, in device memory for the device entries and host memory for the host twins;
+ * N = num_worlds R rows of this config.  The caller allocates it and keeps it from call to call. */
+typedef struct rlca_latency_state {
+    float *scan_ring;            /* (N, scan_hi + 1, beams) float: the last scan_hi + 1 true frames per agent */
+    float *cmd_ring;             /* (N, cmd_hi + 1, 2) float: the last cmd_hi + 1 issued commands per agent */
+    uint8_t *scan_delay;         /* (N,) the scan delay of each agent's episode, ticks */
+    uint8_t *cmd_delay;          /* (N,) the command delay of each agent's episode, ticks */
+} rlca_latency_state;
+
+/* In place on stack_dev (N, 3, beams) float, after a tick: the newest frame (slot 2) becomes the delayed frame.
+ * RLCA_ERR_INVALID for a NULL cfg, params, state or stack, robots_per_world outside 1..64, num_worlds or beams < 1,
+ * world_offset < 0, a delay range with lo < 0, lo > hi or hi > RLCA_LATENCY_MAX_DELAY, stream_id >= 2^24, or, with
+ * scan_hi > 0, a NULL scan_ring or scan_delay. */
+int rlca_latency_scan(const rlca_env_config *cfg, const rlca_latency_params *p, const rlca_latency_state *state,
+                      uint32_t draw, const unsigned char *flags_dev, float *stack_dev, void *stream);
+/* Before a tick: the command the robots execute, action_out_dev (N, 2), from the issued command action_in_dev (N, 2),
+ * which is never written.  The same argument checks, with cmd_ring / cmd_delay for the command, and action_in_dev /
+ * action_out_dev not NULL. */
+int rlca_latency_action(const rlca_env_config *cfg, const rlca_latency_params *p, const rlca_latency_state *state,
+                        uint32_t draw, const unsigned char *flags_dev, const float *action_in_dev,
+                        float *action_out_dev, void *stream);
+/* The same on HOST buffers (state included) by serial loops over the same code; the outputs equal the kernels'. */
+int rlca_latency_scan_host(const rlca_env_config *cfg, const rlca_latency_params *p, const rlca_latency_state *state,
+                           uint32_t draw, const unsigned char *flags_host, float *stack_host);
+int rlca_latency_action_host(const rlca_env_config *cfg, const rlca_latency_params *p, const rlca_latency_state *state,
+                             uint32_t draw, const unsigned char *flags_host, const float *action_in_host,
+                             float *action_out_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

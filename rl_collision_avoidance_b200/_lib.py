@@ -103,6 +103,18 @@ class NoiseParams(C.Structure):
                 ('w_gain_sigma', C.c_float), ('seed', C.c_uint64), ('stream_id', C.c_uint32)]
 
 
+class LatencyParams(C.Structure):
+    """Mirror of rlca_latency_params (include/rlca.h)."""
+    _fields_ = [('scan_lo', C.c_int32), ('scan_hi', C.c_int32), ('cmd_lo', C.c_int32), ('cmd_hi', C.c_int32),
+                ('seed', C.c_uint64), ('stream_id', C.c_uint32)]
+
+
+class LatencyState(C.Structure):
+    """Mirror of rlca_latency_state (include/rlca.h): device pointers, or host pointers for the host twins."""
+    _fields_ = [('scan_ring', C.c_void_p), ('cmd_ring', C.c_void_p), ('scan_delay', C.c_void_p),
+                ('cmd_delay', C.c_void_p)]
+
+
 # rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
 EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
                  'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
@@ -241,6 +253,14 @@ SYMBOLS = {
     'rlca_noise_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(NoiseParams), C.c_uint32, _P, _P, _P]),
     'rlca_noise_scan_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(NoiseParams), C.c_uint32, _P, _P]),
     'rlca_noise_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(NoiseParams), C.c_uint32, _P, _P]),
+    'rlca_latency_scan': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LatencyParams), C.POINTER(LatencyState),
+                                    C.c_uint32, _P, _P, _P]),
+    'rlca_latency_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LatencyParams), C.POINTER(LatencyState),
+                                      C.c_uint32, _P, _P, _P, _P]),
+    'rlca_latency_scan_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LatencyParams), C.POINTER(LatencyState),
+                                         C.c_uint32, _P, _P]),
+    'rlca_latency_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LatencyParams), C.POINTER(LatencyState),
+                                           C.c_uint32, _P, _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

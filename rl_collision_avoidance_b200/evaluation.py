@@ -472,7 +472,7 @@ def metrics(tot):
 
 
 def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None,
-             progress=None, noise=None):
+             progress=None, noise=None, latency=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
@@ -508,7 +508,18 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     after every tick, the stack the tick wrote get `noise.scan` (with env.flags), and the command, after the
     non-cooperative override and the circle rule, becomes `noise.action`'s executed command before control_vel.
     env.obs, env.gs and the state are never perturbed, so the trackers keep measuring the true scan and poses.  The
-    result then also holds 'noise' (the settings).  Scan noise needs a policy: the ORCA baselines do not read the scan."""
+    result then also holds 'noise' (the settings).  Scan noise needs a policy: the ORCA baselines do not read the scan.
+
+    With `latency` (a latency.Latency on `env`, DESIGN.md §9q) the robots read old scans and execute old commands: the
+    first stack and, after every tick, the stack the tick wrote get `latency.scan` (with env.flags) before any noise,
+    and the command, after the circle rule and before noise, becomes `latency.action`'s executed command, with the
+    flags of the previous tick (None on the first).  A circle robot stopped by the circle rule still runs out the
+    commands already queued.  The result then also holds 'latency' (the settings).  Scan delay needs a policy."""
+    if latency is not None:
+        if latency.env is not env:
+            raise ValueError('the latency belongs to another env')
+        if latency.params.scan_on and isinstance(policy, (OrcaController, NhOrcaController)):
+            raise ValueError('scan delay changes what a policy reads; the ORCA baselines do not read the scan')
     E = int(episodes)
     if int(check_every) < 1:
         raise ValueError('check_every must be >= 1')
@@ -534,6 +545,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         hybrid.reset()
     obs = env.get_laser_observation()
     stacks = [obs[:, None, :].repeat(1, 3, 1).contiguous(), torch.empty(N, 3, env.beam_mum, device=dev)]
+    if latency is not None:
+        latency.scan(stacks[0])
     if noise is not None:
         noise.scan(stacks[0])
     terminal = torch.zeros(N, dtype=torch.bool, device=dev)
@@ -553,9 +566,13 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             non_cooperative.apply(scaled)
         if circle:
             scaled = torch.stack((torch.where(terminal, 0.0, scaled[:, 0]), scaled[:, 1]), 1)
+        if latency is not None:
+            scaled = latency.action(scaled, env.flags if tick > 0 else None)
         if noise is not None:
             scaled = noise.action(scaled)
         env.control_vel(scaled, stack_in=stacks[k], stack_out=stacks[1 - k])
+        if latency is not None:
+            latency.scan(stacks[1 - k], env.flags)
         if noise is not None:
             noise.scan(stacks[1 - k], env.flags)
         if safe is not None:
@@ -599,4 +616,6 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
                                        'non_cooperative': progress_metrics(progress_totals(ps[:, 1]))}
     if noise is not None:
         out['noise'] = noise.settings()
+    if latency is not None:
+        out['latency'] = latency.settings()
     return out
