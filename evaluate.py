@@ -25,6 +25,9 @@ return, beams that read no return, and a relative gain error on the executed v a
 --scan-delay T[,T_MAX] and --command-delay T[,T_MAX] evaluate under sensing and command latency: each robot reads the
 scan of T ticks (0.1 s each) earlier and executes the command issued T ticks earlier, or a delay drawn in T..T_MAX per
 robot and episode from --latency-seed (default --seed; DESIGN.md §9q).  Only --command-delay applies to the baselines.
+--accel-limit A[,A_MAX] and --angular-accel-limit B[,B_MAX] evaluate under acceleration limits: each tick the executed v
+changes by at most A dt and w by at most B dt, with limits drawn in A..A_MAX and B..B_MAX per robot and episode from
+--dynamics-seed (default --seed; DESIGN.md §9r).  They apply to the baselines too.
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -43,6 +46,8 @@ robot and episode from --latency-seed (default --seed; DESIGN.md §9q).  Only --
         --scan-noise 0.05 --beam-dropout 0.1 --action-noise 0.1
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
         --scan-delay 2 --command-delay 1,3
+    python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
+        --accel-limit 1 --angular-accel-limit 2
 """
 import argparse
 import json
@@ -51,6 +56,8 @@ import os
 
 import torch
 
+from rl_collision_avoidance_b200.dynamics import DYNAMICS_FLAGS, Dynamics, add_dynamics_arguments, \
+    dynamics_from_arguments
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, PROGRESS_COLUMNS, PROGRESS_DEFAULTS, \
     SAFETY_COLUMNS, evaluate, non_cooperative_mask
 from rl_collision_avoidance_b200.latency import LATENCY_FLAGS, Latency, add_latency_arguments, \
@@ -115,6 +122,7 @@ def main(argv=None):
                          'implies --timeouts' % PROGRESS_DEFAULTS['window'])
     add_noise_arguments(ap)
     add_latency_arguments(ap)
+    add_dynamics_arguments(ap)
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -149,6 +157,7 @@ def main(argv=None):
     if args.baseline is not None and args.scan_delay is not None:
         ap.error('--scan-delay applies to --policy only: the ORCA baselines do not read the scan')
     latency_params = latency_from_arguments(ap, args)
+    dynamics_params = dynamics_from_arguments(ap, args)
     hybrid_params = None
     if args.hybrid:
         hybrid_params = dict(HYBRID_DEFAULTS)
@@ -190,8 +199,9 @@ def main(argv=None):
     hy = Hybrid(env, **hybrid_params) if args.hybrid else None
     noise = Noise(env, noise_params) if noise_params is not None else None
     latency = Latency(env, latency_params) if latency_params is not None else None
+    dynamics = Dynamics(env, dynamics_params) if dynamics_params is not None else None
     out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy,
-                   safety=safety, progress=progress, noise=noise, latency=latency)
+                   safety=safety, progress=progress, noise=noise, latency=latency, dynamics=dynamics)
 
     def line(m, robots, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -210,6 +220,11 @@ def main(argv=None):
         ls = out['latency']
         print('latency  scan delay %d..%d ticks  command delay %d..%d ticks  (tick %g s)  seed %d'
               % (*ls['scan_delay'], *ls['command_delay'], env.cfg.dt, ls['seed']))
+    if dynamics is not None:
+        ds = out['dynamics']
+        limit = lambda r, unit: 'off' if r[1] == 0 else ('%g' % r[0] if r[0] == r[1] else '%g..%g' % tuple(r)) + unit
+        print('dynamics  linear accel limit %s  angular accel limit %s  (tick %g s)  seed %d'
+              % (limit(ds['linear'], ' m/s^2'), limit(ds['angular'], ' rad/s^2'), env.cfg.dt, ds['seed']))
     line(m, env.N)
     if nc is not None:
         k = args.non_cooperative * args.num_worlds
@@ -253,7 +268,8 @@ def main(argv=None):
         hidden = (() if safety is not None else ('safety', 'near_miss')) + \
             (() if progress is not None else ('timeouts', 'stall_window')) + \
             (() if noise is not None else tuple(f[2:].replace('-', '_') for f in NOISE_FLAGS)) + \
-            (() if latency is not None else tuple(f[2:].replace('-', '_') for f in LATENCY_FLAGS))
+            (() if latency is not None else tuple(f[2:].replace('-', '_') for f in LATENCY_FLAGS)) + \
+            (() if dynamics is not None else tuple(f[2:].replace('-', '_') for f in DYNAMICS_FLAGS))
         shown = {k: v for k, v in vars(args).items() if k not in hidden}
         res = {'args': shown, 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
@@ -263,6 +279,8 @@ def main(argv=None):
             res['noise'] = out['noise']
         if latency is not None:
             res['latency'] = out['latency']
+        if dynamics is not None:
+            res['dynamics'] = out['dynamics']
         if nc is not None:
             res['by_role'] = out['by_role']
             res['partials_split'] = out['partials_split'].tolist()

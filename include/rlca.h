@@ -1028,6 +1028,57 @@ int rlca_latency_action_host(const rlca_env_config *cfg, const rlca_latency_para
                              uint32_t draw, const unsigned char *flags_host, const float *action_in_host,
                              float *action_out_host);
 
+/* =====================================================================================
+ * Acceleration limits (csrc/rlca_dynamics.cu, DESIGN.md §9r): a separate launch just before the tick, issued only when
+ * a run asks for limits; the tick itself and its outputs are untouched.
+ *
+ * Limits: an agent draws its linear limit a in [lin_lo, lin_hi] m/s^2 and its angular limit b in [ang_lo, ang_hi]
+ * rad/s^2 when it starts an episode (a row whose flags[4 a + 3], was_reset, is set, or every row when flags is NULL),
+ * and holds them until its next one.  With w0, w1 the first two words of Philox-4x32-10 under the key (seed lo, seed
+ * hi) of the counter
+ *   (global agent = (world_offset + w) R + r, draw, 0, 0xE6 | stream_id << 8)
+ * (one-byte purpose; the environment uses 1-5, the sampler 0x5A17, noise 0xE1-0xE3, latency 0xE4-0xE5),
+ * a = lin_lo + (lin_hi - lin_lo) u0 and b = ang_lo + (ang_hi - ang_lo) u1 with u = (w >> 8) 2^-24, in float32.
+ * `draw` is the caller's own counter of calls, 0, 1, 2, ...
+ *
+ * Rule, per component, before the tick with the flags of the PREVIOUS tick (NULL on a run's first tick): the target is
+ * what the tick would execute (a value with |x| > 3e38 or NaN becomes 0, then the clip to [v_min, v_max] / [w_min,
+ * w_max]); prev is the agent's executed velocity of the last call, or (0, 0) for a fresh row and for a row whose
+ * flags[4 a + 1] (crashed) is set; d = target - prev, s = limit * cfg->dt; the executed value is prev + s if d > s,
+ * prev - s if d < -s, and the target itself otherwise.  It is written to action_out and stored in vel.  A kind whose
+ * range is (0, 0) is off: its component is the target.  Limits that never bind therefore give the command the tick
+ * would execute anyway, bit for bit.  Every function is shared by the kernel and the host twin, built without
+ * contraction, so the two are equal bit for bit, and no limit depends on num_worlds, the launch shape or anything but
+ * the key and the counter.
+ * ===================================================================================== */
+#define RLCA_DYNAMICS_MAX_ACCEL 100
+typedef struct rlca_dynamics_params {
+    float lin_lo, lin_hi;        /* m/s^2; (0, 0) off, else finite with 0 < lo <= hi <= RLCA_DYNAMICS_MAX_ACCEL */
+    float ang_lo, ang_hi;        /* rad/s^2; the same */
+    uint64_t seed;
+    uint32_t stream_id;          /* < 2^24 */
+} rlca_dynamics_params;
+
+/* The state of one env handle's limits, in device memory for the device entry and host memory for the host twin;
+ * N = num_worlds R rows of this config.  The caller allocates it and keeps it from call to call. */
+typedef struct rlca_dynamics_state {
+    float *vel;                  /* (N, 2) float: the (v, w) each agent executed on the last call */
+    float *lin_limit;            /* (N,) float: the linear limit of each agent's episode, m/s^2 (0 when off) */
+    float *ang_limit;            /* (N,) float: the angular limit, rad/s^2 (0 when off) */
+} rlca_dynamics_state;
+
+/* Before a tick: the command the robots execute, action_out_dev (N, 2), from the command action_in_dev (N, 2), which is
+ * never written.  RLCA_ERR_INVALID for a NULL cfg, params, state, state buffer, action_in_dev or action_out_dev,
+ * robots_per_world outside 1..64, num_worlds < 1, world_offset < 0, a range that is not (0, 0) and not finite with
+ * 0 < lo <= hi <= RLCA_DYNAMICS_MAX_ACCEL, or stream_id >= 2^24. */
+int rlca_dynamics_action(const rlca_env_config *cfg, const rlca_dynamics_params *p, const rlca_dynamics_state *state,
+                         uint32_t draw, const unsigned char *flags_dev, const float *action_in_dev,
+                         float *action_out_dev, void *stream);
+/* The same on HOST buffers (state included) by a serial loop over the same code; the outputs equal the kernel's. */
+int rlca_dynamics_action_host(const rlca_env_config *cfg, const rlca_dynamics_params *p,
+                              const rlca_dynamics_state *state, uint32_t draw, const unsigned char *flags_host,
+                              const float *action_in_host, float *action_out_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

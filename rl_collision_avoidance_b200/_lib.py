@@ -115,6 +115,17 @@ class LatencyState(C.Structure):
                 ('cmd_delay', C.c_void_p)]
 
 
+class DynamicsParams(C.Structure):
+    """Mirror of rlca_dynamics_params (include/rlca.h)."""
+    _fields_ = [('lin_lo', C.c_float), ('lin_hi', C.c_float), ('ang_lo', C.c_float), ('ang_hi', C.c_float),
+                ('seed', C.c_uint64), ('stream_id', C.c_uint32)]
+
+
+class DynamicsState(C.Structure):
+    """Mirror of rlca_dynamics_state (include/rlca.h): device pointers, or host pointers for the host twin."""
+    _fields_ = [('vel', C.c_void_p), ('lin_limit', C.c_void_p), ('ang_limit', C.c_void_p)]
+
+
 # rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
 EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
                  'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
@@ -261,6 +272,10 @@ SYMBOLS = {
                                          C.c_uint32, _P, _P]),
     'rlca_latency_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LatencyParams), C.POINTER(LatencyState),
                                            C.c_uint32, _P, _P, _P]),
+    'rlca_dynamics_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(DynamicsParams), C.POINTER(DynamicsState),
+                                       C.c_uint32, _P, _P, _P, _P]),
+    'rlca_dynamics_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(DynamicsParams),
+                                            C.POINTER(DynamicsState), C.c_uint32, _P, _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

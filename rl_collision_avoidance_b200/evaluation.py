@@ -472,7 +472,7 @@ def metrics(tot):
 
 
 def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None,
-             progress=None, noise=None, latency=None):
+             progress=None, noise=None, latency=None, dynamics=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
@@ -514,7 +514,15 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     first stack and, after every tick, the stack the tick wrote get `latency.scan` (with env.flags) before any noise,
     and the command, after the circle rule and before noise, becomes `latency.action`'s executed command, with the
     flags of the previous tick (None on the first).  A circle robot stopped by the circle rule still runs out the
-    commands already queued.  The result then also holds 'latency' (the settings).  Scan delay needs a policy."""
+    commands already queued.  The result then also holds 'latency' (the settings).  Scan delay needs a policy.
+
+    With `dynamics` (a dynamics.Dynamics on `env`, DESIGN.md §9r) the robots have acceleration limits: the command,
+    last of all, after any noise, becomes `dynamics.action`'s executed command, with the flags of the previous tick
+    (None on the first).  A circle robot stopped by the circle rule brakes at its limit instead of stopping on the
+    spot.  The ORCA baselines command velocities like the policy, so the limits apply to them too.  The result then
+    also holds 'dynamics' (the settings)."""
+    if dynamics is not None and dynamics.env is not env:
+        raise ValueError('the dynamics belongs to another env')
     if latency is not None:
         if latency.env is not env:
             raise ValueError('the latency belongs to another env')
@@ -570,6 +578,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             scaled = latency.action(scaled, env.flags if tick > 0 else None)
         if noise is not None:
             scaled = noise.action(scaled)
+        if dynamics is not None:
+            scaled = dynamics.action(scaled, env.flags if tick > 0 else None)
         env.control_vel(scaled, stack_in=stacks[k], stack_out=stacks[1 - k])
         if latency is not None:
             latency.scan(stacks[1 - k], env.flags)
@@ -618,4 +628,6 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         out['noise'] = noise.settings()
     if latency is not None:
         out['latency'] = latency.settings()
+    if dynamics is not None:
+        out['dynamics'] = dynamics.settings()
     return out

@@ -79,6 +79,13 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def check_flags(env, dev, flags):
+    """ValueError unless `flags` is None or a contiguous (env.N, 4) uint8 tensor on the device `dev` of `env`"""
+    if flags is not None and (tuple(flags.shape) != (env.N, 4) or flags.dtype != torch.uint8 or
+                              not flags.is_contiguous() or flags.device != dev):
+        raise ValueError(f'flags must be a contiguous ({env.N}, 4) uint8 tensor on {env.device}')
+
+
 class Latency:
     """The latency of one env handle: its rings and per-robot delays.  `stream_id` tells apart the handles of one run
     (a mix component's index); the handle's world_offset tells apart the shards of a data-parallel run.  Every `scan`
@@ -120,12 +127,6 @@ class Latency:
         return self._cmd_delay.clone() if self._cmd_delay is not None else \
             torch.zeros(self.env.N, dtype=torch.uint8, device=self.env.device)
 
-    def _check_flags(self, flags):
-        env = self.env
-        if flags is not None and (tuple(flags.shape) != (env.N, 4) or flags.dtype != torch.uint8 or
-                                  not flags.is_contiguous() or flags.device != self._dev):
-            raise ValueError(f'flags must be a contiguous ({env.N}, 4) uint8 tensor on {env.device}')
-
     def scan(self, stack, flags=None):
         """After a tick (and any re-layout): replace the newest frame of `stack` (N, 3, beams) float32 in place with
         the frame of each robot's scan delay earlier, on the env's stream.  Rows whose flags[:, 3] (was_reset) is set,
@@ -135,7 +136,7 @@ class Latency:
         if tuple(stack.shape) != (env.N, 3, env.beam_mum) or stack.dtype != torch.float32 or \
                 not stack.is_contiguous() or stack.device != self._dev:
             raise ValueError(f'stack must be a contiguous ({env.N}, 3, {env.beam_mum}) float32 tensor on {env.device}')
-        self._check_flags(flags)
+        check_flags(env, self._dev, flags)
         draw = self.scan_calls
         self.scan_calls += 1
         if self.params.scan_on:
@@ -149,7 +150,7 @@ class Latency:
         episode and execute its first command until l ticks have passed.  Returns `self.executed`, one buffer reused by every call, or `cmd` itself when
         command latency is off."""
         env = self.env
-        self._check_flags(flags)
+        check_flags(env, self._dev, flags)
         draw = self.action_calls
         self.action_calls += 1
         if not self.params.command_on:

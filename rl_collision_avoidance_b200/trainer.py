@@ -17,6 +17,7 @@ import torch
 from .mix import MIX_AUTO_RESET, MIX_SCENARIOS, SLICE_ALIGN, check_aligned
 from .model.ppo import generate_action, generate_train_data, ppo_update_stage1, ppo_update_stage2
 from .model.utils import get_filter_index
+from .dynamics import Dynamics
 from .latency import Latency
 from .noise import Noise
 from .stage_world import RESULT_STRINGS
@@ -49,10 +50,11 @@ class Rollout:
 class _Component:
     """One env handle of a run and its views of the rollout: agent columns [a, b), sliced once."""
 
-    def __init__(self, env, ro, a, b, noise=None, latency=None):
+    def __init__(self, env, ro, a, b, noise=None, latency=None, dynamics=None):
         self.env, self.a, self.b = env, a, b
         self.noise = noise                              # noise.Noise of the env, or None
         self.latency = latency                          # latency.Latency of the env, or None
+        self.dynamics = dynamics                        # dynamics.Dynamics of the env, or None
         self.ticked = False                             # a tick has run, so self.flags holds its flags
         self.name = env.sc.name
         self.relayout = env.sc.layout is not None
@@ -89,14 +91,18 @@ class _Component:
         noise.action's command (ro.scaled, which PPO's actions were drawn with, is not written) and the stack the tick
         and the re-layout wrote is perturbed as a noisy robot would read it.  With latency the command is delayed
         first, with the flags of the tick before (at t = 0 slot H - 1 of the previous rollout, still intact; None on
-        the run's first tick), and the stack is delayed after the re-layout and before any noise."""
+        the run's first tick), and the stack is delayed after the re-layout and before any noise.  With dynamics the
+        command, last of all, is limited in acceleration, with the same flags of the tick before."""
         e = self.env
         cmd = self.scaled
+        prev = self.flags[t - 1] if t > 0 else self.flags[-1] if self.ticked else None
         if self.latency is not None:
-            cmd = self.latency.action(cmd, self.flags[t - 1] if t > 0 else self.flags[-1] if self.ticked else None)
+            cmd = self.latency.action(cmd, prev)
         self.ticked = True
         if self.noise is not None:
             cmd = self.noise.action(cmd)
+        if self.dynamics is not None:
+            cmd = self.dynamics.action(cmd, prev)
         e.control_vel(cmd, live=e.live if self.relayout else None, stack_in=self.stacks[t],
                       stack_out=self.stacks[t + 1],
                       out={'reward': self.rewards[t], 'flags': self.flags[t], 'gs': self.gs[t + 1],
@@ -109,15 +115,16 @@ class _Component:
             self.noise.scan(self.stacks[t + 1], self.flags[t])
 
 
-def compose(envs, ro, noise=None, latency=None):
+def compose(envs, ro, noise=None, latency=None, dynamics=None):
     """The components of `envs` on the rollout `ro`: env k owns the agent columns that follow env k - 1's.  With more
     than one env, ValueError for a slice the kernels cannot read at its alignment (mix.SLICE_ALIGN).  `noise`
-    (noise.NoiseParams) gives component k a noise.Noise with stream id k, and `latency` (latency.LatencyParams) a
-    latency.Latency with stream id k."""
+    (noise.NoiseParams) gives component k a noise.Noise with stream id k, `latency` (latency.LatencyParams) a
+    latency.Latency with stream id k and `dynamics` (dynamics.DynamicsParams) a dynamics.Dynamics with stream id k."""
     comps, a = [], 0
     for k, e in enumerate(envs):
         comps.append(_Component(e, ro, a, a + e.N, None if noise is None else Noise(e, noise, stream_id=k),
-                                None if latency is None else Latency(e, latency, stream_id=k)))
+                                None if latency is None else Latency(e, latency, stream_id=k),
+                                None if dynamics is None else Dynamics(e, dynamics, stream_id=k)))
         a += e.N
     if a != ro.scaled.shape[0]:
         raise ValueError('the envs hold %d agents, the rollout %d' % (a, ro.scaled.shape[0]))
@@ -151,7 +158,7 @@ def _check_mix(envs, stage):
 
 def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logger_cal=None, stage=1, max_updates=None,
         process_group=None, rank=0, save_every=20, generator=None, start_update=0, diagnostics=False, target_kl=None,
-        noise=None, latency=None):
+        noise=None, latency=None, dynamics=None):
     """hp: dict with HORIZON, GAMMA, LAMDA, BATCH_SIZE, EPOCH, COEFF_ENTROPY, CLIP_VALUE, NUM_ENV, OBS_SIZE, ACT_SIZE,
     LASER_HIST, MAX_EPISODES.  `start_update` continues the checkpoint numbering of a resumed run.
     A random scenario (env.sc.layout, DESIGN.md §9k) trains with stage 2's update on per-world layouts: the env runs
@@ -171,6 +178,9 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     `latency` (latency.LatencyParams, DESIGN.md §9q) trains under sensing and command latency: component k gets a
     latency.Latency with stream id k, its robots execute the command of l ticks earlier and read the scan of d ticks
     earlier, both before any noise; PPO still stores the issued action and its log-probability.  None launches nothing.
+    `dynamics` (dynamics.DynamicsParams, DESIGN.md §9r) trains under acceleration limits: component k gets a
+    dynamics.Dynamics with stream id k, applied to the command last, after any noise; PPO still stores the issued
+    action.  None launches nothing.
     Returns per-update stats (for tests / benchmarks); 'by_scenario' splits the episodes by component."""
     envs = list(env) if isinstance(env, (list, tuple)) else [env]
     if not envs:
@@ -185,8 +195,11 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     H, N = hp['HORIZON'], sum(e.N for e in envs)
     dev = envs[0].device
     ro = Rollout(H, N, envs[0].beam_mum, dev)
-    # without latency, compose is called as it always was, so wrappers of its older signature keep working
-    comps = compose(envs, ro, noise) if latency is None else compose(envs, ro, noise, latency)
+    # without latency or dynamics, compose is called as it always was, so wrappers of its older signature keep working
+    if dynamics is not None:
+        comps = compose(envs, ro, noise, latency, dynamics)
+    else:
+        comps = compose(envs, ro, noise) if latency is None else compose(envs, ro, noise, latency)
     col_comp = np.repeat(np.arange(len(comps)), [e.N for e in envs])     # component of every agent column
     for c in comps:
         c.start()
