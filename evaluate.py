@@ -28,6 +28,11 @@ robot and episode from --latency-seed (default --seed; DESIGN.md §9q).  Only --
 --accel-limit A[,A_MAX] and --angular-accel-limit B[,B_MAX] evaluate under acceleration limits: each tick the executed v
 changes by at most A dt and w by at most B dt, with limits drawn in A..A_MAX and B..B_MAX per robot and episode from
 --dynamics-seed (default --seed; DESIGN.md §9r).  They apply to the baselines too.
+--pose-error S[,S_MAX], --heading-error S[,S_MAX] and --speed-error SV[,SW] evaluate under localization error: the
+policy's local goal is computed from a believed pose whose position and heading errors have standard deviations S m and
+S rad (or drawn in S..S_MAX per robot and episode) and a correlation time of --pose-error-time T s (default 2; 0 new on
+every tick, inf one offset per episode), and the speed it reads carries white noise, from --localization-seed (default
+--seed; DESIGN.md §9s).  Success, crashes and every metric stay on the true poses.  --policy only, not --hybrid.
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -48,6 +53,8 @@ changes by at most A dt and w by at most B dt, with limits drawn in A..A_MAX and
         --scan-delay 2 --command-delay 1,3
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
         --accel-limit 1 --angular-accel-limit 2
+    python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
+        --pose-error 0.1,0.3 --heading-error 0.05 --speed-error 0.05,0.1
 """
 import argparse
 import json
@@ -62,6 +69,8 @@ from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, PROGRESS
     SAFETY_COLUMNS, evaluate, non_cooperative_mask
 from rl_collision_avoidance_b200.latency import LATENCY_FLAGS, Latency, add_latency_arguments, \
     latency_from_arguments
+from rl_collision_avoidance_b200.localization import LOCALIZATION_FLAGS, Localization, add_localization_arguments, \
+    localization_from_arguments
 from rl_collision_avoidance_b200.model.net import CNNPolicy
 from rl_collision_avoidance_b200.noise import NOISE_FLAGS, Noise, add_noise_arguments, noise_from_arguments
 from rl_collision_avoidance_b200.orca import HYBRID_DEFAULTS, Hybrid, NonCooperative, \
@@ -123,6 +132,7 @@ def main(argv=None):
     add_noise_arguments(ap)
     add_latency_arguments(ap)
     add_dynamics_arguments(ap)
+    add_localization_arguments(ap)
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -158,6 +168,10 @@ def main(argv=None):
         ap.error('--scan-delay applies to --policy only: the ORCA baselines do not read the scan')
     latency_params = latency_from_arguments(ap, args)
     dynamics_params = dynamics_from_arguments(ap, args)
+    localization_params = localization_from_arguments(ap, args)
+    if localization_params is not None and (args.baseline is not None or args.hybrid):
+        ap.error('--pose-error / --heading-error / --speed-error apply to --policy without --hybrid only: the ORCA '
+                 'baselines and the hybrid driver read the true state')
     hybrid_params = None
     if args.hybrid:
         hybrid_params = dict(HYBRID_DEFAULTS)
@@ -200,8 +214,10 @@ def main(argv=None):
     noise = Noise(env, noise_params) if noise_params is not None else None
     latency = Latency(env, latency_params) if latency_params is not None else None
     dynamics = Dynamics(env, dynamics_params) if dynamics_params is not None else None
+    localization = Localization(env, localization_params) if localization_params is not None else None
     out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy,
-                   safety=safety, progress=progress, noise=noise, latency=latency, dynamics=dynamics)
+                   safety=safety, progress=progress, noise=noise, latency=latency, dynamics=dynamics,
+                   localization=localization)
 
     def line(m, robots, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -225,6 +241,12 @@ def main(argv=None):
         limit = lambda r, unit: 'off' if r[1] == 0 else ('%g' % r[0] if r[0] == r[1] else '%g..%g' % tuple(r)) + unit
         print('dynamics  linear accel limit %s  angular accel limit %s  (tick %g s)  seed %d'
               % (limit(ds['linear'], ' m/s^2'), limit(ds['angular'], ' rad/s^2'), env.cfg.dt, ds['seed']))
+    if localization is not None:
+        lo = out['localization']
+        sig = lambda r, unit: 'off' if r[1] == 0 else ('%g' % r[0] if r[0] == r[1] else '%g..%g' % tuple(r)) + unit
+        print('localization  pose sigma %s  heading sigma %s  correlation time %g s  speed sigma %g m/s %g rad/s  '
+              'seed %d' % (sig(lo['pose_sigma'], ' m'), sig(lo['heading_sigma'], ' rad'), lo['correlation_time'],
+                           *lo['speed_sigma'], lo['seed']))
     line(m, env.N)
     if nc is not None:
         k = args.non_cooperative * args.num_worlds
@@ -269,7 +291,8 @@ def main(argv=None):
             (() if progress is not None else ('timeouts', 'stall_window')) + \
             (() if noise is not None else tuple(f[2:].replace('-', '_') for f in NOISE_FLAGS)) + \
             (() if latency is not None else tuple(f[2:].replace('-', '_') for f in LATENCY_FLAGS)) + \
-            (() if dynamics is not None else tuple(f[2:].replace('-', '_') for f in DYNAMICS_FLAGS))
+            (() if dynamics is not None else tuple(f[2:].replace('-', '_') for f in DYNAMICS_FLAGS)) + \
+            (() if localization is not None else tuple(f[2:].replace('-', '_') for f in LOCALIZATION_FLAGS))
         shown = {k: v for k, v in vars(args).items() if k not in hidden}
         res = {'args': shown, 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
@@ -281,6 +304,8 @@ def main(argv=None):
             res['latency'] = out['latency']
         if dynamics is not None:
             res['dynamics'] = out['dynamics']
+        if localization is not None:
+            res['localization'] = out['localization']
         if nc is not None:
             res['by_role'] = out['by_role']
             res['partials_split'] = out['partials_split'].tolist()

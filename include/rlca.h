@@ -1079,6 +1079,67 @@ int rlca_dynamics_action_host(const rlca_env_config *cfg, const rlca_dynamics_pa
                               const rlca_dynamics_state *state, uint32_t draw, const unsigned char *flags_host,
                               const float *action_in_host, float *action_out_host);
 
+/* =====================================================================================
+ * Localization error (csrc/rlca_localization.cu, DESIGN.md §9s): a separate launch after the tick, issued only when a
+ * run asks for it; the tick itself, its state and its outputs are untouched, so success, crashes, rewards and every
+ * tracker stay on the true state.  It changes only what the policy reads as gs: the local goal and the speed.
+ *
+ * Error process: each agent holds a pose-estimate error e = (ex, ey, etheta) in the world frame.  Each call, per
+ * component, e <- rho e + kappa sigma xi with xi ~ N(0, 1), rho = exp(-dt / tau) and kappa = sqrt(1 - rho^2), both
+ * computed once per call on the host in double and rounded to float (tau = 0: rho = 0, kappa = 1, white jitter;
+ * tau = +inf: rho = 1, kappa = 0, and e is held as it is, a constant offset for the episode).  sigma is sigma_xy for
+ * ex and ey and sigma_theta for etheta.  A row starts an episode (every row when flags is NULL, else a row whose
+ * flags[4 a + 3], was_reset, of the tick just run is set): it draws sigma_xy in [xy_lo, xy_hi] and sigma_theta in
+ * [theta_lo, theta_hi] and starts from the stationary distribution, e = sigma xi.
+ *
+ * What the policy reads, gs_out[a]: the local goal of goal_speed (the tick's own rule) at the believed pose
+ * (x + ex, y + ey, theta + etheta) with dev_sincosf(theta + etheta), where a component whose error is exactly 0 keeps
+ * the true value as it is (so zero error gives the tick's gs bit for bit, -0 included); and the speed gs_in[a].zw plus
+ * N(0, v_sigma^2) and N(0, w_sigma^2) noise, fresh every call (a sigma of 0 keeps the value as it is).  The goal comes
+ * from the env state's goal, the pose from its pose; gs_in is read for the speed only.
+ *
+ * Draws: with c = Philox-4x32-10 under the key (seed lo, seed hi) of the counter
+ *   (global agent = (world_offset + w) R + r, draw, group, 0xE7 | stream_id << 8)
+ * (one-byte purpose; the environment uses 1-5, the sampler 0x5A17, noise 0xE1-0xE3, latency 0xE4-0xE5, dynamics 0xE6),
+ * group 0 gives the normals of ex, ey (Box-Muller of words 0, 1) and etheta, v (words 2, 3), and group 1 the normal of
+ * w (words 0, 1) and the uniforms u = (w >> 8) 2^-24 of sigma_xy = xy_lo + (xy_hi - xy_lo) u2 and sigma_theta =
+ * theta_lo + (theta_hi - theta_lo) u3.  Box-Muller is noise's (§9p).  `draw` is the caller's own counter of calls,
+ * 0, 1, 2, ...  Every function is shared by the kernel and the host twin, built without contraction, so the two are
+ * equal bit for bit, and no value depends on num_worlds, the launch shape or anything but the key and the counter.
+ * ===================================================================================== */
+typedef struct rlca_localization_params {
+    float xy_lo, xy_hi;          /* m; finite, 0 <= lo <= hi */
+    float theta_lo, theta_hi;    /* rad; the same */
+    float tau;                   /* s; >= 0 or +inf */
+    float v_sigma, w_sigma;      /* m/s, rad/s; finite, >= 0 */
+    uint64_t seed;
+    uint32_t stream_id;          /* < 2^24 */
+} rlca_localization_params;
+
+/* The state of one env handle's localization error, in device memory for the device entry and host memory for the
+ * host twin; N = num_worlds R rows of this config.  The caller allocates it and keeps it from call to call. */
+typedef struct rlca_localization_state {
+    float *err;                  /* (N, 4) float: ex, ey, etheta of each agent, and a pad */
+    float *sigma;                /* (N, 2) float: sigma_xy and sigma_theta of each agent's episode */
+} rlca_localization_state;
+
+/* After a tick (and any re-layout, latency and noise): the believed gs, gs_out_dev (N, 4), from the env state the tick
+ * just wrote (state_env: pose_dev and goal_dev are read, nothing is written) and the true gs_in_dev (N, 4).  gs_in_dev
+ * may equal gs_out_dev (in place).  RLCA_ERR_INVALID for a NULL cfg, params, state, state buffer, state_env, pose or
+ * goal buffer, gs_in_dev or gs_out_dev, robots_per_world outside 1..64, num_worlds < 1, world_offset < 0, a sigma
+ * range that is not finite with 0 <= lo <= hi, a speed sigma that is not finite and >= 0, tau that is not >= 0 or +inf,
+ * or stream_id >= 2^24. */
+int rlca_localization_observe(const rlca_env_config *cfg, const rlca_localization_params *p,
+                              const rlca_localization_state *state, uint32_t draw, const unsigned char *flags_dev,
+                              const rlca_env_state *state_env, const float *gs_in_dev, float *gs_out_dev,
+                              void *stream);
+/* The same on HOST buffers (state and env state included) by a serial loop over the same code; the outputs equal the
+ * kernel's. */
+int rlca_localization_observe_host(const rlca_env_config *cfg, const rlca_localization_params *p,
+                                   const rlca_localization_state *state, uint32_t draw,
+                                   const unsigned char *flags_host, const rlca_env_state *state_host,
+                                   const float *gs_in_host, float *gs_out_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

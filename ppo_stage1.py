@@ -9,7 +9,8 @@ Fine-tuning on random layouts (DESIGN.md §9k) runs through ppo_stage2.py --scen
 train under lidar and actuation noise (DESIGN.md §9p), with any scenario or mix.  --scan-delay T[,T_MAX] and
 --command-delay T[,T_MAX] train under sensing and command latency, in ticks of 0.1 s (DESIGN.md §9q).
 --accel-limit A[,A_MAX] and --angular-accel-limit B[,B_MAX] train under acceleration limits, in m/s^2 and rad/s^2
-(DESIGN.md §9r).
+(DESIGN.md §9r).  --pose-error S[,S_MAX], --heading-error S[,S_MAX], --pose-error-time T and --speed-error SV[,SW]
+train under localization error in the policy's local goal and speed (DESIGN.md §9s).
 """
 import argparse
 import logging
@@ -21,6 +22,7 @@ import torch
 
 from rl_collision_avoidance_b200.dynamics import add_dynamics_arguments, dynamics_from_arguments
 from rl_collision_avoidance_b200.latency import add_latency_arguments, latency_from_arguments
+from rl_collision_avoidance_b200.localization import add_localization_arguments, localization_from_arguments
 from rl_collision_avoidance_b200.mix import MIX_AUTO_RESET, parse_mix, plan
 from rl_collision_avoidance_b200.model.diagnostics import check_target_kl, setup_diag_log
 from rl_collision_avoidance_b200.model.net import Adam, CNNPolicy
@@ -122,10 +124,12 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     add_noise_arguments(ap)
     add_latency_arguments(ap)
     add_dynamics_arguments(ap)
+    add_localization_arguments(ap)
     args = ap.parse_args(argv)
     noise = noise_from_arguments(ap, args)
     latency = latency_from_arguments(ap, args)
     dynamics = dynamics_from_arguments(ap, args)
+    localization = localization_from_arguments(ap, args)
     if args.target_kl is not None:
         try:
             args.target_kl = check_target_kl(args.target_kl)
@@ -224,7 +228,7 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
         stats = run(env=env, policy=policy, policy_path=args.policy_path, action_bound=action_bound, optimizer=opt, hp=hp,
                     logger=logger, logger_cal=logger_cal, stage=stage, max_updates=args.updates, process_group=pg, rank=rank,
                     start_update=start_update, diagnostics=args.diagnostics, target_kl=args.target_kl, noise=noise,
-                    latency=latency, dynamics=dynamics)
+                    latency=latency, dynamics=dynamics, localization=localization)
         if rank == 0 and stats:
             s = stats[-1]
             print('update %d: rollout %.3fs update %.3fs -> %.0f agent-steps/s per GPU; mean ep reward %.2f' %

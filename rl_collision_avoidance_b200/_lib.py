@@ -126,6 +126,18 @@ class DynamicsState(C.Structure):
     _fields_ = [('vel', C.c_void_p), ('lin_limit', C.c_void_p), ('ang_limit', C.c_void_p)]
 
 
+class LocalizationParams(C.Structure):
+    """Mirror of rlca_localization_params (include/rlca.h)."""
+    _fields_ = [('xy_lo', C.c_float), ('xy_hi', C.c_float), ('theta_lo', C.c_float), ('theta_hi', C.c_float),
+                ('tau', C.c_float), ('v_sigma', C.c_float), ('w_sigma', C.c_float), ('seed', C.c_uint64),
+                ('stream_id', C.c_uint32)]
+
+
+class LocalizationState(C.Structure):
+    """Mirror of rlca_localization_state (include/rlca.h): device pointers, or host pointers for the host twin."""
+    _fields_ = [('err', C.c_void_p), ('sigma', C.c_void_p)]
+
+
 # rlca_eval_reduce partials per world (the RLCA_EVAL_* columns of include/rlca.h)
 EVAL_PARTIALS = ('reached', 'crashed', 'timed_out', 'unfinished', 'sum_time', 'sum_time_sq', 'sum_extra_time',
                  'sum_extra_time_sq', 'sum_extra_distance', 'sum_extra_distance_sq', 'sum_speed', 'sum_speed_sq',
@@ -276,6 +288,12 @@ SYMBOLS = {
                                        C.c_uint32, _P, _P, _P, _P]),
     'rlca_dynamics_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(DynamicsParams),
                                             C.POINTER(DynamicsState), C.c_uint32, _P, _P, _P]),
+    'rlca_localization_observe': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LocalizationParams),
+                                            C.POINTER(LocalizationState), C.c_uint32, _P, C.POINTER(EnvState), _P,
+                                            _P, _P]),
+    'rlca_localization_observe_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LocalizationParams),
+                                                 C.POINTER(LocalizationState), C.c_uint32, _P, C.POINTER(EnvState),
+                                                 _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

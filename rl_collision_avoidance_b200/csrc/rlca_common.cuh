@@ -152,3 +152,24 @@ __host__ __device__ __forceinline__ float dev_logf(float x)
     y = fmaf(-0.5f, z, y);
     return fmaf(fe, 0.693359375f, f + y);
 }
+
+// Box-Muller on the Philox words (a, b) (noise, DESIGN.md §9p; localization, §9s): u1 = ((a >> 8) + 1) 2^-24 in
+// (0, 1], u2 = (b >> 8) 2^-24
+__host__ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float &z0, float &z1)
+{
+    const float u1 = ((float)(a >> 8) + 1.0f) * 5.9604644775390625e-08f;
+    const float u2 = (float)(b >> 8) * 5.9604644775390625e-08f;
+    const float rho = sqrtf(-2.0f * dev_logf(u1));
+    float s, c;
+    dev_sincosf(6.28318548202514648438f * u2, s, c);
+    z0 = rho * c;
+    z1 = rho * s;
+}
+
+// the policy's goal / speed input: the goal in the robot's frame (heading sin s, cos c) and the last command (the tick,
+// rlca_env.cu; the believed goal of localization, §9s)
+__host__ __device__ __forceinline__ float4 goal_speed(const float4 &pose, const float4 &goal, float s, float c)
+{
+    const float ddx = goal.x - pose.x, ddy = goal.y - pose.y;
+    return make_float4(fmaf(ddx, c, ddy * s), fmaf(ddy, c, -(ddx * s)), goal.z, goal.w);
+}

@@ -41,18 +41,6 @@ __host__ __device__ __forceinline__ void noise_words(const NoiseArgs &q, uint32_
     dev_philox(c, q.k0, q.k1);
 }
 
-// Box-Muller on the words (a, b): u1 = ((a >> 8) + 1) 2^-24 in (0, 1], u2 = (b >> 8) 2^-24
-__host__ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float &z0, float &z1)
-{
-    const float u1 = ((float)(a >> 8) + 1.0f) * 5.9604644775390625e-08f;
-    const float u2 = (float)(b >> 8) * 5.9604644775390625e-08f;
-    const float rho = sqrtf(-2.0f * dev_logf(u1));
-    float s, c;
-    dev_sincosf(6.28318548202514648438f * u2, s, c);
-    z0 = rho * c;
-    z1 = rho * s;
-}
-
 // normals z (range noise) and uniforms u (dropout) of the four beams of group g; unused kinds are not drawn
 __host__ __device__ __forceinline__ void group_draws(const NoiseArgs &q, uint32_t agent, uint32_t g, float (&z)[4],
                                                      float (&u)[4])

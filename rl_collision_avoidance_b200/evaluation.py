@@ -472,7 +472,7 @@ def metrics(tot):
 
 
 def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None,
-             progress=None, noise=None, latency=None, dynamics=None):
+             progress=None, noise=None, latency=None, dynamics=None, localization=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
@@ -520,9 +520,23 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     last of all, after any noise, becomes `dynamics.action`'s executed command, with the flags of the previous tick
     (None on the first).  A circle robot stopped by the circle rule brakes at its limit instead of stopping on the
     spot.  The ORCA baselines command velocities like the policy, so the limits apply to them too.  The result then
-    also holds 'dynamics' (the settings)."""
+    also holds 'dynamics' (the settings).
+
+    With `localization` (a localization.Localization on `env`, DESIGN.md §9s) the policy reads its local goal from a
+    believed pose and its speed with odometry noise: at the start (flags None) and after every tick, after any latency
+    and noise have touched the stack, `localization.observe` with env.flags turns env.gs into the gs the policy reads
+    next.  env.gs and the state stay the truth, so success, crashes and every tracker measure the true poses.  The
+    result then also holds 'localization' (the settings).  Policies only, not hybrid: the ORCA baselines and the hybrid
+    driver read the true state through their own kernels; non-cooperative robots keep the truth."""
     if dynamics is not None and dynamics.env is not env:
         raise ValueError('the dynamics belongs to another env')
+    if localization is not None:
+        if localization.env is not env:
+            raise ValueError('the localization belongs to another env')
+        if isinstance(policy, (OrcaController, NhOrcaController)):
+            raise ValueError('localization error changes what a policy reads; the ORCA baselines read the true state')
+        if hybrid is not None:
+            raise ValueError('localization error changes what a policy reads; the hybrid driver reads the true state')
     if latency is not None:
         if latency.env is not env:
             raise ValueError('the latency belongs to another env')
@@ -557,6 +571,7 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         latency.scan(stacks[0])
     if noise is not None:
         noise.scan(stacks[0])
+    gs = localization.observe() if localization is not None else None
     terminal = torch.zeros(N, dtype=torch.bool, device=dev)
     goal_done = 1 if circle else E
     ticks = 0
@@ -565,9 +580,9 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         if isinstance(policy, (OrcaController, NhOrcaController)):
             scaled = policy()
         else:
-            _, scaled = generate_action_no_sampling(env=env, state_list=(stacks[k], env.get_local_goal(),
-                                                                         env.get_self_speed()),
-                                                    policy=policy, action_bound=ACTION_BOUND)
+            goal, speed = (env.get_local_goal(), env.get_self_speed()) if gs is None else (gs[:, 0:2], gs[:, 2:4])
+            _, scaled = generate_action_no_sampling(env=env, state_list=(stacks[k], goal, speed), policy=policy,
+                                                    action_bound=ACTION_BOUND)
             if hybrid is not None:
                 hybrid.apply(scaled, stacks[k], tracker)
         if non_cooperative is not None:
@@ -585,6 +600,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             latency.scan(stacks[1 - k], env.flags)
         if noise is not None:
             noise.scan(stacks[1 - k], env.flags)
+        if localization is not None:
+            gs = localization.observe(env.flags)
         if safe is not None:
             safe.track()
         if prog is not None:
@@ -630,4 +647,6 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         out['latency'] = latency.settings()
     if dynamics is not None:
         out['dynamics'] = dynamics.settings()
+    if localization is not None:
+        out['localization'] = localization.settings()
     return out

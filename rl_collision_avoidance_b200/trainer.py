@@ -19,6 +19,7 @@ from .model.ppo import generate_action, generate_train_data, ppo_update_stage1, 
 from .model.utils import get_filter_index
 from .dynamics import Dynamics
 from .latency import Latency
+from .localization import Localization
 from .noise import Noise
 from .stage_world import RESULT_STRINGS
 
@@ -50,11 +51,12 @@ class Rollout:
 class _Component:
     """One env handle of a run and its views of the rollout: agent columns [a, b), sliced once."""
 
-    def __init__(self, env, ro, a, b, noise=None, latency=None, dynamics=None):
+    def __init__(self, env, ro, a, b, noise=None, latency=None, dynamics=None, localization=None):
         self.env, self.a, self.b = env, a, b
         self.noise = noise                              # noise.Noise of the env, or None
         self.latency = latency                          # latency.Latency of the env, or None
         self.dynamics = dynamics                        # dynamics.Dynamics of the env, or None
+        self.localization = localization                # localization.Localization of the env, or None
         self.ticked = False                             # a tick has run, so self.flags holds its flags
         self.name = env.sc.name
         self.relayout = env.sc.layout is not None
@@ -85,6 +87,8 @@ class _Component:
         if self.noise is not None:
             self.noise.scan(self.stacks[0])             # what a noisy robot's first scan reads, in all three slots
         self.gs[0] = e.gs
+        if self.localization is not None:
+            self.localization.observe(gs=self.gs[0], out=self.gs[0])    # every row starts an episode
 
     def tick(self, t):
         """Tick t on the component's slices, after the policy has written ro.scaled.  With noise the robots execute
@@ -92,7 +96,9 @@ class _Component:
         and the re-layout wrote is perturbed as a noisy robot would read it.  With latency the command is delayed
         first, with the flags of the tick before (at t = 0 slot H - 1 of the previous rollout, still intact; None on
         the run's first tick), and the stack is delayed after the re-layout and before any noise.  With dynamics the
-        command, last of all, is limited in acceleration, with the same flags of the tick before."""
+        command, last of all, is limited in acceleration, with the same flags of the tick before.  With localization
+        the gs the tick and the re-layout wrote becomes, in place and last of all, the gs the robot believes, with the
+        flags of this tick."""
         e = self.env
         cmd = self.scaled
         prev = self.flags[t - 1] if t > 0 else self.flags[-1] if self.ticked else None
@@ -113,18 +119,22 @@ class _Component:
             self.latency.scan(self.stacks[t + 1], self.flags[t])
         if self.noise is not None:
             self.noise.scan(self.stacks[t + 1], self.flags[t])
+        if self.localization is not None:
+            self.localization.observe(self.flags[t], gs=self.gs[t + 1], out=self.gs[t + 1])
 
 
-def compose(envs, ro, noise=None, latency=None, dynamics=None):
+def compose(envs, ro, noise=None, latency=None, dynamics=None, localization=None):
     """The components of `envs` on the rollout `ro`: env k owns the agent columns that follow env k - 1's.  With more
     than one env, ValueError for a slice the kernels cannot read at its alignment (mix.SLICE_ALIGN).  `noise`
     (noise.NoiseParams) gives component k a noise.Noise with stream id k, `latency` (latency.LatencyParams) a
-    latency.Latency with stream id k and `dynamics` (dynamics.DynamicsParams) a dynamics.Dynamics with stream id k."""
+    latency.Latency with stream id k, `dynamics` (dynamics.DynamicsParams) a dynamics.Dynamics with stream id k and
+    `localization` (localization.LocalizationParams) a localization.Localization with stream id k."""
     comps, a = [], 0
     for k, e in enumerate(envs):
         comps.append(_Component(e, ro, a, a + e.N, None if noise is None else Noise(e, noise, stream_id=k),
                                 None if latency is None else Latency(e, latency, stream_id=k),
-                                None if dynamics is None else Dynamics(e, dynamics, stream_id=k)))
+                                None if dynamics is None else Dynamics(e, dynamics, stream_id=k),
+                                None if localization is None else Localization(e, localization, stream_id=k)))
         a += e.N
     if a != ro.scaled.shape[0]:
         raise ValueError('the envs hold %d agents, the rollout %d' % (a, ro.scaled.shape[0]))
@@ -158,7 +168,7 @@ def _check_mix(envs, stage):
 
 def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logger_cal=None, stage=1, max_updates=None,
         process_group=None, rank=0, save_every=20, generator=None, start_update=0, diagnostics=False, target_kl=None,
-        noise=None, latency=None, dynamics=None):
+        noise=None, latency=None, dynamics=None, localization=None):
     """hp: dict with HORIZON, GAMMA, LAMDA, BATCH_SIZE, EPOCH, COEFF_ENTROPY, CLIP_VALUE, NUM_ENV, OBS_SIZE, ACT_SIZE,
     LASER_HIST, MAX_EPISODES.  `start_update` continues the checkpoint numbering of a resumed run.
     A random scenario (env.sc.layout, DESIGN.md §9k) trains with stage 2's update on per-world layouts: the env runs
@@ -181,6 +191,10 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     `dynamics` (dynamics.DynamicsParams, DESIGN.md §9r) trains under acceleration limits: component k gets a
     dynamics.Dynamics with stream id k, applied to the command last, after any noise; PPO still stores the issued
     action.  None launches nothing.
+    `localization` (localization.LocalizationParams, DESIGN.md §9s) trains under localization error: component k gets
+    a localization.Localization with stream id k, and every gs the policy reads (ro.gs, slot 0 and every slot a tick
+    wrote, after any re-layout) is the believed one, so PPO stores and re-evaluates what the policy read.  Rewards and
+    episode ends stay on the true state.  None launches nothing.
     Returns per-update stats (for tests / benchmarks); 'by_scenario' splits the episodes by component."""
     envs = list(env) if isinstance(env, (list, tuple)) else [env]
     if not envs:
@@ -195,8 +209,11 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     H, N = hp['HORIZON'], sum(e.N for e in envs)
     dev = envs[0].device
     ro = Rollout(H, N, envs[0].beam_mum, dev)
-    # without latency or dynamics, compose is called as it always was, so wrappers of its older signature keep working
-    if dynamics is not None:
+    # without latency, dynamics or localization, compose is called as it always was, so wrappers of its older
+    # signature keep working
+    if localization is not None:
+        comps = compose(envs, ro, noise, latency, dynamics, localization)
+    elif dynamics is not None:
         comps = compose(envs, ro, noise, latency, dynamics)
     else:
         comps = compose(envs, ro, noise) if latency is None else compose(envs, ro, noise, latency)
