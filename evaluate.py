@@ -33,6 +33,9 @@ policy's local goal is computed from a believed pose whose position and heading 
 S rad (or drawn in S..S_MAX per robot and episode) and a correlation time of --pose-error-time T s (default 2; 0 new on
 every tick, inf one offset per episode), and the speed it reads carries white noise, from --localization-seed (default
 --seed; DESIGN.md §9s).  Success, crashes and every metric stay on the true poses.  --policy only, not --hybrid.
+--crowd K makes K agents of every world a social-force crowd that avoids each other, the other agents (not with
+--crowd-ignores-robots) and, with --crowd-map, the static map, with --crowd-speed, --crowd-strength, --crowd-range and
+--crowd-side-bias; the metrics are also printed per role (DESIGN.md §9t).  Not with --non-cooperative.
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -55,6 +58,8 @@ every tick, inf one offset per episode), and the speed it reads carries white no
         --accel-limit 1 --angular-accel-limit 2
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
         --pose-error 0.1,0.3 --heading-error 0.05 --speed-error 0.05,0.1
+    python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
+        --crowd 5 --crowd-map
 """
 import argparse
 import json
@@ -63,6 +68,7 @@ import os
 
 import torch
 
+from rl_collision_avoidance_b200.crowd import CROWD_FLAGS, Crowd, add_crowd_arguments, crowd_from_arguments
 from rl_collision_avoidance_b200.dynamics import DYNAMICS_FLAGS, Dynamics, add_dynamics_arguments, \
     dynamics_from_arguments
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, PROGRESS_COLUMNS, PROGRESS_DEFAULTS, \
@@ -108,6 +114,7 @@ def main(argv=None):
                          'everyone else; the metrics are also printed per role (DESIGN.md §9h)')
     ap.add_argument('--non-cooperative-speed', type=float, default=None, metavar='S',
                     help='speed of the non-cooperative robots, m/s, in (0, v_max] (default v_max)')
+    add_crowd_arguments(ap)
     ap.add_argument('--hybrid', action='store_true',
                     help='switch the policy per robot by its nearest scan return: drive straight to the goal in free '
                          'space, cap the speed near obstacles (DESIGN.md §9j)')
@@ -190,6 +197,9 @@ def main(argv=None):
         sc = make_scenario(args.scenario)
     if args.non_cooperative is not None and not 1 <= args.non_cooperative <= sc.robots_per_world:
         ap.error('--non-cooperative must be in 1..%d on %s' % (sc.robots_per_world, args.scenario))
+    if args.crowd is not None and not 1 <= args.crowd <= sc.robots_per_world:
+        ap.error('--crowd must be in 1..%d on %s' % (sc.robots_per_world, args.scenario))
+    crowd_params = crowd_from_arguments(ap, args, v_max)
     env = StageWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, seed=args.seed,
                      auto_reset=AUTO_RESET[args.scenario])
     if args.baseline is not None:
@@ -210,6 +220,12 @@ def main(argv=None):
     if args.non_cooperative is not None:
         nc = NonCooperative(env, non_cooperative_mask(sc.robots_per_world, args.num_worlds, args.non_cooperative),
                             speed=args.non_cooperative_speed)
+    crowd = None
+    if crowd_params is not None:
+        k, cp, crowd_map = crowd_params
+        crowd = Crowd(env, non_cooperative_mask(sc.robots_per_world, args.num_worlds, k), cp, obstacles=crowd_map)
+    masked = nc if nc is not None else crowd
+    role, label = ('crowd', 'crowd  ') if crowd is not None else ('non_cooperative', 'non-cooperative  ')
     hy = Hybrid(env, **hybrid_params) if args.hybrid else None
     noise = Noise(env, noise_params) if noise_params is not None else None
     latency = Latency(env, latency_params) if latency_params is not None else None
@@ -217,7 +233,7 @@ def main(argv=None):
     localization = Localization(env, localization_params) if localization_params is not None else None
     out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy,
                    safety=safety, progress=progress, noise=noise, latency=latency, dynamics=dynamics,
-                   localization=localization)
+                   localization=localization, crowd=crowd)
 
     def line(m, robots, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -248,29 +264,29 @@ def main(argv=None):
               'seed %d' % (sig(lo['pose_sigma'], ' m'), sig(lo['heading_sigma'], ' rad'), lo['correlation_time'],
                            *lo['speed_sigma'], lo['seed']))
     line(m, env.N)
-    if nc is not None:
-        k = args.non_cooperative * args.num_worlds
+    if masked is not None:
+        k = int(masked.mask.count_nonzero())
         line(out['by_role']['cooperative'], env.N - k, 'cooperative  ')
-        line(out['by_role']['non_cooperative'], k, 'non-cooperative  ')
+        line(out['by_role'][role], k, label)
     if hy is not None:
         s = out['modes']
         print('hybrid modes over %d %srobot-ticks: policy %.4f  driver %.4f  safe %.4f'
-              % (s['agent_ticks'], 'cooperative ' if nc is not None else '', s['policy'], s['driver'], s['safe']))
+              % (s['agent_ticks'], 'cooperative ' if masked is not None else '', s['policy'], s['driver'], s['safe']))
 
     def safety_line(m, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
         print('safety  %scrashes static %d  robot %d (both in range %d%s)  robot share %.4f  min separation %s m  '
               'min clearance %s m  near-miss rate %.4f (< %g m)  least separation %.3f m'
               % (role, m['crash_static'], m['crash_robot'], m['crash_both_in_range'],
-                 ', into non-cooperative %d' % m['crash_into_masked'] if nc is not None else '',
+                 ', into %s %d' % (label.strip(), m['crash_into_masked']) if masked is not None else '',
                  m['crash_robot_share'], f('min_separation_reached'), f('min_clearance_reached'), m['near_miss_rate'],
                  safety, m['min_separation']))
 
     if safety is not None:
         safety_line(out['safety'])
-        if nc is not None:
+        if masked is not None:
             safety_line(out['safety_by_role']['cooperative'], 'cooperative  ')
-            safety_line(out['safety_by_role']['non_cooperative'], 'non-cooperative  ')
+            safety_line(out['safety_by_role'][role], label)
 
     def progress_line(m, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -283,16 +299,17 @@ def main(argv=None):
 
     if progress is not None:
         progress_line(out['progress'])
-        if nc is not None:
+        if masked is not None:
             progress_line(out['progress_by_role']['cooperative'], 'cooperative  ')
-            progress_line(out['progress_by_role']['non_cooperative'], 'non-cooperative  ')
+            progress_line(out['progress_by_role'][role], label)
     if args.json:
         hidden = (() if safety is not None else ('safety', 'near_miss')) + \
             (() if progress is not None else ('timeouts', 'stall_window')) + \
             (() if noise is not None else tuple(f[2:].replace('-', '_') for f in NOISE_FLAGS)) + \
             (() if latency is not None else tuple(f[2:].replace('-', '_') for f in LATENCY_FLAGS)) + \
             (() if dynamics is not None else tuple(f[2:].replace('-', '_') for f in DYNAMICS_FLAGS)) + \
-            (() if localization is not None else tuple(f[2:].replace('-', '_') for f in LOCALIZATION_FLAGS))
+            (() if localization is not None else tuple(f[2:].replace('-', '_') for f in LOCALIZATION_FLAGS)) + \
+            (() if crowd is not None else ('crowd',) + tuple(f[2:].replace('-', '_') for f in CROWD_FLAGS))
         shown = {k: v for k, v in vars(args).items() if k not in hidden}
         res = {'args': shown, 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
@@ -306,7 +323,9 @@ def main(argv=None):
             res['dynamics'] = out['dynamics']
         if localization is not None:
             res['localization'] = out['localization']
-        if nc is not None:
+        if crowd is not None:
+            res['crowd'] = crowd.settings()
+        if masked is not None:
             res['by_role'] = out['by_role']
             res['partials_split'] = out['partials_split'].tolist()
         if hy is not None:
@@ -315,14 +334,14 @@ def main(argv=None):
         if safety is not None:
             res['safety'] = {'near_miss': safety, 'metrics': out['safety'], 'columns': list(SAFETY_COLUMNS),
                              'totals': out['safety_totals'].tolist(), 'partials': out['safety_partials'].tolist()}
-            if nc is not None:
+            if masked is not None:
                 res['safety']['by_role'] = out['safety_by_role']
                 res['safety']['partials_split'] = out['safety_partials_split'].tolist()
         if progress is not None:
             res['progress'] = {'params': out['progress_tracker'].params, 'metrics': out['progress'],
                                'columns': list(PROGRESS_COLUMNS), 'totals': out['progress_totals'].tolist(),
                                'partials': out['progress_partials'].tolist()}
-            if nc is not None:
+            if masked is not None:
                 res['progress']['by_role'] = out['progress_by_role']
                 res['progress']['partials_split'] = out['progress_partials_split'].tolist()
         with open(args.json, 'w') as fh:

@@ -511,6 +511,37 @@ int rlca_noncoop_action_host(const rlca_env_config *cfg, const float *pose_host,
                              const int32_t *meta_host, const uint8_t *mask_host, float speed, float heading_gain,
                              float *action_host);
 
+/* Social-force crowd (DESIGN.md §9t): masked agents driven by a Helbing-Molnar style social force that avoid each
+ * other, the static map and (see_robots != 0) the other agents.  action_dev (N,2) is read and written in place: for
+ * every agent i with mask_dev[i] != 0 (N uint8), from the state the next rlca_env_step reads, in float32:
+ *   p, heading (c, s), v = last command along the heading (0 when the stall flag is set);
+ *   u0 = the non-cooperative driver's preferred velocity at v_max = speed;  f = (u0 - v) (1 / relax_time);
+ *   for every other agent j of the world with 0 < d = |p_i - p_j| < neighbour_dist (see_robots == 0: mask[j] != 0
+ *   only), n = (p_i - p_j) / d, t = n rotated by +90 degrees, cos phi = -n . (c, s),
+ *   w = anisotropy + (1 - anisotropy)(1 + cos phi) / 2:  f += strength exp((2 radius - d) / range) w (n + side_bias t);
+ *   with an obstacle set, for every segment of the agent's bin list within wall_dist with the agent strictly on its
+ *   free side, q its nearest point, d = |p - q| > 0, n = (p - q) / d:
+ *   f += wall_strength exp((radius - d) / wall_range) n;
+ *   u = v + f cfg.dt on the disk of radius speed; the action is ORCA-DD's heading tracker on u with k_w = heading_gain
+ *   (w bounds from cfg).
+ * Rows with mask 0 are not touched; obstacles NULL is map-blind.  RLCA_ERR_INVALID for a NULL buffer, speed outside
+ * (0, cfg->v_max], relax_time, range, wall_range, radius, neighbour_dist or heading_gain not finite and > 0, strength
+ * or wall_strength not finite and >= 0, anisotropy outside [0, 1], side_bias not finite and >= 0, wall_dist not finite
+ * and > 0 or above the obstacle set's max_range. */
+typedef struct rlca_crowd_params {
+    float speed, relax_time, strength, range, anisotropy, side_bias, radius, neighbour_dist;
+    float wall_strength, wall_range, wall_dist, heading_gain;
+    int32_t see_robots;
+} rlca_crowd_params;
+int rlca_crowd_action(const rlca_env_config *cfg, const rlca_crowd_params *params, const rlca_env_state *state,
+                      const uint8_t *mask_dev, struct rlca_orca_obstacles *obstacles, float *action_dev, void *stream);
+/* The same from HOST buffers (pose, goal: (N,4) float; meta: (N,4) int32); equal to rlca_crowd_action bit for bit. */
+int rlca_crowd_action_host(const rlca_env_config *cfg, const rlca_crowd_params *params,
+                           struct rlca_orca_obstacles *obstacles, const float *pose_host, const float *goal_host,
+                           const int32_t *meta_host, const uint8_t *mask_host, float *action_host);
+/* The kernel's e^x (a cephes-style polynomial that rounds alike on host and device) on n host floats, for tests. */
+int rlca_crowd_expf_host(const float *x_host, int32_t n, float *out_host);
+
 /* Hybrid controller (DESIGN.md §9j): switches a policy's action per agent by the nearest return of its newest scan.
  * With m the minimum of frame 2 of the (N,3,beams) scan stack the tick reads (values scan / range_max - 0.5) and
  * d = (m + 0.5f) * cfg->range_max in metres, action_dev (N,2) is rewritten in place:

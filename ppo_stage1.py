@@ -10,7 +10,10 @@ train under lidar and actuation noise (DESIGN.md §9p), with any scenario or mix
 --command-delay T[,T_MAX] train under sensing and command latency, in ticks of 0.1 s (DESIGN.md §9q).
 --accel-limit A[,A_MAX] and --angular-accel-limit B[,B_MAX] train under acceleration limits, in m/s^2 and rad/s^2
 (DESIGN.md §9r).  --pose-error S[,S_MAX], --heading-error S[,S_MAX], --pose-error-time T and --speed-error SV[,SW]
-train under localization error in the policy's local goal and speed (DESIGN.md §9s).
+train under localization error in the policy's local goal and speed (DESIGN.md §9s).  --non-cooperative K
+[--non-cooperative-speed S] puts K straight-to-goal drivers into every world (DESIGN.md §9h), --crowd K (with
+--crowd-speed, --crowd-ignores-robots, --crowd-map, --crowd-strength, --crowd-range, --crowd-side-bias) K social-force
+crowd agents (DESIGN.md §9t); either way their rows are left out of every PPO update, with any scenario or mix.
 """
 import argparse
 import logging
@@ -20,6 +23,8 @@ import sys
 
 import torch
 
+from rl_collision_avoidance_b200.crowd import add_crowd_arguments, crowd_from_arguments, \
+    non_cooperative_from_arguments
 from rl_collision_avoidance_b200.dynamics import add_dynamics_arguments, dynamics_from_arguments
 from rl_collision_avoidance_b200.latency import add_latency_arguments, latency_from_arguments
 from rl_collision_avoidance_b200.localization import add_localization_arguments, localization_from_arguments
@@ -28,7 +33,7 @@ from rl_collision_avoidance_b200.model.diagnostics import check_target_kl, setup
 from rl_collision_avoidance_b200.model.net import Adam, CNNPolicy
 from rl_collision_avoidance_b200.model.ppo import setup_ppo_log
 from rl_collision_avoidance_b200.noise import add_noise_arguments, noise_from_arguments
-from rl_collision_avoidance_b200.scenarios import add_random_arguments, check_random_arguments, \
+from rl_collision_avoidance_b200.scenarios import COMMON, add_random_arguments, check_random_arguments, \
     random_scenario_from_arguments
 from rl_collision_avoidance_b200.stage_world import StageWorld as RandomWorld
 from rl_collision_avoidance_b200.stage_world1 import StageWorld
@@ -125,11 +130,14 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     add_latency_arguments(ap)
     add_dynamics_arguments(ap)
     add_localization_arguments(ap)
+    add_crowd_arguments(ap, non_cooperative=True)
     args = ap.parse_args(argv)
     noise = noise_from_arguments(ap, args)
     latency = latency_from_arguments(ap, args)
     dynamics = dynamics_from_arguments(ap, args)
     localization = localization_from_arguments(ap, args)
+    non_cooperative = non_cooperative_from_arguments(ap, args, COMMON['v_max'])
+    crowd = crowd_from_arguments(ap, args, COMMON['v_max'])
     if args.target_kl is not None:
         try:
             args.target_kl = check_target_kl(args.target_kl)
@@ -183,6 +191,11 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     else:
         env = world_cls(LASER_BEAM, index=0, num_env=num_env, num_worlds=args.num_worlds, device=device,
                         seed=args.seed, auto_reset=1 if stage == 1 else 2, world_offset=rank * args.num_worlds)
+    masked_k = non_cooperative[0] if non_cooperative is not None else crowd[0] if crowd is not None else None
+    least_r = min(e.cfg.robots_per_world for e in (env if comps is not None else [env]))
+    if masked_k is not None and masked_k > least_r:
+        ap.error('--%s must be in 1..%d: a world has %d robots'
+                 % ('crowd' if crowd is not None else 'non-cooperative', least_r, least_r))
     action_bound = [[0, -1], [1, 1]]
     n_agents = sum(e.N for e in env) if comps is not None else env.N
     policy = CNNPolicy(frames=LASER_HIST, action_space=2, device=device, seed=args.seed, max_batch=max(batch_size, n_agents))
@@ -228,13 +241,18 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
         stats = run(env=env, policy=policy, policy_path=args.policy_path, action_bound=action_bound, optimizer=opt, hp=hp,
                     logger=logger, logger_cal=logger_cal, stage=stage, max_updates=args.updates, process_group=pg, rank=rank,
                     start_update=start_update, diagnostics=args.diagnostics, target_kl=args.target_kl, noise=noise,
-                    latency=latency, dynamics=dynamics, localization=localization)
+                    latency=latency, dynamics=dynamics, localization=localization, non_cooperative=non_cooperative,
+                    crowd=crowd)
         if rank == 0 and stats:
             s = stats[-1]
             print('update %d: rollout %.3fs update %.3fs -> %.0f agent-steps/s per GPU; mean ep reward %.2f' %
                   (s['update'], s['rollout_s'], s['update_s'], s['agent_steps_per_s'], s['mean_ep_reward']))
             for c in comps or ():
                 print(component_summary(c, stats))
+            if 'by_role' in s:
+                for role, r in s['by_role'].items():
+                    print('last update, %s: %d episodes, success %.3f, crash %.3f'
+                          % (role, r['episodes'], r['success_rate'], r['crash_rate']))
     except KeyboardInterrupt:
         pass
     finally:

@@ -12,6 +12,10 @@ timing out after --random-timeout ticks (default 3 ceil(S sqrt(2) / (v_max dt)),
 --mix trains on several scenarios in one run (DESIGN.md §9l): stage 2, the circle and random layouts side by side,
 world counts per GPU, every PPO update over all of them (the --random-* flags shape the random component):
     python ppo_stage2.py --mix stage2:31,random:128,circle:14 --random-robots 16 --updates 100
+
+--crowd K puts K social-force crowd agents into every world (DESIGN.md §9t), --non-cooperative K K straight-to-goal
+drivers (§9h); their rows are left out of every PPO update:
+    python ppo_stage2.py --scenario random --random-robots 16 --num-worlds 128 --updates 100 --crowd 4 --crowd-map
 """
 from ppo_stage1 import main
 from rl_collision_avoidance_b200.stage_world2 import StageWorld

@@ -126,6 +126,13 @@ class DynamicsState(C.Structure):
     _fields_ = [('vel', C.c_void_p), ('lin_limit', C.c_void_p), ('ang_limit', C.c_void_p)]
 
 
+class CrowdParams(C.Structure):
+    """Mirror of rlca_crowd_params (include/rlca.h)."""
+    _fields_ = [(k, C.c_float) for k in ('speed', 'relax_time', 'strength', 'range', 'anisotropy', 'side_bias', 'radius',
+                                         'neighbour_dist', 'wall_strength', 'wall_range', 'wall_dist', 'heading_gain')] + \
+        [('see_robots', C.c_int32)]
+
+
 class LocalizationParams(C.Structure):
     """Mirror of rlca_localization_params (include/rlca.h)."""
     _fields_ = [('xy_lo', C.c_float), ('xy_hi', C.c_float), ('theta_lo', C.c_float), ('theta_hi', C.c_float),
@@ -221,6 +228,10 @@ SYMBOLS = {
                                         _P, _P, _P]),
     'rlca_noncoop_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(EnvState), _P, C.c_float, C.c_float, _P, _P]),
     'rlca_noncoop_action_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_float, C.c_float, _P]),
+    'rlca_crowd_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(CrowdParams), C.POINTER(EnvState), _P, _P, _P,
+                                    _P]),
+    'rlca_crowd_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(CrowdParams), _P, _P, _P, _P, _P, _P]),
+    'rlca_crowd_expf_host': (C.c_int, [_P, C.c_int32, _P]),
     'rlca_hybrid_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(HybridParams), C.POINTER(EnvState), _P, _P, _P,
                                      _P, _P, _P]),
     'rlca_hybrid_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(HybridParams), _P, _P, _P, _P, _P, _P, _P,

@@ -153,6 +153,36 @@ __host__ __device__ __forceinline__ float dev_logf(float x)
     return fmaf(fe, 0.693359375f, f + y);
 }
 
+// e^x under the same contract (crowd, DESIGN.md §9t): n = floor(x log2(e) + 1/2), r = x - n ln 2 in two parts, the
+// cephes expf polynomial on r (explicit FMAs only), then 2^n applied as two exact power-of-two scalings (2^n alone
+// overflows the exponent field at n = 128).  +inf above ln(FLT_MAX), 0 below ln(FLT_MIN); NaN stays NaN.
+__host__ __device__ __forceinline__ float dev_expf(float x)
+{
+    if (x > 88.7228394f) return INFINITY;
+    if (!(x >= -87.3365448f)) return x != x ? x : 0.0f;
+    const float n = floorf(fmaf(x, 1.44269504088896341f, 0.5f));
+    float r = fmaf(-n, 0.693359375f, x);
+    r = fmaf(-n, -2.12194440e-4f, r);
+    const float z = r * r;
+    float p = fmaf(1.9875691500e-4f, r, 1.3981999507e-3f);
+    p = fmaf(p, r, 8.3334519073e-3f);
+    p = fmaf(p, r, 4.1665795894e-2f);
+    p = fmaf(p, r, 1.6666665459e-1f);
+    p = fmaf(p, r, 5.0000001201e-1f);
+    p = fmaf(p, z, r) + 1.0f;
+    const int k = (int)n, k1 = k >> 1, k2 = k - k1;
+    const uint32_t b1 = (uint32_t)(k1 + 127) << 23, b2 = (uint32_t)(k2 + 127) << 23;
+    float s1, s2;
+#ifdef __CUDA_ARCH__
+    s1 = __uint_as_float(b1);
+    s2 = __uint_as_float(b2);
+#else
+    memcpy(&s1, &b1, sizeof(s1));
+    memcpy(&s2, &b2, sizeof(s2));
+#endif
+    return p * s1 * s2;
+}
+
 // Box-Muller on the Philox words (a, b) (noise, DESIGN.md §9p; localization, §9s): u1 = ((a >> 8) + 1) 2^-24 in
 // (0, 1], u2 = (b >> 8) 2^-24
 __host__ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float &z0, float &z1)

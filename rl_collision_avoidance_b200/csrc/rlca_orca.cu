@@ -1510,17 +1510,9 @@ extern "C" int rlca_orca_obstacles_segments(const rlca_orca_obstacles *obs, int3
     return RLCA_OK;
 }
 
-// The launch parameters for obstacle radius r_o and horizon tau_o; device = true takes (or makes) the device copy.
-static int obs_params(rlca_orca_obstacles *obs, const rlca_env_config *cfg, float r_o, float obstacle_time_horizon,
-                      bool device, ObsParams &m)
+// The set's segments and bins as a launch reads them; device = true takes (or makes) the device copy.
+static int obs_bins(rlca_orca_obstacles *obs, bool device, ObsParams &m)
 {
-    if (!obs) return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacles: the obstacle set is NULL");
-    if (!(obstacle_time_horizon > 0.0f && obstacle_time_horizon < INFINITY))
-        return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacle_time_horizon must be finite and > 0");
-    const float range = obstacle_time_horizon * cfg->v_max + r_o;
-    if (!(range <= obs->max_range))
-        return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacles: obstacle_time_horizon * v_max + obstacle radius exceeds "
-                                              "the set's max_range");
     if (device) {
         const int rc = obs_device(obs);
         if (rc) return rc;
@@ -1533,6 +1525,22 @@ static int obs_params(rlca_orca_obstacles *obs, const rlca_env_config *cfg, floa
     m.inv_bin = (float)(1.0 / OBS_BIN);
     m.nbx = obs->nbx;
     m.nby = obs->nby;
+    return RLCA_OK;
+}
+
+// The launch parameters for obstacle radius r_o and horizon tau_o; device = true takes (or makes) the device copy.
+static int obs_params(rlca_orca_obstacles *obs, const rlca_env_config *cfg, float r_o, float obstacle_time_horizon,
+                      bool device, ObsParams &m)
+{
+    if (!obs) return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacles: the obstacle set is NULL");
+    if (!(obstacle_time_horizon > 0.0f && obstacle_time_horizon < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacle_time_horizon must be finite and > 0");
+    const float range = obstacle_time_horizon * cfg->v_max + r_o;
+    if (!(range <= obs->max_range))
+        return rlca_set_err(RLCA_ERR_INVALID, "ORCA obstacles: obstacle_time_horizon * v_max + obstacle radius exceeds "
+                                              "the set's max_range");
+    const int rc = obs_bins(obs, device, m);
+    if (rc) return rc;
     m.range2 = range * range;
     m.inv_tau = 1.0f / obstacle_time_horizon;
     m.r = r_o;
@@ -1669,5 +1677,219 @@ extern "C" int rlca_orca_obstacle_lines_host(const rlca_env_config *cfg, rlca_or
     }
     *nlines = no;
     *dropped = d;
+    return RLCA_OK;
+}
+
+// ------------------------------------------------------------------------------------ social-force crowd (§9t)
+// Masked agents steer by a Helbing-Molnar style social force: a driving term towards the §9h driver's preferred
+// velocity, an anisotropic repulsion with a sideways bias from the other agents of the world, a repulsion from the
+// static map's segments, and ORCA-DD's heading tracker on the velocity that results.
+struct CrowdParams {
+    float inv_relax, strength, range, aniso, side_bias, two_r, nd;
+    float wall_strength, wall_range, radius, dt;
+    int32_t see_robots;
+};
+
+// The force an agent at (ox, oy) exerts on me, added to (fx, fy); none unless 0 < d < neighbour_dist.
+__host__ __device__ __forceinline__ void crowd_agent_force(const OrcaAgent &me, float ox, float oy,
+                                                           const CrowdParams &c, float &fx, float &fy)
+{
+    const float dx = me.px - ox, dy = me.py - oy, d = sqrtf(dx * dx + dy * dy);
+    if (!(d > 0.0f && d < c.nd)) return;
+    const float nx = dx / d, ny = dy / d, tx = -ny, ty = nx;
+    const float cphi = -(nx * me.ct + ny * me.st);
+    const float w = c.aniso + (1.0f - c.aniso) * (1.0f + cphi) * 0.5f;
+    const float k = c.strength * dev_expf((c.two_r - d) / c.range) * w;
+    fx += k * (nx + c.side_bias * tx);
+    fy += k * (ny + c.side_bias * ty);
+}
+
+// The force segment s exerts on me, added to (fx, fy), when it is a candidate (obs_candidate with m.range2 =
+// wall_dist^2); q is its nearest point, computed as obs_candidate computes it.
+__host__ __device__ __forceinline__ void crowd_wall_force(const OrcaAgent &me, const ObsSeg &s, const ObsParams &m,
+                                                          const CrowdParams &c, float &fx, float &fy)
+{
+    float d2;
+    if (!obs_candidate(me, s, m.range2, d2)) return;
+    const float r1x = s.x0 - me.px, r1y = s.y0 - me.py, ex = s.x1 - s.x0, ey = s.y1 - s.y0;
+    const float t = fminf(fmaxf(-(r1x * ex + r1y * ey) / (ex * ex + ey * ey), 0.0f), 1.0f);
+    const float qx = r1x + t * ex, qy = r1y + t * ey, d = sqrtf(d2);
+    if (!(d > 0.0f)) return;
+    const float k = c.wall_strength * dev_expf((c.radius - d) / c.wall_range);
+    fx += k * (-qx / d);
+    fy += k * (-qy / d);
+}
+
+// The action from the summed agent and wall forces (sx, sy): driving term, one Euler step on the speed disk, tracker.
+__host__ __device__ __forceinline__ float2 crowd_action(const OrcaAgent &me, float4 goal, const OrcaParams &q,
+                                                        const CrowdParams &c, float sx, float sy)
+{
+    float ox, oy, ux, uy;
+    orca_pref(me, goal, q, ox, oy);
+    const float fx = (ox - me.vx) * c.inv_relax + sx, fy = (oy - me.vy) * c.inv_relax + sy;
+    lp2_start(q.v_max, me.vx + fx * c.dt, me.vy + fy * c.dt, false, ux, uy);
+    return orca_track(me, ux, uy, q);
+}
+
+// One warp per agent; warps of unmasked agents return at once.  Lane l sums the forces of agents base + l, l + 32, ...
+// and then of bin entries b0 + l, b0 + l + 32, ..., in that order; the xor butterfly (offsets 16 .. 1) adds the
+// partials, and every lane ends with the same sum since each step adds the same two values on both lanes of a pair.
+template <bool MAP>
+__global__ void __launch_bounds__(ORCA_THREADS) rlca_crowd_kernel(int n, int R, OrcaParams q, CrowdParams c,
+                                                                   const float4 *__restrict__ pose,
+                                                                   const float4 *__restrict__ goal,
+                                                                   const int4 *__restrict__ meta,
+                                                                   const uint8_t *__restrict__ mask,
+                                                                   float2 *__restrict__ action, ObsParams om)
+{
+    const int a = blockIdx.x * ORCA_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (a >= n || !mask[a]) return;
+    const int base = a - a % R;
+    const OrcaAgent me = orca_agent(pose, goal, meta, a);
+    float fx = 0.0f, fy = 0.0f;
+    for (int j = lane; j < R; j += 32) {
+        const int b = base + j;
+        if (b != a && (c.see_robots || mask[b])) {
+            const float4 p = pose[b];
+            crowd_agent_force(me, p.x, p.y, c, fx, fy);
+        }
+    }
+    if (MAP) {
+        const int bin = obs_bin(om, me.px, me.py);
+        if (bin >= 0)
+            for (int k = om.bin_off[bin] + lane; k < om.bin_off[bin + 1]; k += 32)
+                crowd_wall_force(me, om.seg[om.bin_idx[k]], om, c, fx, fy);
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        fx += __shfl_xor_sync(FULL_MASK, fx, o);
+        fy += __shfl_xor_sync(FULL_MASK, fy, o);
+    }
+    if (lane == 0) action[a] = crowd_action(me, goal[a], q, c, fx, fy);
+}
+
+static int crowd_args(const rlca_env_config *cfg, const rlca_crowd_params *p, const rlca_orca_obstacles *obs,
+                      OrcaParams &q, CrowdParams &c)
+{
+    if (!cfg || !p) return rlca_set_err(RLCA_ERR_INVALID, "crowd: cfg or params is NULL");
+    const float pos[6] = {p->relax_time, p->range, p->wall_range, p->radius, p->neighbour_dist, p->heading_gain};
+    for (float x : pos)
+        if (!(x > 0.0f && x < INFINITY))
+            return rlca_set_err(RLCA_ERR_INVALID, "crowd: relax_time, range, wall_range, radius, neighbour_dist and "
+                                                  "heading_gain must be finite and > 0");
+    if (!(p->strength >= 0.0f && p->strength < INFINITY && p->wall_strength >= 0.0f && p->wall_strength < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "crowd: strength and wall_strength must be finite and >= 0");
+    if (!(p->anisotropy >= 0.0f && p->anisotropy <= 1.0f))
+        return rlca_set_err(RLCA_ERR_INVALID, "crowd: anisotropy must be in [0, 1]");
+    if (!(p->side_bias >= 0.0f && p->side_bias < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "crowd: side_bias must be finite and >= 0");
+    if (!(p->wall_dist > 0.0f && p->wall_dist < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "crowd: wall_dist must be finite and > 0");
+    if (obs && !(p->wall_dist <= obs->max_range))
+        return rlca_set_err(RLCA_ERR_INVALID, "crowd: wall_dist exceeds the obstacle set's max_range");
+    if (!(p->speed > 0.0f && p->speed <= cfg->v_max && p->speed < INFINITY))
+        return rlca_set_err(RLCA_ERR_INVALID, "crowd: speed must be finite and in (0, cfg.v_max]");
+    const int rc = noncoop_args(cfg, p->speed, p->heading_gain, q);
+    if (rc) return rc;
+    c.inv_relax = 1.0f / p->relax_time;
+    c.strength = p->strength;
+    c.range = p->range;
+    c.aniso = p->anisotropy;
+    c.side_bias = p->side_bias;
+    c.two_r = 2.0f * p->radius;
+    c.nd = p->neighbour_dist;
+    c.wall_strength = p->wall_strength;
+    c.wall_range = p->wall_range;
+    c.radius = p->radius;
+    c.dt = cfg->dt;
+    c.see_robots = p->see_robots != 0;
+    return RLCA_OK;
+}
+
+extern "C" int rlca_crowd_action(const rlca_env_config *cfg, const rlca_crowd_params *params,
+                                 const rlca_env_state *state, const uint8_t *mask_dev, rlca_orca_obstacles *obstacles,
+                                 float *action_dev, void *stream)
+{
+    OrcaParams q;
+    CrowdParams c;
+    ObsParams m = {};
+    int rc = crowd_args(cfg, params, obstacles, q, c);
+    if (rc) return rc;
+    if (!state || !state->pose_dev || !state->goal_dev || !state->meta_dev || !mask_dev || !action_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_crowd_action: state, mask or action buffer is NULL");
+    if (obstacles) {
+        rc = obs_bins(obstacles, true, m);
+        if (rc) return rc;
+        m.range2 = params->wall_dist * params->wall_dist;
+    }
+    const int n = cfg->robots_per_world * cfg->num_worlds;
+    const dim3 grid((n + ORCA_WARPS - 1) / ORCA_WARPS);
+    const float4 *pose = reinterpret_cast<const float4 *>(state->pose_dev);
+    const float4 *goal = reinterpret_cast<const float4 *>(state->goal_dev);
+    const int4 *meta = reinterpret_cast<const int4 *>(state->meta_dev);
+    float2 *action = reinterpret_cast<float2 *>(action_dev);
+    if (obstacles)
+        rlca_crowd_kernel<true><<<grid, ORCA_THREADS, 0, (cudaStream_t)stream>>>(
+            n, cfg->robots_per_world, q, c, pose, goal, meta, mask_dev, action, m);
+    else
+        rlca_crowd_kernel<false><<<grid, ORCA_THREADS, 0, (cudaStream_t)stream>>>(
+            n, cfg->robots_per_world, q, c, pose, goal, meta, mask_dev, action, m);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+// rlca_crowd_kernel by serial loops: the 32 lanes' partials in the same order, then the same butterfly.
+extern "C" int rlca_crowd_action_host(const rlca_env_config *cfg, const rlca_crowd_params *params,
+                                      rlca_orca_obstacles *obstacles, const float *pose_host, const float *goal_host,
+                                      const int32_t *meta_host, const uint8_t *mask_host, float *action_host)
+{
+    OrcaParams q;
+    CrowdParams c;
+    ObsParams m = {};
+    int rc = crowd_args(cfg, params, obstacles, q, c);
+    if (rc) return rc;
+    if (!pose_host || !goal_host || !meta_host || !mask_host || !action_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_crowd_action_host: a buffer is NULL");
+    if (obstacles) {
+        rc = obs_bins(obstacles, false, m);
+        if (rc) return rc;
+        m.range2 = params->wall_dist * params->wall_dist;
+    }
+    const float4 *pose = reinterpret_cast<const float4 *>(pose_host), *goal = reinterpret_cast<const float4 *>(goal_host);
+    const int4 *meta = reinterpret_cast<const int4 *>(meta_host);
+    const int R = cfg->robots_per_world, n = R * cfg->num_worlds;
+    for (int a = 0; a < n; ++a) {
+        if (!mask_host[a]) continue;
+        const int base = a - a % R;
+        const OrcaAgent me = orca_agent(pose, goal, meta, a);
+        float fx[32] = {}, fy[32] = {}, gx[32], gy[32];
+        for (int j = 0; j < R; ++j) {
+            const int b = base + j;
+            if (b != a && (c.see_robots || mask_host[b]))
+                crowd_agent_force(me, pose[b].x, pose[b].y, c, fx[j & 31], fy[j & 31]);
+        }
+        if (obstacles) {
+            const int bin = obs_bin(m, me.px, me.py);
+            if (bin >= 0)
+                for (int k = m.bin_off[bin]; k < m.bin_off[bin + 1]; ++k)
+                    crowd_wall_force(me, m.seg[m.bin_idx[k]], m, c, fx[(k - m.bin_off[bin]) & 31],
+                                     fy[(k - m.bin_off[bin]) & 31]);
+        }
+        for (int o = 16; o; o >>= 1) {
+            for (int l = 0; l < 32; ++l) { gx[l] = fx[l] + fx[l ^ o]; gy[l] = fy[l] + fy[l ^ o]; }
+            memcpy(fx, gx, sizeof fx);
+            memcpy(fy, gy, sizeof fy);
+        }
+        const float2 act = crowd_action(me, goal[a], q, c, fx[0], fy[0]);
+        action_host[2 * a] = act.x;
+        action_host[2 * a + 1] = act.y;
+    }
+    return RLCA_OK;
+}
+
+extern "C" int rlca_crowd_expf_host(const float *x_host, int32_t n, float *out_host)
+{
+    if (!x_host || !out_host || n < 0) return rlca_set_err(RLCA_ERR_INVALID, "rlca_crowd_expf_host: bad arguments");
+    for (int32_t i = 0; i < n; ++i) out_host[i] = dev_expf(x_host[i]);
     return RLCA_OK;
 }

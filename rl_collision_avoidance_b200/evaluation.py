@@ -472,7 +472,7 @@ def metrics(tot):
 
 
 def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None,
-             progress=None, noise=None, latency=None, dynamics=None, localization=None):
+             progress=None, noise=None, latency=None, dynamics=None, localization=None, crowd=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
@@ -527,7 +527,18 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     and noise have touched the stack, `localization.observe` with env.flags turns env.gs into the gs the policy reads
     next.  env.gs and the state stay the truth, so success, crashes and every tracker measure the true poses.  The
     result then also holds 'localization' (the settings).  Policies only, not hybrid: the ORCA baselines and the hybrid
-    driver read the true state through their own kernels; non-cooperative robots keep the truth."""
+    driver read the true state through their own kernels; non-cooperative robots keep the truth.
+
+    With `crowd` (a crowd.Crowd on `env`, DESIGN.md §9t) its agents follow the social force instead, applied where the
+    non-cooperative override is, and the result holds the same role splits with the keys 'cooperative' and 'crowd'
+    (mode counts over the cooperative robots likewise).  Crowd agents read the true state.  ValueError together with
+    `non_cooperative`: the split has two roles."""
+    if crowd is not None:
+        if non_cooperative is not None:
+            raise ValueError('crowd and non_cooperative cannot be combined: the metrics split into two roles')
+        if crowd.env is not env:
+            raise ValueError('the crowd belongs to another env')
+    masked, role = (crowd, 'crowd') if crowd is not None else (non_cooperative, 'non_cooperative')
     if dynamics is not None and dynamics.env is not env:
         raise ValueError('the dynamics belongs to another env')
     if localization is not None:
@@ -585,8 +596,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
                                                     action_bound=ACTION_BOUND)
             if hybrid is not None:
                 hybrid.apply(scaled, stacks[k], tracker)
-        if non_cooperative is not None:
-            non_cooperative.apply(scaled)
+        if masked is not None:
+            masked.apply(scaled)
         if circle:
             scaled = torch.stack((torch.where(terminal, 0.0, scaled[:, 0]), scaled[:, 1]), 1)
         if latency is not None:
@@ -615,32 +626,32 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     part = tracker.partials()
     tot = totals(part)
     out = {'partials': part, 'totals': tot, 'metrics': metrics(tot), 'ticks': ticks, 'tracker': tracker}
-    if non_cooperative is not None:
-        split = tracker.partials_split(non_cooperative.mask)
+    if masked is not None:
+        split = tracker.partials_split(masked.mask)
         out['partials_split'] = split
         out['by_role'] = {'cooperative': metrics(totals(split[:, 0])),
-                          'non_cooperative': metrics(totals(split[:, 1]))}
+                          role: metrics(totals(split[:, 1]))}
     if hybrid is not None:
-        out['mode_counts'] = hybrid.counts_per_world(None if non_cooperative is None else non_cooperative.mask)
+        out['mode_counts'] = hybrid.counts_per_world(None if masked is None else masked.mask)
         out['modes'] = mode_shares(out['mode_counts'])
     if safe is not None:
         sp = safe.partials()
         out.update(safety_partials=sp, safety_totals=safety_totals(sp), safety_tracker=safe)
         out['safety'] = safety_metrics(out['safety_totals'])
-        if non_cooperative is not None:
-            ss = safe.partials(role_mask=non_cooperative.mask)
+        if masked is not None:
+            ss = safe.partials(role_mask=masked.mask)
             out['safety_partials_split'] = ss
             out['safety_by_role'] = {'cooperative': safety_metrics(safety_totals(ss[:, 0])),
-                                     'non_cooperative': safety_metrics(safety_totals(ss[:, 1]))}
+                                     role: safety_metrics(safety_totals(ss[:, 1]))}
     if prog is not None:
         pp = prog.partials()
         out.update(progress_partials=pp, progress_totals=progress_totals(pp), progress_tracker=prog)
         out['progress'] = progress_metrics(out['progress_totals'])
-        if non_cooperative is not None:
-            ps = prog.partials(role_mask=non_cooperative.mask)
+        if masked is not None:
+            ps = prog.partials(role_mask=masked.mask)
             out['progress_partials_split'] = ps
             out['progress_by_role'] = {'cooperative': progress_metrics(progress_totals(ps[:, 0])),
-                                       'non_cooperative': progress_metrics(progress_totals(ps[:, 1]))}
+                                       role: progress_metrics(progress_totals(ps[:, 1]))}
     if noise is not None:
         out['noise'] = noise.settings()
     if latency is not None:

@@ -242,11 +242,12 @@ def _ppo_update(policy: CNNPolicy, optimizer, batch_size, memory, epoch, coeff_e
 
 def ppo_update_stage1(policy, optimizer, batch_size, memory, epoch, coeff_entropy=0.02, clip_value=0.2, num_step=2048,
                       num_env=12, frames=1, obs_size=24, act_size=4, generator=None, process_group=None,
-                      permutations=None, diagnostics=None, target_kl=None):
-    """model/ppo.py:143-194 (drop_last=False)."""
+                      permutations=None, diagnostics=None, target_kl=None, filter_index=None):
+    """model/ppo.py:143-194 (drop_last=False).  `filter_index` (flat rows t * num_env + i) leaves rows out of the
+    update, as stage 2's does; None is the reference's update over every row."""
     rows = _ppo_update(policy, optimizer, batch_size, memory, epoch, coeff_entropy, clip_value, num_step, num_env,
-                       frames, obs_size, act_size, None, False, generator, process_group, permutations=permutations,
-                       diagnostics=diagnostics, target_kl=target_kl)
+                       frames, obs_size, act_size, filter_index, False, generator, process_group,
+                       permutations=permutations, diagnostics=diagnostics, target_kl=target_kl)
     print('update')
     return rows
 

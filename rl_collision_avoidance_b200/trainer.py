@@ -17,10 +17,13 @@ import torch
 from .mix import MIX_AUTO_RESET, MIX_SCENARIOS, SLICE_ALIGN, check_aligned
 from .model.ppo import generate_action, generate_train_data, ppo_update_stage1, ppo_update_stage2
 from .model.utils import get_filter_index
+from .crowd import Crowd
 from .dynamics import Dynamics
+from .evaluation import non_cooperative_mask
 from .latency import Latency
 from .localization import Localization
 from .noise import Noise
+from .orca import NonCooperative
 from .stage_world import RESULT_STRINGS
 
 
@@ -57,6 +60,7 @@ class _Component:
         self.latency = latency                          # latency.Latency of the env, or None
         self.dynamics = dynamics                        # dynamics.Dynamics of the env, or None
         self.localization = localization                # localization.Localization of the env, or None
+        self.masked = None                              # orca.NonCooperative or crowd.Crowd of the env, or None
         self.ticked = False                             # a tick has run, so self.flags holds its flags
         self.name = env.sc.name
         self.relayout = env.sc.layout is not None
@@ -98,8 +102,11 @@ class _Component:
         the run's first tick), and the stack is delayed after the re-layout and before any noise.  With dynamics the
         command, last of all, is limited in acceleration, with the same flags of the tick before.  With localization
         the gs the tick and the re-layout wrote becomes, in place and last of all, the gs the robot believes, with the
-        flags of this tick."""
+        flags of this tick.  With masked agents their rows of ro.scaled are overwritten first, before any latency; PPO
+        keeps the policy's sampled action in ro.actions."""
         e = self.env
+        if self.masked is not None:
+            self.masked.apply(self.scaled)
         cmd = self.scaled
         prev = self.flags[t - 1] if t > 0 else self.flags[-1] if self.ticked else None
         if self.latency is not None:
@@ -144,6 +151,37 @@ def compose(envs, ro, noise=None, latency=None, dynamics=None, localization=None
     return comps
 
 
+def masked_agents(comps, non_cooperative=None, crowd=None):
+    """Give every component its masked agents and return the (N,) bool mask of the rollout's masked columns, or None
+    when there are none.  non_cooperative = (k, speed or None): an orca.NonCooperative; crowd = (k, crowd.CrowdParams,
+    map flag): a crowd.Crowd (DESIGN.md §9t); in both, robots floor(j R_c / k), j < k, of every world of component c
+    (evaluation.non_cooperative_mask: ValueError unless 1 <= k <= R_c).  ValueError for both."""
+    if non_cooperative is not None and crowd is not None:
+        raise ValueError('crowd and non_cooperative cannot be combined: the stats split into two roles')
+    if non_cooperative is None and crowd is None:
+        return None
+    k = non_cooperative[0] if non_cooperative is not None else crowd[0]
+    masks = [non_cooperative_mask(c.env.cfg.robots_per_world, c.env.cfg.num_worlds, k) for c in comps]
+    for c, m in zip(comps, masks):
+        if non_cooperative is not None:
+            c.masked = NonCooperative(c.env, m, speed=non_cooperative[1])
+        else:
+            c.masked = Crowd(c.env, m, crowd[1], obstacles=crowd[2])
+    return np.concatenate(masks) != 0
+
+
+def masked_rows(H, col_mask):
+    """Every row t * N + i of a masked column i, sorted: stage 1's filter."""
+    N = col_mask.shape[0]
+    return (np.arange(H)[:, None] * N + np.flatnonzero(col_mask)[None, :]).reshape(-1).tolist()
+
+
+def masked_filter_index(dones, col_mask):
+    """Stage 2's filter with masked columns: get_filter_index(dones) over every column (the reference's quirk
+    unchanged) united with masked_rows, sorted."""
+    return np.union1d(np.asarray(get_filter_index(dones), np.int64), masked_rows(dones.shape[0], col_mask)).tolist()
+
+
 def _check_mix(envs, stage):
     """ValueError unless `envs` can share one stage-2 rollout (DESIGN.md §9l)."""
     if stage != 2:
@@ -168,7 +206,7 @@ def _check_mix(envs, stage):
 
 def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logger_cal=None, stage=1, max_updates=None,
         process_group=None, rank=0, save_every=20, generator=None, start_update=0, diagnostics=False, target_kl=None,
-        noise=None, latency=None, dynamics=None, localization=None):
+        noise=None, latency=None, dynamics=None, localization=None, non_cooperative=None, crowd=None):
     """hp: dict with HORIZON, GAMMA, LAMDA, BATCH_SIZE, EPOCH, COEFF_ENTROPY, CLIP_VALUE, NUM_ENV, OBS_SIZE, ACT_SIZE,
     LASER_HIST, MAX_EPISODES.  `start_update` continues the checkpoint numbering of a resumed run.
     A random scenario (env.sc.layout, DESIGN.md §9k) trains with stage 2's update on per-world layouts: the env runs
@@ -195,6 +233,10 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     a localization.Localization with stream id k, and every gs the policy reads (ro.gs, slot 0 and every slot a tick
     wrote, after any re-layout) is the believed one, so PPO stores and re-evaluates what the policy read.  Rewards and
     episode ends stay on the true state.  None launches nothing.
+    `non_cooperative` ((k, speed or None), DESIGN.md §9h) or `crowd` ((k, crowd.CrowdParams, map flag), §9t) puts k
+    masked agents into every world of every component (masked_agents); their rows of the action are overwritten before
+    any latency, and every row of their columns is left out of every PPO update (stage 1: filter_index; stage 2:
+    united with get_filter_index).  The stats then also hold 'by_role' {'cooperative', 'non_cooperative' or 'crowd'}.
     Returns per-update stats (for tests / benchmarks); 'by_scenario' splits the episodes by component."""
     envs = list(env) if isinstance(env, (list, tuple)) else [env]
     if not envs:
@@ -217,6 +259,8 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
         comps = compose(envs, ro, noise, latency, dynamics)
     else:
         comps = compose(envs, ro, noise) if latency is None else compose(envs, ro, noise, latency)
+    col_mask = masked_agents(comps, non_cooperative, crowd)
+    role = 'crowd' if crowd is not None else 'non_cooperative'
     col_comp = np.repeat(np.arange(len(comps)), [e.N for e in envs])     # component of every agent column
     for c in comps:
         c.start()
@@ -255,12 +299,15 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
                       frames=hp['LASER_HIST'], obs_size=hp['OBS_SIZE'], act_size=hp['ACT_SIZE'], generator=generator,
                       process_group=process_group, diagnostics=diag, target_kl=target_kl)
         if stage == 1:
-            rows = ppo_update_stage1(**common)
+            if col_mask is None:
+                rows = ppo_update_stage1(**common)
+            else:
+                rows = ppo_update_stage1(filter_index=masked_rows(H, col_mask), **common)
         else:
             # ppo_stage2.py:112.  The reference's run counter is not reset between columns, so a run of done carries
             # from one robot's column into the next; in a mix it carries across the boundary between two components
             # in the same way (§9l), exactly as for one env of N columns.
-            filter_index = get_filter_index(dones)
+            filter_index = get_filter_index(dones) if col_mask is None else masked_filter_index(dones, col_mask)
             rows = ppo_update_stage2(filter_index=filter_index, **common)
         torch.cuda.synchronize(dev)
         t2 = time.perf_counter()
@@ -304,6 +351,9 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
                       'success_rate': float((ep[:, 6] == 1).mean()) if len(ep) else float('nan'),
                       'losses': rows[-1] if rows else None,
                       'by_scenario': {c.name: _episode_stats(ep[ep_comp == k]) for k, c in enumerate(comps)}})
+        if col_mask is not None:
+            ep_masked = col_mask[idx[:, 1]]
+            stats[-1]['by_role'] = {'cooperative': _episode_stats(ep[~ep_masked]), role: _episode_stats(ep[ep_masked])}
         if diag is not None:
             stats[-1]['diagnostics'] = diag.metrics()
             if rank == 0:
