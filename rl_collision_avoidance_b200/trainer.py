@@ -251,14 +251,7 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     H, N = hp['HORIZON'], sum(e.N for e in envs)
     dev = envs[0].device
     ro = Rollout(H, N, envs[0].beam_mum, dev)
-    # without latency, dynamics or localization, compose is called as it always was, so wrappers of its older
-    # signature keep working
-    if localization is not None:
-        comps = compose(envs, ro, noise, latency, dynamics, localization)
-    elif dynamics is not None:
-        comps = compose(envs, ro, noise, latency, dynamics)
-    else:
-        comps = compose(envs, ro, noise) if latency is None else compose(envs, ro, noise, latency)
+    comps = compose(envs, ro, noise, latency, dynamics, localization)
     col_mask = masked_agents(comps, non_cooperative, crowd)
     role = 'crowd' if crowd is not None else 'non_cooperative'
     col_comp = np.repeat(np.arange(len(comps)), [e.N for e in envs])     # component of every agent column

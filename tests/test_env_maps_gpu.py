@@ -20,6 +20,7 @@ from rl_collision_avoidance_b200.scenarios import fill_config, make_scenario
 from test_env_maps import CASE_IDS, MAP_CASES, RANGE_MAX, build_map, oreach, padded
 
 pytestmark = pytest.mark.gpu
+PROFILED_TICKS = 3
 
 
 def _scenario(case, m):
@@ -137,18 +138,25 @@ def test_map_case_against_oracle(built, case):
     assert_outputs_equal(env, orc, f'{case.name} first observation')
     rng = np.random.default_rng(case.grid_w)
 
-    # the path: kernels of one tick by name; the footprint window from oreach
+    # the path: kernels of one tick by name; the footprint window from oreach.  The profiler's activity records
+    # occasionally lose one kernel of a tick whose launch call it did record, so a tick missing a wanted kernel is
+    # profiled again (up to PROFILED_TICKS ticks, each checked against the oracle); a kernel that is not launched is
+    # missing from every one of them, and no profiled tick may launch an absent kernel.
     a = random_actions(rng, N, wide=True)
-    got, raw = _kernel_names(env, torch.from_numpy(a).cuda())
-    orc.step(a)
     want, absent = _expected_kernels(case)
-    for k in want:
-        assert any(k in g for g in got), f'{case.name}: {k} not launched; kernels: {sorted(raw)}'
-    for k in absent:
-        assert not any(k in g for g in got), f'{case.name}: {k} launched; kernels: {sorted(raw)}'
+    missing = list(want)
+    for p in range(PROFILED_TICKS):
+        got, raw = _kernel_names(env, torch.from_numpy(a).cuda())
+        orc.step(a)
+        for k in absent:
+            assert not any(k in g for g in got), f'{case.name}: {k} launched; kernels: {sorted(raw)}'
+        assert_state_equal(env, orc, f'{case.name} profiled tick {p}')
+        assert_outputs_equal(env, orc, f'{case.name} profiled tick {p}')
+        missing = [k for k in missing if not any(k in g for g in got)]
+        if not missing:
+            break
+    assert not missing, f'{case.name}: {missing} not launched in {PROFILED_TICKS} ticks; kernels: {sorted(raw)}'
     assert (32 if oreach(case.res) <= 15 else 64) == case.win
-    assert_state_equal(env, orc, f'{case.name} profiled tick')
-    assert_outputs_equal(env, orc, f'{case.name} profiled tick')
 
     # ticks of wide random actions
     cov = _Coverage(case, sc, N)

@@ -3,7 +3,13 @@ trainer imports and of the optimizer instance, then every update replayed agains
 
 a. The environment, bit for bit: one CPU oracle per component, driven by the executed commands, with the scan deque of
    tests/trainer_ref.py, the re-layout host twin (random layouts) and the noise host twins.  Stacks, goal | speed,
-   rewards, flags and the eplog rows of ended episodes equal the device rollout's.
+   rewards, flags and the eplog rows of ended episodes equal the device rollout's.  The perturbation chain is restated
+   per component and tick: the executed command is the sampled one with the masked rows overridden (the crowd and
+   straight-driver host twins on the oracle's state, themselves within their float64 restatements' bounds), then
+   latency_ref's command ring, the noise twin and dynamics_ref's limits, the last two links with the flags of the tick
+   before; it equals what the env's control_vel received, bit for bit.  The stack is the deque after the re-layout
+   refresh, then latency_ref's scan ring and the noise twin; the gs the policy reads is localization_ref's believed gs
+   on the oracle's pose and goal after the re-layout.
 b. The policy per tick, at the weights of the update's start: values against the float64 forward within
    learner_ref.check_forward's bound for the tensor-core mode, means within the bound at _forward64; actions,
    log-probabilities and the clip against sample_ref (test_sample_gpu's bounds); the stored action is the sampled,
@@ -11,12 +17,14 @@ b. The policy per tick, at the weights of the update's start: values against the
 c. The update: GAE targets and advantages against the float64 recurrence on the replayed rewards and dones (1 float32
    ulp, test_learner_shapes_gpu.test_gae_vs_float64_recurrence); filter_index exactly; the epochs' permutations drawn
    again from the generator state at entry give the restated minibatch schedule (a ragged last minibatch in stage 1,
-   the tail dropped in stage 2); then per optimizer step, teacher-forced from the device's parameters at that step, on
+   the tail dropped in stage 2) over the rows the restated filter keeps (stage 2: get_filter_index united with every
+   row of a masked column; stage 1: those rows alone); then per optimizer step, teacher-forced from the device's parameters at that step, on
    the rows of the replayed minibatch with the restated advantage normalisation (before np.delete): the ppo.log row
    against learner_ref.ref_losses, all 23 gradients against float64 autograd relative to their layer's scale, and the
    Adam step against trainer_ref.adam_step in float64 from the device's gradient (bounds at step_checks and
    adam_bounds).  Every replayed PPO ratio is asserted to be learner_ref.MARGIN away from 1 +- clip.
-d. The Env log lines against the replay's own episode bookkeeping.
+d. The Env log lines against the replay's own episode bookkeeping, and the stats run returns (episodes, success rate,
+   mean episode reward, by_scenario and, with masked agents, by_role) against the replay's eplog rows of ended episodes.
 
 Real rollouts are not decisive batches (learner_ref): a pre-activation within fp32 rounding of zero can flip its ReLU
 mask between the kernels and float64, which moves that tower's gradients by ~1e-3 of their scale.  A tower's tensors are
@@ -25,6 +33,7 @@ of its conv pre-activations is within learner_ref.MARGIN of its layer's max of z
 mask moves its row's whole contribution, so that side's tensors may also differ by twice the float64 gradient of the
 rows holding one.  Elsewhere the tight bounds hold.
 """
+import collections
 import dataclasses
 import logging
 import math
@@ -35,9 +44,15 @@ import numpy as np
 import pytest
 import torch
 
+import crowd_ref
+import dynamics_ref
+import latency_ref
+import localization_ref
+import orca_ref
 import sample_ref
 import trainer_ref as ref
 from learner_ref import (CLIP, COEFF, MARGIN, VCOEF, Checks, layer_scale, maxabs, ref_forward, ref_logprob, ref_losses)
+from test_crowd import TOL as CROWD_TOL
 from test_sample_gpu import action_bound, lp_bound
 
 pytestmark = pytest.mark.gpu
@@ -49,7 +64,18 @@ LR = 5e-5
 B1, B2 = float(np.float32(0.9)), float(np.float32(0.999))      # the betas as the fused Adam kernel receives them
 TINY = 2.0 ** -148        # two float32 subnormal steps: the absolute floor of a rounding near zero
 
-# (scenario, worlds, auto_reset, timeout, extra make_scenario arguments) per component
+LATENCY = dict(scan_delay=(0, 4), command_delay=(1, 3), seed=2 ** 34 + 7)
+DYNAMICS = dict(linear=(0.5, 2.0), angular=(1.0, 4.0), seed=2 ** 35 + 9)
+LOCALIZATION = dict(pose_sigma=(0.05, 0.2), heading_sigma=(0.02, 0.1), correlation_time=2.0, speed_sigma=(0.05, 0.1),
+                    seed=2 ** 36 + 11)
+CHAIN_SEED = 1            # the chain's localization seed: with LOCALIZATION's, a PPO ratio falls within MARGIN of 1 + clip
+NONCOOP_TOL = 1e-5       # the straight driver's twin against orca_ref's preferred velocity and tracker (test_noncoop)
+MIX = [('stage2', 1, 2, 25, {}), ('circle', 2, 2, 100, dict(robots_per_world=8, radius=1.5)),
+       ('random', 4, 0, 60, dict(robots_per_world=8, side=6.0))]
+
+# (scenario, worlds, auto_reset, timeout, extra make_scenario arguments) per component; the perturbations are the
+# keyword arguments of latency.LatencyParams, dynamics.DynamicsParams and localization.LocalizationParams, 'crowd' the
+# k of crowd=(k, CrowdParams(), True) and 'non_cooperative' the (k, speed) of trainer.run
 CASES = {
     # 2 x 24 robots; episodes time out after 20 ticks, so the first ones end on tick 19 and 39 = the horizon's last;
     # H N = 1920 is 7.5 minibatches of 256: a ragged last minibatch
@@ -61,10 +87,23 @@ CASES = {
                    ckpt='stage2.pth', noise=True),
     # stage 2 | circle | random in mix.MIX_SCENARIOS order; the stage-2 groups end together on tick 51 = H - 1, and
     # circle and random robots that finished early idle on update 2's first tick: filter runs cross the boundaries
-    'mix': dict(stage=2, comps=[('stage2', 1, 2, 25, {}), ('circle', 2, 2, 100, dict(robots_per_world=8, radius=1.5)),
-                                ('random', 4, 0, 60, dict(robots_per_world=8, side=6.0))],
-                H=52, batch=256, ckpt='stage2.pth', noise=False),
+    'mix': dict(stage=2, comps=MIX, H=52, batch=256, ckpt='stage2.pth', noise=False),
     'noise': dict(stage=1, comps=[('stage1', 2, 1, 19, {})], H=40, batch=256, ckpt='stage1_2.pth', noise=True),
+    # stage 1's shape: the episodes ending on tick 39 = H - 1 restart their command rings on update 2's tick 0
+    'latency': dict(stage=1, comps=[('stage1', 2, 1, 19, {})], H=40, batch=256, ckpt='stage1_2.pth', noise=False,
+                    latency=LATENCY),
+    # stage 2's shape: crashed robots' limits restart from 0, groups re-spawn, early finishers idle
+    'dynamics': dict(stage=2, comps=[('stage2', 1, 2, 25, {})], H=52, batch=256, ckpt='stage2.pth', noise=False,
+                     dynamics=DYNAMICS),
+    # random layouts: a re-laid robot's believed gs is drawn from its new layout with fresh sigmas
+    'localization': dict(stage=2, comps=[('random', 8, 0, 25, dict(robots_per_world=8, side=6.0))], H=52, batch=128,
+                         ckpt='stage2.pth', noise=False, localization=LOCALIZATION),
+    # stage 1 with 2 straight drivers per world: H (N - 4) = 1760 kept rows are 6.9 minibatches of 256
+    'masked_stage1': dict(stage=1, comps=[('stage1', 2, 1, 19, {})], H=40, batch=256, ckpt='stage1_2.pth', noise=False,
+                          non_cooperative=(2, 0.8)),
+    # the mix with every link of the chain on and a crowd that sees the map
+    'chain': dict(stage=2, comps=MIX, H=52, batch=256, ckpt='stage2.pth', noise=True, latency=LATENCY,
+                  dynamics=DYNAMICS, localization=dict(LOCALIZATION, seed=CHAIN_SEED), crowd=2),
 }
 SEED = 3
 
@@ -90,21 +129,41 @@ def _np(t):
 
 # ------------------------------------------------------------------------------------------------ recording
 class Recorder:
-    def __init__(self, monkeypatch, policy, optimizer, generator):
+    def __init__(self, monkeypatch, policy, optimizer, generator, envs):
         from rl_collision_avoidance_b200 import noise as noise_mod
         from rl_collision_avoidance_b200 import trainer
+        from rl_collision_avoidance_b200.crowd import Crowd
+        from rl_collision_avoidance_b200.orca import NonCooperative
         self.policy, self.opt, self.gen = policy, optimizer, generator
         self.ticks, self.fv, self.noise_cmds, self.gtd, self.updates = [], [], [], [], []
-        self.ro = self.comps = None
+        self.executed = [[] for _ in envs]          # per component and tick: the command control_vel received
+        self.overrides = [[] for _ in envs]         # per component and tick: the action after the masked override
+        self.ro = self.comps = self.stats = None
         rec = self
 
         compose0 = trainer.compose
 
-        def compose(envs, ro, noise=None):
+        def compose(envs, ro, noise=None, latency=None, dynamics=None, localization=None):
             rec.ro = ro
-            rec.comps = compose0(envs, ro, noise)
+            rec.comps = compose0(envs, ro, noise, latency, dynamics, localization)
             return rec.comps
         monkeypatch.setattr(trainer, 'compose', compose)
+
+        def index(env):
+            return next(k for k, e in enumerate(envs) if e is env)
+
+        for k, e in enumerate(envs):
+            def control_vel(action, *args, _cv0=e.control_vel, _k=k, **kw):
+                rec.executed[_k].append(action.detach().clone())
+                return _cv0(action, *args, **kw)
+            monkeypatch.setattr(e, 'control_vel', control_vel)
+
+        for cls in (Crowd, NonCooperative):
+            def apply(self_, action, _apply0=cls.apply):
+                out = _apply0(self_, action)
+                rec.overrides[index(self_.env)].append(out.clone())
+                return out
+            monkeypatch.setattr(cls, 'apply', apply)
 
         fv0 = policy.forward_values
 
@@ -171,9 +230,28 @@ class Recorder:
         monkeypatch.setattr(optimizer, 'step', step)
 
 
+def _perturbations(c):
+    """The perturbation settings of case c: noise, latency, dynamics and localization params (or None) and the
+    masked agents ('crowd', k, CrowdParams) / ('non_cooperative', k, speed) (or None)."""
+    from rl_collision_avoidance_b200.crowd import CrowdParams
+    from rl_collision_avoidance_b200.dynamics import DynamicsParams
+    from rl_collision_avoidance_b200.latency import LatencyParams
+    from rl_collision_avoidance_b200.localization import LocalizationParams
+    from rl_collision_avoidance_b200.noise import NoiseParams
+    masked = None
+    if 'crowd' in c:
+        masked = ('crowd', c['crowd'], CrowdParams())
+    elif 'non_cooperative' in c:
+        masked = ('non_cooperative',) + tuple(c['non_cooperative'])
+    return dict(noise=NoiseParams(**NOISE) if c['noise'] else None,
+                latency=LatencyParams(**c['latency']) if 'latency' in c else None,
+                dynamics=DynamicsParams(**c['dynamics']) if 'dynamics' in c else None,
+                localization=LocalizationParams(**c['localization']) if 'localization' in c else None,
+                masked=masked)
+
+
 def _train(case, monkeypatch):
     from rl_collision_avoidance_b200.model.net import Adam, CNNPolicy
-    from rl_collision_avoidance_b200.noise import NoiseParams
     from rl_collision_avoidance_b200.stage_world import StageWorld
     from rl_collision_avoidance_b200.trainer import run
     c = CASES[case]
@@ -189,8 +267,9 @@ def _train(case, monkeypatch):
     gen = torch.Generator(device='cuda').manual_seed(SEED)
     hp = dict(HORIZON=c['H'], GAMMA=0.99, LAMDA=0.95, BATCH_SIZE=c['batch'], EPOCH=2, COEFF_ENTROPY=COEFF,
               CLIP_VALUE=CLIP, NUM_ENV=N, OBS_SIZE=512, ACT_SIZE=2, LASER_HIST=3, MAX_EPISODES=5000)
-    noise = NoiseParams(**NOISE) if c['noise'] else None
-    rec = Recorder(monkeypatch, policy, opt, gen)
+    pt = _perturbations(c)
+    masked = pt['masked']
+    rec = Recorder(monkeypatch, policy, opt, gen, envs)
     lg, lc = logging.getLogger(f'replay_{case}'), logging.getLogger(f'replay_cal_{case}')
     hl, hc = _Lines(), _Lines()
     for l, h in ((lg, hl), (lc, hc)):
@@ -198,26 +277,30 @@ def _train(case, monkeypatch):
         l.propagate = False
         l.addHandler(h)
     try:
-        run(env=envs if len(envs) > 1 else envs[0], policy=policy, policy_path=None, action_bound=[[0, -1], [1, 1]],
-            optimizer=opt, hp=hp, logger=lg, logger_cal=lc, stage=c['stage'], max_updates=2, generator=gen,
-            noise=noise)
+        rec.stats = run(env=envs if len(envs) > 1 else envs[0], policy=policy, policy_path=None,
+                        action_bound=[[0, -1], [1, 1]], optimizer=opt, hp=hp, logger=lg, logger_cal=lc,
+                        stage=c['stage'], max_updates=2, generator=gen, noise=pt['noise'], latency=pt['latency'],
+                        dynamics=pt['dynamics'], localization=pt['localization'],
+                        non_cooperative=masked[1:] if masked and masked[0] == 'non_cooperative' else None,
+                        crowd=(masked[1], masked[2], True) if masked and masked[0] == 'crowd' else None)
     finally:
         lg.removeHandler(hl)
         lc.removeHandler(hc)
     torch.cuda.synchronize()
-    return rec, envs, scs, noise, hl.records, hc.records
+    return rec, envs, scs, pt, hl.records, hc.records
 
 
 # ------------------------------------------------------------------------------------------------ a. environment
 class OracleComponent:
     """The CPU oracle of one component, the restated scan deque and the episode bookkeeping of its robots."""
 
-    def __init__(self, k, comp, sc, W, ar, noise):
+    def __init__(self, k, comp, sc, W, ar, pt):
         from oracle.oracle import OracleWorld, OrcConfig
         from rl_collision_avoidance_b200.noise import scan_host
+        from rl_collision_avoidance_b200.orca import ObstacleSet
         from rl_collision_avoidance_b200.scenarios import fill_config, random_layout_host
-        self.k, self.c, self.sc, self.noise = k, comp, sc, noise
-        self.cfg = comp.env.cfg                      # the product's config struct, for the host twins
+        self.k, self.c, self.sc, self.noise = k, comp, sc, pt['noise']
+        self.cfg = cfg = comp.env.cfg                # the product's config struct, for the host twins
         ocfg = fill_config(OrcConfig(), sc, num_worlds=W, beams=512, auto_reset=ar, seed=SEED)
         o = self.o = OracleWorld(ocfg, sc.map.cells, sc.init_tab, sc.goal_tab)
         self.relayout = sc.layout is not None
@@ -230,13 +313,39 @@ class OracleComponent:
             assert not status.any()
             o.observe()
         n = o.N
+        R, off = int(cfg.robots_per_world), int(cfg.world_offset)
+        # the chain's restatements, stream k as compose gives component k
+        lp, dp, zp = pt['latency'], pt['dynamics'], pt['localization']
+        self.lat = None if lp is None else latency_ref.Latency(R, W, lp.scan_delay, lp.command_delay, lp.seed, off, k)
+        self.dyn = None if dp is None else dynamics_ref.Dynamics(R, W, dp.linear, dp.angular, dp.seed,
+                                                                 (cfg.v_min, cfg.v_max, cfg.w_min, cfg.w_max), cfg.dt,
+                                                                 off, k)
+        self.loc = None if zp is None else localization_ref.Localization(
+            R, W, zp.pose_sigma, zp.heading_sigma, zp.correlation_time, zp.speed_sigma, zp.seed, cfg.dt, off, k)
+        self.masked = pt['masked']
+        self.mask = np.zeros(n, np.uint8)            # robots floor(j R / k), j < k, of every world (§9h, §9t)
+        self.obstacles = self.segments = None
+        if self.masked is not None:
+            kk = self.masked[1]
+            for w in range(W):
+                self.mask[w * R + np.arange(kk) * R // kk] = 1
+            if self.masked[0] == 'crowd':
+                self.obstacles = ObstacleSet(cfg, sc.map.cells, self.masked[2].wall_dist)
+                self.segments = self.obstacles.segments()[0]
+        self.prev = None                             # the flags of the tick before, None before the run's first
         self.live = np.ones(n, np.uint8)
         self.stacks = ref.Stacks(o.obs)
-        self.scan_draws = 0
-        if noise is not None:
-            self.stacks.load(scan_host(self.cfg, noise, 0, self.stacks.array(), None, stream_id=k))
+        arr = self.stacks.array()
+        if self.lat is not None:
+            self.lat.scan(arr)                       # every row starts an episode: its stack is left as it is
+        if self.noise is not None:
+            arr = scan_host(self.cfg, self.noise, 0, arr, None, stream_id=k)
+        self.stacks.load(arr)
         self.scan_draws = 1
         self.gs = o.gs.copy()
+        if self.loc is not None:
+            self.gs = self.loc.observe(o.pose, o.goal, self.gs, None)
+        self.believed = (self.gs != o.gs).any(1)     # rows whose gs is not the true one
         # episode bookkeeping (ppo_stage1.py:51-57, 127-131; ppo_stage2.py:49-56, 136-137)
         self.episode = np.zeros(n, np.int64)
         self.steps = np.zeros(n, np.int64)
@@ -250,7 +359,75 @@ class OracleComponent:
     def state(self):
         return self.stacks.array(), self.gs.copy()
 
-    def tick(self, cmd, g):
+    def command(self, scaled, g, rec, ev):
+        """The command executed on global tick g for the sampled `scaled` rows: masked override -> latency -> noise ->
+        limits, the last two links with the flags of the tick before; each recorded link is held to it bit for bit and
+        the result to what control_vel received."""
+        from rl_collision_avoidance_b200.noise import action_host
+        o, what = self.o, f'tick {g} {self.c.name}'
+        cmd = scaled
+        if self.masked is not None:
+            if self.masked[0] == 'crowd':
+                from rl_collision_avoidance_b200.crowd import crowd_host
+                want = crowd_host(self.cfg, o.pose, o.goal, o.meta, self.mask, cmd, self.masked[2],
+                                  obstacles=self.obstacles)
+            else:
+                from rl_collision_avoidance_b200.orca import noncoop_host
+                want = noncoop_host(self.cfg, o.pose, o.goal, o.meta, self.mask, cmd, speed=self.masked[2])
+            assert _bits_equal(_np(rec.overrides[self.k][g]), want), f'{what}: masked override'
+            self._check_masked(want, ev)
+            ev['masked_changed'] += int((want != cmd).any(1).sum())
+            cmd = want
+        if self.lat is not None:
+            out = self.lat.action(cmd, self.prev)
+            ev['command_delayed'] += int((out != cmd).any(1).sum())
+            cmd = out
+        if self.noise is not None and self.noise.action_on:
+            sid, draw, inp, out = [x for x in rec.noise_cmds if x[0] == self.k][g]
+            assert draw == g and _bits_equal(_np(inp), cmd), f'{what}: the noised command\'s input'
+            want = action_host(self.cfg, self.noise, g, cmd, stream_id=self.k)
+            assert _bits_equal(_np(out), want), f'{what}: noised command'
+            ev['noised_rows'] += int((want != cmd).any(1).sum())
+            cmd = want
+        if self.dyn is not None:
+            vel = self.dyn.vel.copy()
+            out = self.dyn.action(cmd, self.prev)
+            v0, v1, w0, w1 = self.dyn.bounds
+            target = np.stack([dynamics_ref.target(cmd[:, 0], v0, v1), dynamics_ref.target(cmd[:, 1], w0, w1)], 1)
+            ev['limited'] += int((out != cmd).any(1).sum())
+            ev['clamped'] += int((out != target).sum())
+            if self.prev is not None:
+                crashed = (self.prev[:, 1] != 0) & (self.prev[:, 3] == 0)
+                ev['crash_prev_reset'] += int((crashed & vel.any(1)).sum())
+            cmd = out
+        assert _bits_equal(_np(rec.executed[self.k][g]), cmd), f'{what}: the command control_vel received'
+        return cmd
+
+    def _check_masked(self, act, ev):
+        """the twin's masked rows against the float64 restatements: crowd_ref within test_crowd's bound (agents with a
+        distance within 1e-4 of a cut-off left out, as there), the straight driver within test_noncoop's"""
+        from rl_collision_avoidance_b200.orca import DEFAULTS
+        o, cfg = self.o, self.cfg
+        R = int(cfg.robots_per_world)
+        for a in np.flatnonzero(self.mask):
+            if self.masked[0] == 'crowd':
+                p = self.masked[2]
+                segs = _segments_near(self.segments, o.pose[a, 0:2].astype(np.float64), p.wall_dist + 0.01)
+                d = crowd_ref.distances(cfg, o.pose, a, segs)
+                near = np.concatenate((d[:R - 1] - p.neighbour_dist, d[R - 1:] - p.wall_dist))
+                if ((np.abs(near) < 1e-4) & (near != 0)).any():
+                    continue
+                want, tol = crowd_ref.crowd_action(cfg, o.pose, o.goal, o.meta, self.mask, a, p, segs), CROWD_TOL
+            else:
+                pos, th, _ = orca_ref.agent_state(o.pose, o.goal, o.meta)
+                speed = float(self.masked[2])
+                v = orca_ref.preferred(pos[a], o.goal[a, 0:2], speed, float(cfg.dt))
+                want, tol = orca_ref.track(th[a], v, speed, cfg.w_min, cfg.w_max, DEFAULTS['heading_gain']), \
+                    NONCOOP_TOL
+            assert np.abs(act[a] - want).max() <= tol, (self.c.name, a, act[a], want)
+            ev['masked_checked'] += 1
+
+    def tick(self, cmd, g, ev):
         """one tick at global tick g: reward, flags, eplog, the rows that were idle on it and those that ended"""
         from rl_collision_avoidance_b200.noise import scan_host
         from rl_collision_avoidance_b200.scenarios import relayout_host
@@ -273,11 +450,29 @@ class OracleComponent:
             self.stacks.load(arr)
             gs[relaid] = o.gs[relaid]
             restart = relaid
+        arr = self.stacks.array()
+        if self.lat is not None:
+            newest = arr[:, 2].copy()
+            self.lat.scan(arr, flags)
+            ev['scan_delayed'] += int((arr[:, 2] != newest).any(1).sum())
         if self.noise is not None:
-            self.stacks.load(scan_host(self.cfg, self.noise, self.scan_draws, self.stacks.array(), flags,
-                                       stream_id=self.k))
+            newest = arr[:, 2].copy()
+            arr = scan_host(self.cfg, self.noise, self.scan_draws, arr, flags, stream_id=self.k)
+            ev['noised_scans'] += int((arr[:, 2] != newest).any(1).sum())
+        self.stacks.load(arr)
         self.scan_draws += 1
+        if self.loc is not None:
+            # on the oracle's pose and goal after the re-layout, with this tick's flags
+            sigma = self.loc.sigma.copy()
+            believed = self.loc.observe(o.pose, o.goal, gs, flags)
+            fresh = flags[:, 3] != 0
+            ev['sigma_redrawn' if not self.relayout else 'relaid_sigma_redrawn'] += int(
+                (fresh & (self.loc.sigma != sigma).any(1)).sum())
+            self.believed = (believed != gs).any(1)
+            ev['believed'] += int(self.believed.sum())
+            gs = believed
         self.gs = gs
+        self.prev = flags
         # bookkeeping
         lines = []
         live_now = ~idle
@@ -303,6 +498,39 @@ class OracleComponent:
 def _bits_equal(a, b):
     a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
     return a.shape == b.shape and np.array_equal(a.view(np.uint8), b.view(np.uint8))
+
+
+def _segments_near(segments, p, dist):
+    """The segments (S, 4) within `dist` of the point p: crowd_ref walks every segment in Python, and one farther than
+    wall_dist neither pushes the agent nor lies near its cut-off"""
+    s = np.asarray(segments, np.float64).reshape(-1, 4)
+    a, e = s[:, 0:2], s[:, 2:4] - s[:, 0:2]
+    t = np.clip(((p - a) * e).sum(1) / np.maximum((e * e).sum(1), 1e-300), 0.0, 1.0)
+    return s[np.hypot(*(p - a - t[:, None] * e).T) < dist]
+
+
+def _episode_stats(ep):
+    """episodes, success and crash rates (result 1 and 2) and the mean reward of the eplog rows ep (E, 8) float32,
+    in their order; NaN without episodes"""
+    n = len(ep)
+    return {'episodes': n, 'success_rate': float(np.mean(ep[:, 6] == 1)) if n else math.nan,
+            'crash_rate': float(np.mean(ep[:, 6] == 2)) if n else math.nan,
+            'mean_ep_reward': float(ep[:, 2].mean()) if n else math.nan}
+
+
+def _same(a, b):
+    """a == b, NaN equal to NaN, through dicts"""
+    if isinstance(a, dict) or isinstance(b, dict):
+        return isinstance(a, dict) and isinstance(b, dict) and a.keys() == b.keys() and all(_same(a[k], b[k]) for k in a)
+    return a == b or (isinstance(a, float) and isinstance(b, float) and math.isnan(a) and math.isnan(b))
+
+
+def _masked_rows_across_boundaries(fd, starts, col_mask, H, N):
+    """The masked rows t N + a of a component's first column a (`starts`) that continue a run of filtered rows from
+    the previous component's last column, t N + a - 1, which get_filter_index (`fd`) filtered: a run of the united
+    filter that crosses a component boundary with its masked part on one side."""
+    fd = set(fd)
+    return sum(1 for a in starts if col_mask[a] for t in range(H) if t * N + a - 1 in fd)
 
 
 # ------------------------------------------------------------------------------------------------ float64 pieces
@@ -466,20 +694,28 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
     t_start = time.perf_counter()
     c = CASES[case]
     stage, H = c['stage'], c['H']
-    rec, envs, scs, noise, lines, cal = _train(case, monkeypatch)
+    rec, envs, scs, pt, lines, cal = _train(case, monkeypatch)
     t_train = time.perf_counter() - t_start
+    noise = pt['noise']
     policy = rec.policy
     comps = rec.comps
     N = sum(e.N for e in envs)
-    assert len(rec.updates) == 2 and len(rec.gtd) == 2 and len(rec.ticks) == 2 * H
-    oc = [OracleComponent(k, comp, sc, W, ar, noise) for k, (comp, (sc, W, ar)) in enumerate(zip(comps, scs))]
+    assert len(rec.updates) == 2 and len(rec.gtd) == 2 and len(rec.ticks) == 2 * H and len(rec.stats) == 2
+    assert all(len(x) == 2 * H for x in rec.executed)
+    assert all(len(x) == (2 * H if pt['masked'] else 0) for x in rec.overrides)
+    oc = [OracleComponent(k, comp, sc, W, ar, pt) for k, (comp, (sc, W, ar)) in enumerate(zip(comps, scs))]
+    col_mask = np.concatenate([o.mask for o in oc]) != 0
+    col_comp = np.concatenate([np.full(o.o.N, k) for k, o in enumerate(oc)])
     check = Checks()
-    ev = dict(ended=0, ended_last_tick=0, idle=0, respawn=0, relaid=0, filtered=0, boundary_runs=0, noised_rows=0,
-              steps=0, clipped=0, undecided_conv=0, undecided_fc=0, worst_mean_factor=0.0,
-              worst_value_factor=0.0)
+    ev = collections.defaultdict(int)
+    for key in ('ended', 'ended_last_tick', 'idle', 'respawn', 'relaid', 'filtered', 'boundary_runs', 'noised_rows',
+                'steps', 'clipped', 'undecided_conv', 'undecided_fc', 'worst_mean_factor', 'worst_value_factor'):
+        ev[key] = 0
     expected_lines = []
     for u, up in enumerate(rec.updates):
         snap = up['snap']
+        believed = np.zeros((H, N), bool)           # rows whose gs slot t is not the true gs
+        ended_rows = []                             # (t, column, eplog row) of the episodes that ended
         # ---- a. the environment, bit for bit, and the episode bookkeeping
         st0 = [o.state() for o in oc]
         for o, (s, g) in zip(oc, st0):
@@ -496,16 +732,11 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
             scaled = _np(tk['scaled'])
             for o in oc:
                 a, b = o.c.a, o.c.b
-                cmd = scaled[a:b]
-                if noise is not None and noise.action_on:
-                    from rl_collision_avoidance_b200.noise import action_host
-                    sid, draw, inp, out = [x for x in rec.noise_cmds if x[0] == o.k][g]
-                    assert draw == g and _bits_equal(_np(inp), cmd), f'tick {g}: the noised command\'s input'
-                    want = action_host(o.cfg, noise, g, cmd, stream_id=o.k)
-                    assert _bits_equal(_np(out), want), f'tick {g}: executed command of {o.c.name}'
-                    ev['noised_rows'] += int((want != cmd).any(1).sum())
-                    cmd = want
-                r = o.tick(cmd, g)
+                believed[t, a:b] = o.believed
+                if u == 1 and t == 0 and o.lat is not None and o.lat.cr[1] > 0:
+                    # rows whose episode ended on update 1's last tick restart their command rings here
+                    ev['ring_restart_on_boundary'] += int((o.prev[:, 3] != 0).sum())
+                r = o.tick(o.command(scaled[a:b], g, rec, ev), g, ev)
                 s, gsn = o.state()
                 what = f'update {u} tick {t} {o.c.name}'
                 assert _bits_equal(snap['stacks'][t + 1, a:b], s), f'{what}: stack'
@@ -514,6 +745,8 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
                 assert _bits_equal(snap['flags'][t, a:b], r['flags']), f'{what}: flags'
                 e = r['ended']
                 assert _bits_equal(snap['eplog'][t, a:b][e], r['eplog'][e]), f'{what}: eplog of ended episodes'
+                assert (r['flags'][e, 2] != 0).all(), f'{what}: an ended episode without a result'
+                ended_rows += [(t, a + i, r['eplog'][i]) for i in np.flatnonzero(e)]
                 # stage 2's liveflag: an idle robot's row repeats its last reward and stays terminal, result 0
                 idle = r['idle']
                 if idle.any():
@@ -569,11 +802,15 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
         for name, got, want in (('targets', gt['targets'], tg64), ('advantages', gt['advs'], adv64)):
             ulp = np.spacing(np.abs(want).astype(np.float32)).astype(np.float64)
             check(f'update {u} GAE {name} (ulps)', float((np.abs(got - want) / ulp).max()), 1.0)
-        fi = ref.filter_index(dones) if stage == 2 else []
+        # the filter: stage 2's get_filter_index, and every row t N + i of a masked column i (stage 1: those alone)
+        fd = ref.filter_index(dones) if stage == 2 else []
+        masked = [t * N + i for t in range(H) for i in np.flatnonzero(col_mask)]
+        fi = sorted(set(fd) | set(masked)) if masked else fd
         assert up['filter_index'] == fi, f'update {u}: filter_index'
         ev['filtered'] += len(fi)
         starts = {o.c.a for o in oc if o.c.a > 0}
-        ev['boundary_runs'] += sum(1 for j in fi if j < N and j in starts)
+        ev['boundary_runs'] += sum(1 for j in fd if j < N and j in starts)
+        ev['masked_boundary_rows'] += _masked_rows_across_boundaries(fd, starts, col_mask, H, N)
         keep = ref.kept_rows(H * N, fi)
         gen = torch.Generator(device='cuda')
         gen.set_state(up['gen_state'])
@@ -583,7 +820,8 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
             batches += ref.minibatches(keep[perm], c['batch'], drop_last=stage == 2)
         assert len(batches) == len(up['steps']) == len(up['rows']), (len(batches), len(up['steps']), len(up['rows']))
         if stage == 1:
-            assert len(batches[-1]) < c['batch'] or (H * N) % c['batch'] == 0
+            assert len(batches[-1]) < c['batch'] or len(keep) % c['batch'] == 0
+            ev['ragged_last'] += int(len(batches[-1]) < c['batch'])
         # the restated normalisation of the device's GAE output: over all H N rows, before np.delete (model/ppo.py:148,
         # 202, 212-218); the device forms it in float32 from float64 moments, a few u of each value (ADV_U below)
         adv_n = torch.from_numpy(ref.normalise(gt['advs'].astype(np.float64)).reshape(-1)).cuda()
@@ -596,11 +834,30 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
             assert _bits_equal(_np(st['p']), _np(up['flat'] if k == 0 else up['steps'][k - 1]['p1'])), \
                 f'{what}: the parameters the step starts from'
             ev['steps'] += 1
+            ev['steps_on_believed_gs'] += int(believed.reshape(-1)[idx].any())
             step_checks(check, what, policy, st, up['rows'][k], torch.from_numpy(idx).cuda(), x, gsx, act_all,
                         lp_all, adv_n, tgt_all, ev)
         # ---- d. the episode log lines of this update, in the trainer's (tick, column) order
         upd_lines.sort(key=lambda x: (x[0], x[1]))
         expected_lines += upd_lines
+        # ---- d. the update's stats against the replay's eplog rows of ended episodes, in (tick, column) order
+        ended_rows.sort(key=lambda x: (x[0], x[1]))
+        ep = np.array([x[2] for x in ended_rows], np.float32).reshape(-1, 8)
+        cols = np.array([x[1] for x in ended_rows], np.int64)
+        s = rec.stats[u]
+        want = _episode_stats(ep)
+        for key in ('episodes', 'success_rate', 'mean_ep_reward'):
+            assert _same(s[key], want[key]), f'update {u}: stats {key} {s[key]} != {want[key]}'
+        want = {o.c.name: _episode_stats(ep[col_comp[cols] == k]) for k, o in enumerate(oc)}
+        assert _same(s['by_scenario'], want), f'update {u}: by_scenario {s["by_scenario"]} != {want}'
+        if pt['masked'] is None:
+            assert 'by_role' not in s
+        else:
+            m = col_mask[cols]
+            want = {'cooperative': _episode_stats(ep[~m]), pt['masked'][0]: _episode_stats(ep[m])}
+            assert _same(s['by_role'], want), f'update {u}: by_role {s["by_role"]} != {want}'
+            ev['episodes_cooperative'] += int((~m).sum())
+            ev['episodes_masked'] += int(m.sum())
     # ---- d. log lines against the bookkeeping
     from rl_collision_avoidance_b200.stage_world import RESULT_STRINGS
     env_lines = [l for l in lines if isinstance(l, str) and l.startswith('Env ')]
@@ -626,15 +883,34 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
         assert abs(got_r - rsum) <= 0.05 + tol + 1e-9, (line, rsum)
     check.done()
     # ---- the events each case exists for
-    print(f'[events] {case}: {ev}, train {t_train:.1f} s, total {time.perf_counter() - t_start:.1f} s')
+    print(f'[events] {case}: {dict(ev)}, train {t_train:.1f} s, total {time.perf_counter() - t_start:.1f} s')
     assert ev['ended'] > 0 and len(env_lines) > 0 and ev['steps'] > 0
-    if case in ('stage1', 'noise'):
+    if case in ('stage1', 'noise', 'latency'):
         assert ev['ended_last_tick'] > 0 and ev['respawn'] > 0
     if noise is not None:
         assert ev['noised_rows'] > 0
-    if case in ('stage2', 'mix'):
+    if case in ('stage2', 'mix', 'dynamics'):
         assert ev['filtered'] > 0 and ev['idle'] > 0 and ev['respawn'] > 0
-    if case in ('random', 'mix'):
+    if case in ('random', 'mix', 'localization'):
         assert ev['relaid'] > 0
     if case == 'mix':
         assert ev['boundary_runs'] > 0, 'no filter run crossed a component boundary'
+    if case == 'latency':
+        assert ev['scan_delayed'] > 0 and ev['command_delayed'] > 0, 'no delayed scan or command'
+        assert ev['ring_restart_on_boundary'] > 0, 'no command ring restarted on the horizon boundary'
+    if case == 'dynamics':
+        assert ev['clamped'] > 0, 'no limit was reached'
+        assert ev['crash_prev_reset'] > 0, 'no moving robot crashed'
+    if case == 'localization':
+        assert ev['believed'] > 0 and ev['relaid_sigma_redrawn'] > 0, 'no believed gs or no redrawn sigma'
+        assert ev['steps_on_believed_gs'] == ev['steps'], 'a PPO step on true gs alone'
+    if case == 'masked_stage1':
+        assert ev['masked_checked'] > 0 and ev['masked_changed'] > 0 and ev['filtered'] > 0
+        assert ev['ragged_last'] == 2, 'the kept rows filled the last minibatch'
+        assert ev['episodes_cooperative'] > 0 and ev['episodes_masked'] > 0, 'a role without episodes'
+    if case == 'chain':
+        for link in ('masked_changed', 'command_delayed', 'noised_rows', 'limited', 'scan_delayed', 'noised_scans',
+                     'believed'):
+            assert ev[link] > 0, f'{link}: this link changed no row'
+        assert ev['masked_checked'] > 0 and ev['episodes_masked'] > 0
+        assert ev['masked_boundary_rows'] > 0, 'no masked row in a filter run crossing a component boundary'
