@@ -36,6 +36,9 @@ every tick, inf one offset per episode), and the speed it reads carries white no
 --crowd K makes K agents of every world a social-force crowd that avoids each other, the other agents (not with
 --crowd-ignores-robots) and, with --crowd-map, the static map, with --crowd-speed, --crowd-strength, --crowd-range and
 --crowd-side-bias; the metrics are also printed per role (DESIGN.md §9t).  Not with --non-cooperative.
+--baseline dwa drives every robot with the dynamic-window baseline, which reads what the policy reads (the newest scan,
+the local goal and its speed), so every sensing perturbation applies to it; --dwa-radius, --dwa-horizon,
+--dwa-heading-time, --dwa-samples V,W, --dwa-accel A[,B], --dwa-brake and --dwa-weights H,C,S set it (DESIGN.md §9u).
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -60,6 +63,7 @@ every tick, inf one offset per episode), and the speed it reads carries white no
         --pose-error 0.1,0.3 --heading-error 0.05 --speed-error 0.05,0.1
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 \\
         --crowd 5 --crowd-map
+    python evaluate.py --scenario stage2 --baseline dwa --num-worlds 8 --episodes 3 --scan-noise 0.05 --timeouts
 """
 import argparse
 import json
@@ -69,6 +73,8 @@ import os
 import torch
 
 from rl_collision_avoidance_b200.crowd import CROWD_FLAGS, Crowd, add_crowd_arguments, crowd_from_arguments
+from rl_collision_avoidance_b200.dwa import DWA_FLAGS, DwaController, add_arguments as add_dwa_arguments, \
+    check_arguments as check_dwa_arguments, from_arguments as dwa_from_arguments
 from rl_collision_avoidance_b200.dynamics import DYNAMICS_FLAGS, Dynamics, add_dynamics_arguments, \
     dynamics_from_arguments
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, PROGRESS_COLUMNS, PROGRESS_DEFAULTS, \
@@ -96,9 +102,10 @@ def main(argv=None):
     ap.add_argument('--scenario', required=True, choices=sorted(AUTO_RESET))
     who = ap.add_mutually_exclusive_group(required=True)
     who.add_argument('--policy', help='state_dict of CNNPolicy (e.g. tests/golden/checkpoints/stage2.pth)')
-    who.add_argument('--baseline', choices=['orca', 'nh-orca'],
-                     help='drive with the ORCA-DD or the NH-ORCA controller instead of a policy')
+    who.add_argument('--baseline', choices=['orca', 'nh-orca', 'dwa'],
+                     help='drive with the ORCA-DD, the NH-ORCA or the dynamic-window controller instead of a policy')
     add_controller_arguments(ap)
+    add_dwa_arguments(ap)
     ap.add_argument('--num-worlds', type=int, default=1)
     ap.add_argument('--episodes', type=int, default=1, help='recorded episodes per robot (circle, random: at most 1)')
     ap.add_argument('--seed', type=int, default=0)
@@ -144,8 +151,10 @@ def main(argv=None):
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
         ap.error('policy file %s not found' % args.policy)
+    check_dwa_arguments(ap, args)
     check_controller_arguments(ap, args)
-    if args.baseline is None and args.orca_map:
+    orca = args.baseline in ('orca', 'nh-orca')
+    if not orca and args.orca_map:
         ap.error('--orca-map applies to --baseline orca / nh-orca only')
     if args.scenario != 'circle' and (args.circle_robots is not None or args.circle_radius is not None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
@@ -168,15 +177,15 @@ def main(argv=None):
     progress = None
     if args.timeouts or args.stall_window is not None:
         progress = {} if args.stall_window is None else {'window': args.stall_window}
-    if args.baseline is not None and (args.scan_noise is not None or args.beam_dropout is not None):
+    if orca and (args.scan_noise is not None or args.beam_dropout is not None):
         ap.error('--scan-noise / --beam-dropout apply to --policy only: the ORCA baselines do not read the scan')
     noise_params = noise_from_arguments(ap, args)
-    if args.baseline is not None and args.scan_delay is not None:
+    if orca and args.scan_delay is not None:
         ap.error('--scan-delay applies to --policy only: the ORCA baselines do not read the scan')
     latency_params = latency_from_arguments(ap, args)
     dynamics_params = dynamics_from_arguments(ap, args)
     localization_params = localization_from_arguments(ap, args)
-    if localization_params is not None and (args.baseline is not None or args.hybrid):
+    if localization_params is not None and (orca or args.hybrid):
         ap.error('--pose-error / --heading-error / --speed-error apply to --policy without --hybrid only: the ORCA '
                  'baselines and the hybrid driver read the true state')
     hybrid_params = None
@@ -200,9 +209,12 @@ def main(argv=None):
     if args.crowd is not None and not 1 <= args.crowd <= sc.robots_per_world:
         ap.error('--crowd must be in 1..%d on %s' % (sc.robots_per_world, args.scenario))
     crowd_params = crowd_from_arguments(ap, args, v_max)
+    dwa_params = dwa_from_arguments(ap, args)
     env = StageWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, seed=args.seed,
                      auto_reset=AUTO_RESET[args.scenario])
-    if args.baseline is not None:
+    if dwa_params is not None:
+        policy, controller = DwaController(env, dwa_params), 'dwa'
+    elif args.baseline is not None:
         policy, controller = controller_from_arguments(env, args)
     else:
         policy = CNNPolicy(frames=LASER_HIST, action_space=2, max_batch=env.N)
@@ -264,6 +276,9 @@ def main(argv=None):
               'seed %d' % (sig(lo['pose_sigma'], ' m'), sig(lo['heading_sigma'], ' rad'), lo['correlation_time'],
                            *lo['speed_sigma'], lo['seed']))
     line(m, env.N)
+    if dwa_params is not None:
+        print('dwa  fallback share %.4f of robot-ticks (no admissible candidate: (0, 0) commanded)'
+              % out['dwa']['fallback_share'])
     if masked is not None:
         k = int(masked.mask.count_nonzero())
         line(out['by_role']['cooperative'], env.N - k, 'cooperative  ')
@@ -309,7 +324,8 @@ def main(argv=None):
             (() if latency is not None else tuple(f[2:].replace('-', '_') for f in LATENCY_FLAGS)) + \
             (() if dynamics is not None else tuple(f[2:].replace('-', '_') for f in DYNAMICS_FLAGS)) + \
             (() if localization is not None else tuple(f[2:].replace('-', '_') for f in LOCALIZATION_FLAGS)) + \
-            (() if crowd is not None else ('crowd',) + tuple(f[2:].replace('-', '_') for f in CROWD_FLAGS))
+            (() if crowd is not None else ('crowd',) + tuple(f[2:].replace('-', '_') for f in CROWD_FLAGS)) + \
+            (() if dwa_params is not None else tuple(f[2:].replace('-', '_') for f in DWA_FLAGS))
         shown = {k: v for k, v in vars(args).items() if k not in hidden}
         res = {'args': shown, 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
@@ -325,6 +341,8 @@ def main(argv=None):
             res['localization'] = out['localization']
         if crowd is not None:
             res['crowd'] = crowd.settings()
+        if dwa_params is not None:
+            res['dwa'] = out['dwa']
         if masked is not None:
             res['by_role'] = out['by_role']
             res['partials_split'] = out['partials_split'].tolist()

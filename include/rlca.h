@@ -1171,6 +1171,54 @@ int rlca_localization_observe_host(const rlca_env_config *cfg, const rlca_locali
                                    const unsigned char *flags_host, const rlca_env_state *state_host,
                                    const float *gs_in_host, float *gs_out_host);
 
+/* =====================================================================================
+ * Dynamic-window baseline (DESIGN.md §9u), csrc/rlca_dwa.cu: a sensor-level classical controller that reads exactly
+ * what the policy reads, so it can stand in the policy's slot of an evaluation (Fox, Burgard, Thrun 1997).
+ *
+ * Inputs, N = num_worlds R rows: stack (N, 3, beams), the policy's scan FIFO, of which only frame 2 (the newest) is
+ * read, a beam's range being (s + 0.5) range_max and a beam at range_max having no return; gs (N, 4), the local goal
+ * x, y in the robot frame and the speed v, w the policy reads; beam_cos_sin (beams, 2), each beam's unit vector in the
+ * robot frame (the env's own beam angles).  Per robot, with the disc of radius rho = radius and constant-(v, w) arcs:
+ *   window     v_samples x w_samples candidates over [v0 - accel dt, v0 + accel dt] n [v_min, v_max] and the same for
+ *              w with angular_accel, (v0, w0) = the gs speed clamped into the action box; a limit of 0 takes the
+ *              whole box.  Sample i of n is lo + (hi - lo) (i / (n - 1)), hi exactly at i = n - 1, the midpoint at
+ *              n = 1; candidate c = iv w_samples + iw.
+ *   clearance  the arc length the disc drives before it first touches a return within reach (v_hi horizon + rho), in
+ *              closed form (straight below |w| = 1e-6 rad/s), capped at v horizon; clearance_cap when v = 0; and 0 for
+ *              every candidate when any return lies within rho.
+ *   admissible clearance > 0 and clearance >= v dt + v^2 / (2 brake).
+ *   score      heading_weight (1 - |bearing of the goal from the pose after heading_time| / pi)
+ *              + clearance_weight min(clearance, cap) / cap + speed_weight v / v_max.
+ * The action is the admissible candidate of highest score, the lowest index among equals, with status 0; with none,
+ * (0, 0) and status 1.  One warp per robot; every function is shared with the host entry and the file is built
+ * without contraction, so the two are equal bit for bit.
+ * ===================================================================================== */
+#define RLCA_DWA_MAX_CANDIDATES 1024
+#define RLCA_DWA_MAX_BEAMS 512
+typedef struct rlca_dwa_params {
+    int32_t v_samples, w_samples;    /* candidate grid over the window, both >= 1, product <= RLCA_DWA_MAX_CANDIDATES */
+    float radius;                    /* disc radius of the robot, m */
+    float horizon;                   /* arc simulated per candidate, s */
+    float heading_time;              /* the goal bearing is scored from the pose predicted after this, s */
+    float accel, angular_accel;      /* window half-widths are accel*dt, angular_accel*dt; 0 = the whole action box */
+    float brake;                     /* admissible iff clearance >= v*dt + v^2 / (2 brake), m/s^2 */
+    float heading_weight, clearance_weight, speed_weight;
+    float clearance_cap;             /* clearance is scored as min(clearance, cap) / cap, m */
+} rlca_dwa_params;
+
+/* The action (N, 2) and status (N) of every robot, on `stream`.  RLCA_ERR_INVALID for a NULL pointer, robots_per_world
+ * or num_worlds < 1, beams outside 2..RLCA_DWA_MAX_BEAMS, a config without finite range_max, dt, v_max > 0 and
+ * v_min <= v_max, w_min <= w_max, a sample count < 1 or a grid above RLCA_DWA_MAX_CANDIDATES, a radius, horizon, brake
+ * or cap that is not finite and > 0, or a heading_time, limit or weight that is not finite and >= 0. */
+int rlca_dwa_action(const rlca_env_config *cfg, const rlca_dwa_params *p, const float *beam_cos_sin_dev,
+                    const float *stack_dev, const float *gs_dev, float *action_dev, int32_t *status_dev, void *stream);
+/* The same on HOST buffers by a serial loop over the same code; equal to rlca_dwa_action bit for bit.  clearance_host
+ * and score_host, each (N, v_samples w_samples) or NULL, receive every candidate's clearance and score (the score of
+ * inadmissible candidates included). */
+int rlca_dwa_action_host(const rlca_env_config *cfg, const rlca_dwa_params *p, const float *beam_cos_sin_host,
+                         const float *stack_host, const float *gs_host, float *action_host, int32_t *status_host,
+                         float *clearance_host, float *score_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

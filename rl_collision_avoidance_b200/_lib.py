@@ -140,6 +140,13 @@ class LocalizationParams(C.Structure):
                 ('stream_id', C.c_uint32)]
 
 
+class DwaParams(C.Structure):
+    """Mirror of rlca_dwa_params (include/rlca.h)."""
+    _fields_ = [('v_samples', C.c_int32), ('w_samples', C.c_int32)] + \
+        [(k, C.c_float) for k in ('radius', 'horizon', 'heading_time', 'accel', 'angular_accel', 'brake',
+                                  'heading_weight', 'clearance_weight', 'speed_weight', 'clearance_cap')]
+
+
 class LocalizationState(C.Structure):
     """Mirror of rlca_localization_state (include/rlca.h): device pointers, or host pointers for the host twin."""
     _fields_ = [('err', C.c_void_p), ('sigma', C.c_void_p)]
@@ -305,6 +312,8 @@ SYMBOLS = {
     'rlca_localization_observe_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LocalizationParams),
                                                  C.POINTER(LocalizationState), C.c_uint32, _P, C.POINTER(EnvState),
                                                  _P, _P]),
+    'rlca_dwa_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(DwaParams), _P, _P, _P, _P, _P, _P]),
+    'rlca_dwa_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(DwaParams), _P, _P, _P, _P, _P, _P, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .dwa import DwaController
 from .model.ppo import generate_action_no_sampling
 from .orca import NhOrcaController, OrcaController, mode_shares
 
@@ -532,7 +533,20 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     With `crowd` (a crowd.Crowd on `env`, DESIGN.md §9t) its agents follow the social force instead, applied where the
     non-cooperative override is, and the result holds the same role splits with the keys 'cooperative' and 'crowd'
     (mode counts over the cooperative robots likewise).  Crowd agents read the true state.  ValueError together with
-    `non_cooperative`: the split has two roles."""
+    `non_cooperative`: the split has two roles.
+
+    With `policy` a dwa.DwaController on `env` (DESIGN.md §9u) every robot is driven by the dynamic-window baseline,
+    which reads what the policy would: on each tick it is called with the stack the policy would read and the gs under
+    localization, env.gs otherwise.  Everything after it is the policy's chain: the masked override, the circle rule,
+    latency, noise and dynamics, so every sensing perturbation applies to it.  The result then also holds 'dwa' (the
+    settings and 'fallback_share': the robot-ticks, over all robot-ticks, on which no candidate was admissible and it
+    commanded (0, 0)).  ValueError together with `hybrid`, which switches a policy."""
+    dwa = isinstance(policy, DwaController)
+    if dwa:
+        if policy.env is not env:
+            raise ValueError('the DWA controller belongs to another env')
+        if hybrid is not None:
+            raise ValueError('hybrid switches a policy; the DWA baseline is not switched')
     if crowd is not None:
         if non_cooperative is not None:
             raise ValueError('crowd and non_cooperative cannot be combined: the metrics split into two roles')
@@ -584,12 +598,16 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         noise.scan(stacks[0])
     gs = localization.observe() if localization is not None else None
     terminal = torch.zeros(N, dtype=torch.bool, device=dev)
+    fallbacks = torch.zeros(N, dtype=torch.int64, device=dev) if dwa else None
     goal_done = 1 if circle else E
     ticks = 0
     for tick in range(int(max_ticks)):
         k = tick & 1
         if isinstance(policy, (OrcaController, NhOrcaController)):
             scaled = policy()
+        elif dwa:
+            scaled = policy(stacks[k], env.gs if gs is None else gs)
+            fallbacks += policy.status()
         else:
             goal, speed = (env.get_local_goal(), env.get_self_speed()) if gs is None else (gs[:, 0:2], gs[:, 2:4])
             _, scaled = generate_action_no_sampling(env=env, state_list=(stacks[k], goal, speed), policy=policy,
@@ -660,4 +678,6 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         out['dynamics'] = dynamics.settings()
     if localization is not None:
         out['localization'] = localization.settings()
+    if dwa:
+        out['dwa'] = dict(policy.settings(), fallback_share=int(fallbacks.sum()) / (ticks * N) if ticks else math.nan)
     return out
