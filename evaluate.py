@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Deterministic evaluation of a policy on stage 1, stage 2, the circle swap or random scenarios, with the metrics of
+"""Deterministic evaluation of a policy on stage 1, stage 2, the circle swap, random or arena scenarios, with the metrics of
 the paper the reference accompanies (DESIGN.md §9c): success / crash / time-out rates, and over the successful episodes
 the mean and population std of extra time, extra distance and average speed.  Every robot drives with the policy's
 mean action (--policy), with the ORCA-DD baseline controller (--baseline orca, DESIGN.md §9d) or with the paper's
@@ -8,7 +8,11 @@ or --max-ticks ticks have run.  --orca-map lets either baseline see the static m
 DESIGN.md §9f).  --non-cooperative K makes K robots of every world drive straight to their goals, ignoring everyone else, and adds the
 metrics of each role (DESIGN.md §9h).  --scenario random gives every world its own layout: --random-robots K robots
 start at random positions in a --random-side S m square on circle.world's map, at least --random-separation D m apart,
-with random goals at least --random-min-travel L m away (defaults 8, 10, 1 and S / 2; DESIGN.md §9i).  --hybrid switches
+with random goals at least --random-min-travel L m away (defaults 8, 10, 1 and S / 2; DESIGN.md §9i).  --scenario arena
+does the same among static obstacles: world w lays out in arena w mod T of a generated map of --arena-count T walled
+arenas of --arena-side S m with --arena-obstacles LO,HI random boxes and discs each, drawn from --arena-seed (another
+seed gives held-out arenas), with --arena-robots, --arena-separation and --arena-min-travel (defaults 64, 10, 4,10, 0,
+8, 1.2 and S / 2; DESIGN.md §9v).  --hybrid switches
 the policy per robot by the nearest return of its newest scan: straight to the goal when it is beyond
 --hybrid-r-safe, the policy's action with v capped at --hybrid-v-safe when it is within --hybrid-r-risk, the policy's
 action otherwise, and prints the share of robot-ticks in each mode (DESIGN.md §9j).  --safety adds how closely the robots
@@ -50,6 +54,7 @@ the local goal and its speed), so every sensing perturbation applies to it; --dw
         --non-cooperative 5
     python evaluate.py --scenario random --baseline nh-orca --orca-map --num-worlds 1024 --random-robots 16
     python evaluate.py --scenario random --policy tests/golden/checkpoints/stage2.pth --num-worlds 1024 --hybrid
+    python evaluate.py --scenario arena --baseline nh-orca --orca-map --num-worlds 64 --arena-seed 1
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage2.pth --num-worlds 8 --episodes 3 --safety
     python evaluate.py --scenario stage2 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3 \\
         --timeouts
@@ -88,8 +93,9 @@ from rl_collision_avoidance_b200.noise import NOISE_FLAGS, Noise, add_noise_argu
 from rl_collision_avoidance_b200.orca import HYBRID_DEFAULTS, Hybrid, NonCooperative, \
     add_arguments as add_controller_arguments, check_arguments as check_controller_arguments, check_hybrid, \
     from_arguments as controller_from_arguments
-from rl_collision_avoidance_b200.scenarios import COMMON, add_random_arguments, check_random_arguments, make_scenario, \
-    random_max_ticks, random_scenario_from_arguments
+from rl_collision_avoidance_b200.scenarios import COMMON, add_arena_arguments, add_random_arguments, \
+    arena_scenario_from_arguments, check_arena_arguments, check_random_arguments, make_scenario, random_max_ticks, \
+    random_scenario_from_arguments
 from rl_collision_avoidance_b200.stage_world import StageWorld
 
 LASER_BEAM = 512
@@ -107,14 +113,16 @@ def main(argv=None):
     add_controller_arguments(ap)
     add_dwa_arguments(ap)
     ap.add_argument('--num-worlds', type=int, default=1)
-    ap.add_argument('--episodes', type=int, default=1, help='recorded episodes per robot (circle, random: at most 1)')
+    ap.add_argument('--episodes', type=int, default=1,
+                    help='recorded episodes per robot (circle, random, arena: at most 1)')
     ap.add_argument('--seed', type=int, default=0)
     ap.add_argument('--max-ticks', type=int, default=None,
                     help='default: episodes x (timeout + 1) on stage 1 / 2, %d on the circle, '
-                         '3 ceil(S sqrt(2) / (v_max dt)) on random' % CIRCLE_MAX_TICKS)
+                         '3 ceil(S sqrt(2) / (v_max dt)) on random and arena' % CIRCLE_MAX_TICKS)
     ap.add_argument('--circle-robots', type=int, default=None, help='K robots on the circle (default: the 50-row table)')
     ap.add_argument('--circle-radius', type=float, default=None, help='circle radius in metres (default 25)')
     add_random_arguments(ap)
+    add_arena_arguments(ap)
     ap.add_argument('--check-every', type=int, default=50)
     ap.add_argument('--non-cooperative', type=int, default=None, metavar='K',
                     help='K robots per world (robots floor(j R / K), j < K) drive straight to their goals and ignore '
@@ -158,6 +166,7 @@ def main(argv=None):
         ap.error('--orca-map applies to --baseline orca / nh-orca only')
     if args.scenario != 'circle' and (args.circle_robots is not None or args.circle_radius is not None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
+    check_arena_arguments(ap, args)
     check_random_arguments(ap, args)
     if args.non_cooperative is None and args.non_cooperative_speed is not None:
         ap.error('--non-cooperative-speed applies with --non-cooperative only')
@@ -202,6 +211,8 @@ def main(argv=None):
         sc = make_scenario(args.scenario, robots_per_world=args.circle_robots, radius=args.circle_radius)
     elif args.scenario == 'random':
         sc = random_scenario_from_arguments(ap, args)
+    elif args.scenario == 'arena':
+        sc = arena_scenario_from_arguments(ap, args, pick=0)
     else:
         sc = make_scenario(args.scenario)
     if args.non_cooperative is not None and not 1 <= args.non_cooperative <= sc.robots_per_world:
@@ -224,7 +235,7 @@ def main(argv=None):
         max_ticks = args.max_ticks
     elif args.scenario == 'circle':
         max_ticks = CIRCLE_MAX_TICKS
-    elif args.scenario == 'random':
+    elif args.scenario in ('random', 'arena'):
         max_ticks = random_max_ticks(sc.layout.side)
     else:
         max_ticks = args.episodes * (sc.timeout + 1)

@@ -759,6 +759,50 @@ int rlca_stack_refresh(const rlca_env_config *cfg, const uint8_t *flags_dev, con
                        const float *gs_src_dev, float *stack_dev, float *gs_dev, void *stream);
 
 /* =====================================================================================
+ * Arena layouts (csrc/rlca_layout.cu, DESIGN.md §9v): one map holds T walled arenas with their own obstacles
+ * (rl_collision_avoidance_b200/arenas.py), and every world lays its robots out in one arena's placeable cells.
+ * ===================================================================================== */
+
+/* The placeable cells of T arenas: arena a owns cells[cell_off[a] .. cell_off[a + 1]), each packed cx | cy << 16
+ * (map column and row).  Device pointers for the device entries, host pointers for the host twins. */
+typedef struct rlca_arena_tables {
+    int32_t num_arenas;          /* T >= 1 */
+    const int32_t *cell_off;     /* T + 1 offsets: cell_off[0] = 0, strictly increasing */
+    const int32_t *cells;        /* cell_off[T] packed cells, each on the cfg's grid_w x grid_h map */
+} rlca_arena_tables;
+
+/* RLCA_OK when host tables hold what the device entries rely on: cell_off[0] = 0, no empty arena, increasing
+ * offsets, every cell on the map.  The device entries cannot read the tables without a synchronisation; run this on
+ * the host copy before uploading them. */
+int rlca_arena_tables_check(const rlca_env_config *cfg, const rlca_arena_tables *tables_host);
+
+/* rlca_layout_random's layout in arenas.  World w (global index g = cfg->world_offset + w) lays out in arena
+ *   pick 0: g mod T;  pick 1: (m T) >> 24, m = 2^24 u0 of the draw (agent g R, episode, draw 0, purpose 0xA0),
+ * and try k of robot r's start (goal) draws (agent g R + r, episode, draw k, purpose 0xA3 (0xA4)): the cell
+ * cells[cell_off[a] + ((m n_a) >> 24)], m = 2^24 u0, n_a the arena's cell count, and the point
+ * x = ((cx - origin_cx) + u1) res, y = ((cy - origin_cy) + u2) res in float32.  Acceptance (separation, min_travel),
+ * heading (purpose 5), the records written and status_dev are rlca_layout_random's; params->side is not read.
+ * RLCA_ERR_INVALID for what rlca_layout_random rejects other than side, min_travel not finite and >= 0, NULL tables,
+ * T < 1 or pick outside {0, 1}. */
+int rlca_layout_arena(const rlca_env_config *cfg, const rlca_layout_params *params, const rlca_arena_tables *tables,
+                      int32_t pick, const rlca_env_state *state, int32_t *status_dev, void *stream);
+/* The same from HOST buffers and host tables by the sequential loop; equal to the device's bit for bit.  Also
+ * RLCA_ERR_INVALID for what rlca_arena_tables_check rejects. */
+int rlca_layout_arena_host(const rlca_env_config *cfg, const rlca_layout_params *params,
+                           const rlca_arena_tables *tables_host, int32_t pick, float *pose_host, float *goal_host,
+                           float *acc_host, int32_t *status_host);
+/* rlca_layout_respawn with the arena sampler: park the latched robots, re-lay a world whose robots are all latched
+ * at episode e = meta.y + 1 (pick 1 draws its arena at that episode too).  rlca_stack_refresh follows as for
+ * rlca_layout_respawn.  RLCA_ERR_INVALID for what rlca_layout_arena rejects, cfg->auto_reset != 0 or a NULL buffer. */
+int rlca_layout_arena_respawn(const rlca_env_config *cfg, const rlca_layout_params *params,
+                              const rlca_arena_tables *tables, int32_t pick, const rlca_env_state *state,
+                              uint8_t *flags_dev, uint8_t *live_dev, int32_t *status_dev, void *stream);
+int rlca_layout_arena_respawn_host(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                   const rlca_arena_tables *tables_host, int32_t pick, float *pose_host,
+                                   float *goal_host, float *acc_host, int32_t *meta_host, uint8_t *flags_host,
+                                   uint8_t *live_host, int32_t *status_host);
+
+/* =====================================================================================
  * Safety metrics (csrc/rlca_safety.cu, DESIGN.md §9m): how closely robots pass and why they crash, per episode of the
  * evaluation tracker above.
  *

@@ -4,8 +4,9 @@
 Same hyper-parameters, log files and checkpoint names; `mpiexec -np 24` is replaced by one process per GPU:
     python ppo_stage1.py --num-worlds 43                       # 1 GPU, 43 x 24 = 1032 robots
     torchrun --nproc-per-node 8 --master-addr 127.0.0.1 ppo_stage1.py --num-worlds 43
-Fine-tuning on random layouts (DESIGN.md §9k) runs through ppo_stage2.py --scenario random, and on a mix of scenarios
-(DESIGN.md §9l) through ppo_stage2.py --mix.  --scan-noise SIGMA_M, --beam-dropout P and --action-noise SIGMA_V[,SIGMA_W]
+Fine-tuning on random layouts (DESIGN.md §9k) runs through ppo_stage2.py --scenario random, on generated obstacle
+arenas (DESIGN.md §9v) through ppo_stage2.py --scenario arena, and on a mix of scenarios (DESIGN.md §9l) through
+ppo_stage2.py --mix.  --scan-noise SIGMA_M, --beam-dropout P and --action-noise SIGMA_V[,SIGMA_W]
 train under lidar and actuation noise (DESIGN.md §9p), with any scenario or mix.  --scan-delay T[,T_MAX] and
 --command-delay T[,T_MAX] train under sensing and command latency, in ticks of 0.1 s (DESIGN.md §9q).
 --accel-limit A[,A_MAX] and --angular-accel-limit B[,B_MAX] train under acceleration limits, in m/s^2 and rad/s^2
@@ -33,8 +34,8 @@ from rl_collision_avoidance_b200.model.diagnostics import check_target_kl, setup
 from rl_collision_avoidance_b200.model.net import Adam, CNNPolicy
 from rl_collision_avoidance_b200.model.ppo import setup_ppo_log
 from rl_collision_avoidance_b200.noise import add_noise_arguments, noise_from_arguments
-from rl_collision_avoidance_b200.scenarios import COMMON, add_random_arguments, check_random_arguments, \
-    random_scenario_from_arguments
+from rl_collision_avoidance_b200.scenarios import COMMON, add_arena_arguments, add_random_arguments, \
+    arena_scenario_from_arguments, check_arena_arguments, check_random_arguments, random_scenario_from_arguments
 from rl_collision_avoidance_b200.stage_world import StageWorld as RandomWorld
 from rl_collision_avoidance_b200.stage_world1 import StageWorld
 from rl_collision_avoidance_b200.trainer import run
@@ -72,14 +73,15 @@ def make_loggers():
     return logger, logger_cal
 
 
-def mix_components(mix, sc, rank):
-    """The Components of a parsed --mix on GPU `rank`: stage 2's 44 robots per world, the shipped circle's 50 and the
-    random scenario `sc`'s K (sc is None without a random component)."""
-    robots = {'stage2': 44, 'circle': 50, 'random': sc.robots_per_world if sc is not None else None}
+def mix_components(mix, sc, rank, arena_sc=None):
+    """The Components of a parsed --mix on GPU `rank`: stage 2's 44 robots per world, the shipped circle's 50, the
+    random scenario `sc`'s K (sc is None without a random component) and the arena scenario `arena_sc`'s K."""
+    robots = {'stage2': 44, 'circle': 50, 'random': sc.robots_per_world if sc is not None else None,
+              'arena': arena_sc.robots_per_world if arena_sc is not None else None}
     return plan(mix, robots, rank)
 
 
-def make_component_env(c, sc, device, seed):
+def make_component_env(c, sc, device, seed, arena_sc=None):
     """The env handle of mix component `c`, built as a single-scenario run of that scenario builds it."""
     kw = dict(num_worlds=c.worlds, device=device, seed=seed, auto_reset=MIX_AUTO_RESET[c.name],
               world_offset=c.world_offset)
@@ -89,6 +91,8 @@ def make_component_env(c, sc, device, seed):
     if c.name == 'circle':
         from rl_collision_avoidance_b200.circle_world import StageWorld as CircleWorld
         return CircleWorld(LASER_BEAM, index=0, num_env=c.robots_per_world, **kw)
+    if c.name == 'arena':
+        return RandomWorld(LASER_BEAM, index=0, scenario=arena_sc, **kw)
     return RandomWorld(LASER_BEAM, index=0, scenario=sc, **kw)
 
 
@@ -113,12 +117,13 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     ap.add_argument('--policy-path', default='policy')
     ap.add_argument('--resume', default=None, help='checkpoint written by this trainer (e.g. policy/Stage1_40): restores the\n'
                     'weights and, from <file>.trainer, the Adam moments / step and the sampling counter')
-    ap.add_argument('--scenario', default=None, choices=[None, 'stage1', 'stage2', 'circle', 'random'],
+    ap.add_argument('--scenario', default=None, choices=[None, 'stage1', 'stage2', 'circle', 'random', 'arena'],
                     help='override the world (e.g. circle: BASELINE config 4 trains on circle.world; random: a new '
-                         'layout in a world whenever all its robots have ended their episodes, stage 2 only)')
+                         'layout in a world whenever all its robots have ended their episodes, stage 2 only; arena: '
+                         'the same in a newly drawn generated obstacle arena)')
     ap.add_argument('--mix', default=None, metavar='NAME:W,...',
                     help='train on several scenarios in one run (stage 2 only; DESIGN.md §9l): world counts per GPU of '
-                         'stage2, circle and random, e.g. stage2:31,random:128,circle:14')
+                         'stage2, circle, random and arena, e.g. stage2:31,random:128,circle:14')
     ap.add_argument('--diagnostics', action='store_true',
                     help='write the health of every PPO update to log/<host>/diag.log (DESIGN.md §9n): approximate KL, '
                          'clip fraction, explained variance, ratio extremes, action saturation, gradient norms')
@@ -126,6 +131,7 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
                     help='skip the remaining epochs of an update once an epoch moved the policy by more than X '
                          '(approx_kl_k3; finite and > 0; implies --diagnostics)')
     add_random_arguments(ap, timeout=True)
+    add_arena_arguments(ap, timeout=True)
     add_noise_arguments(ap)
     add_latency_arguments(ap)
     add_dynamics_arguments(ap)
@@ -157,13 +163,22 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     if args.num_worlds is None:
         args.num_worlds = 1
     random_in_mix = mix is not None and any(name == 'random' for name, _ in mix)
+    arena_in_mix = mix is not None and any(name == 'arena' for name, _ in mix)
+    check_arena_arguments(ap, args, arena_component=arena_in_mix)
     check_random_arguments(ap, args, random_component=random_in_mix)
-    sc = None
+    sc = arena_sc = None
     if args.scenario == 'random' or random_in_mix:
         if stage != 2:
             ap.error('--scenario random trains with ppo_stage2.py: its layouts are per world, and stage 1 re-spawns '
                      'each robot on its own')
         sc = random_scenario_from_arguments(ap, args)
+    if args.scenario == 'arena' or arena_in_mix:
+        if stage != 2:
+            ap.error('--scenario arena trains with ppo_stage2.py: its layouts are per world, and stage 1 re-spawns '
+                     'each robot on its own')
+        arena_sc = arena_scenario_from_arguments(ap, args, pick=1)
+        if mix is None:
+            sc = arena_sc
     rank = int(os.environ.get('RANK', '0'))
     world_size = int(os.environ.get('WORLD_SIZE', '1'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))
@@ -182,8 +197,8 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
         num_env = 50
     comps = None
     if mix is not None:
-        comps = mix_components(mix, sc, rank)
-        env = [make_component_env(c, sc, device, args.seed) for c in comps]
+        comps = mix_components(mix, sc, rank, arena_sc)
+        env = [make_component_env(c, sc, device, args.seed, arena_sc) for c in comps]
     elif sc is not None:
         env = RandomWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, device=device, seed=args.seed,
                           auto_reset=0, world_offset=rank * args.num_worlds)

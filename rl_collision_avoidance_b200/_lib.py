@@ -68,6 +68,11 @@ class LayoutParams(C.Structure):
     _fields_ = [('side', C.c_float), ('separation', C.c_float), ('min_travel', C.c_float)]
 
 
+class ArenaTables(C.Structure):
+    """Mirror of rlca_arena_tables (include/rlca.h)."""
+    _fields_ = [('num_arenas', C.c_int32), ('cell_off', C.c_void_p), ('cells', C.c_void_p)]
+
+
 class HybridParams(C.Structure):
     """Mirror of rlca_hybrid_params (include/rlca.h)."""
     _fields_ = [('r_safe', C.c_float), ('r_risk', C.c_float), ('v_safe', C.c_float), ('heading_gain', C.c_float)]
@@ -271,6 +276,15 @@ SYMBOLS = {
     'rlca_layout_respawn_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), _P, _P, _P, _P, _P, _P,
                                            _P]),
     'rlca_stack_refresh': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, _P, _P]),
+    'rlca_arena_tables_check': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(ArenaTables)]),
+    'rlca_layout_arena': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), C.POINTER(ArenaTables), C.c_int32,
+                                    C.POINTER(EnvState), _P, _P]),
+    'rlca_layout_arena_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), C.POINTER(ArenaTables),
+                                         C.c_int32, _P, _P, _P, _P]),
+    'rlca_layout_arena_respawn': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), C.POINTER(ArenaTables),
+                                            C.c_int32, C.POINTER(EnvState), _P, _P, _P, _P]),
+    'rlca_layout_arena_respawn_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams),
+                                                 C.POINTER(ArenaTables), C.c_int32, _P, _P, _P, _P, _P, _P, _P]),
     'rlca_safety_track': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(SafetyParams), C.POINTER(EnvState),
                                     C.POINTER(EnvState), C.POINTER(StepIO), C.POINTER(EvalState),
                                     C.POINTER(SafetyState), _P]),

@@ -34,7 +34,7 @@ ACTION_BOUND = [[0, -1], [1, 1]]
 # the reference's episode mechanics per scenario: stage 1 re-spawns a robot as soon as it is done
 # (ppo_stage1.py:51-65), stage 2 re-spawns a group when all of it is done (ppo_stage2.py:49-106), circle runs one
 # episode that the caller never resets (circle_test.py:36-84); so does the random scenario, one layout per world
-AUTO_RESET = {'stage1': 1, 'stage2': 2, 'circle': 0, 'random': 0}
+AUTO_RESET = {'stage1': 1, 'stage2': 2, 'circle': 0, 'random': 0, 'arena': 0}
 
 
 def _ptr(t):
@@ -480,8 +480,8 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     tick; auto_reset 0 (circle) runs one episode per robot: a robot that was terminal on the previous tick gets v = 0
     and its first termination is the record, so at most one record per robot.  Robots that hold all their records keep
     driving: they are obstacles for the others.  Completion is checked every `check_every` ticks (one sync each).
-    On a scenario with a random layout (make_scenario('random')) every world first draws its own starts and goals
-    (env.random_layout).  Returns {'partials', 'totals', 'metrics', 'ticks', 'tracker'}.
+    On a scenario with a random layout (make_scenario('random') or 'arena') every world first draws its own starts and
+    goals (env.random_layout).  Returns {'partials', 'totals', 'metrics', 'ticks', 'tracker'}.
 
     With `non_cooperative` (an orca.NonCooperative on `env`) its robots drive straight to their goals instead: the
     override is applied to every tick's action before the circle rule, so they keep the same episode mechanics.  The

@@ -11,10 +11,10 @@ from dataclasses import dataclass
 
 # The scenarios a mix may hold, and the auto_reset each trains with: stage 2 and the circle re-spawn a group inside the
 # tick (auto_reset 2, as ppo_stage2.py trains them alone); a random scenario re-lays finished worlds between ticks
-# (auto_reset 0 with env.live and relayout_finished, §9k).  Stage 1 re-spawns per robot and trains with stage 1's
+# (auto_reset 0 with env.live and relayout_finished, §9k), and so does an arena scenario (§9v).  Stage 1 re-spawns per robot and trains with stage 1's
 # update, so it cannot share a stage-2 update.
-MIX_SCENARIOS = ('stage2', 'circle', 'random')
-MIX_AUTO_RESET = {'stage2': 2, 'circle': 2, 'random': 0}
+MIX_SCENARIOS = ('stage2', 'circle', 'random', 'arena')
+MIX_AUTO_RESET = {'stage2': 2, 'circle': 2, 'random': 0, 'arena': 0}
 
 # Byte alignment of a component's slice of each rollout buffer: the element type rlca_env_step reads or writes a row
 # with (action float2, reward float, flags uchar4, gs and eplog float4), and 16 bytes for the scan FIFO, which
@@ -24,7 +24,7 @@ SLICE_ALIGN = {'action': 8, 'reward': 4, 'flags': 4, 'gs': 16, 'eplog': 16, 'sta
 
 @dataclass(frozen=True)
 class Component:
-    name: str                  # 'stage2', 'circle' or 'random'
+    name: str                  # 'stage2', 'circle', 'random' or 'arena'
     worlds: int                # worlds of this component on one GPU
     robots_per_world: int
     world_offset: int          # global index of this rank's first world of the component

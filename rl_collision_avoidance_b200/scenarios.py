@@ -29,6 +29,20 @@ class Layout:
     min_travel: float          # least start-goal distance
 
 
+@dataclass(frozen=True, eq=False)
+class ArenaLayout:
+    """Parameters of an arena layout (rlca_layout_arena, DESIGN.md §9v): every world lays its robots out in one arena of
+    a generated map (arenas.generate_arenas), in metres."""
+    separation: float          # least start-start and goal-goal distance
+    min_travel: float          # least start-goal distance
+    pick: int                  # 0: world w in arena (world_offset + w) mod T; 1: an arena drawn at every layout
+    tables: object             # arenas.ArenaTables of the map
+    count: int                 # the generator's arguments
+    side: float
+    obstacles: tuple
+    seed: int
+
+
 @dataclass
 class Scenario:
     name: str
@@ -41,7 +55,8 @@ class Scenario:
     init_tab: np.ndarray       # (R,4) x,y,theta,random_flag  float32
     goal_tab: np.ndarray       # (R,4) gx,gy,random_flag,group id   float32
     groups: tuple = ()         # stage-2 group boundaries (model/utils.py:83)
-    layout: Layout | None = None   # random scenario: every world draws its own layout (StageWorld.random_layout)
+    layout: Layout | ArenaLayout | None = None   # random / arena scenario: every world draws its own layout
+                                                 # (StageWorld.random_layout)
 
 
 # constants shared by the three env clients (stage_world1.py:34,183-204)
@@ -122,6 +137,18 @@ def circle_layout(m: WorldMap, robots: int, radius: float):
 RANDOM_DEFAULTS = dict(robots_per_world=8, side=10.0, separation=1.0)     # min_travel defaults to side / 2
 
 
+def _check_separation(who, resolution, D, separation):
+    """(r_c, resolution) in the float32 values rlca_layout_random reads; ValueError for a separation it rejects."""
+    hl, hw = (float(np.float32(COMMON[k])) for k in ('half_len', 'half_wid'))
+    res = float(np.float32(resolution))
+    rc = math.sqrt(hl * hl + hw * hw)
+    d_min = 2.0 * (rc + math.sqrt(2.0) * res)
+    if not (math.isfinite(D) and D > d_min):
+        raise ValueError(f'{who}: separation must be finite and > {d_min:.4g} m (two footprints closer than that can '
+                         f'share a cell), got {separation}')
+    return rc, res
+
+
 def random_layout_params(m: WorldMap, robots: int, side: float, separation: float, min_travel: float) -> Layout:
     """The Layout of a random scenario on map `m` after the checks rlca_layout_random makes (in float32, as it sees the
     values), and that the square grown by the footprint's circumradius r_c and one cell lies on free cells of the map.
@@ -135,13 +162,7 @@ def random_layout_params(m: WorldMap, robots: int, side: float, separation: floa
     if not 0 <= L <= S * math.sqrt(2.0):
         raise ValueError(f'random: min_travel must be in [0, side * sqrt(2)] = [0, {S * math.sqrt(2.0):.4g}], '
                          f'got {min_travel}')
-    hl, hw = (float(np.float32(COMMON[k])) for k in ('half_len', 'half_wid'))
-    res = float(np.float32(m.resolution))
-    rc = math.sqrt(hl * hl + hw * hw)
-    d_min = 2.0 * (rc + math.sqrt(2.0) * res)
-    if not (math.isfinite(D) and D > d_min):
-        raise ValueError(f'random: separation must be finite and > {d_min:.4g} m (two footprints closer than that can '
-                         f'share a cell), got {separation}')
+    rc, res = _check_separation('random', m.resolution, D, separation)
     e = 0.5 * S + rc + res
     ppm = 1.0 / m.resolution
     c0, c1 = math.floor(-e * ppm) + m.origin_cx, math.floor(e * ppm) + m.origin_cx
@@ -188,6 +209,58 @@ def relayout_host(cfg, layout: Layout, pose, goal, acc, meta, flags):
     vp = lambda a: a.ctypes.data_as(C.c_void_p)
     _lib.check(lib.rlca_layout_respawn_host(C.byref(cfg), C.byref(params), vp(pose), vp(goal), vp(acc), vp(meta),
                                             vp(flags), vp(live), vp(status)))
+    return pose, goal, acc, meta, flags, live, status
+
+
+def arena_tables_struct(tables, cell_off_ptr=None, cells_ptr=None):
+    """The rlca_arena_tables of `tables` (arenas.ArenaTables): host pointers into its arrays, or the given device
+    pointers."""
+    from . import _lib
+    if cell_off_ptr is None:
+        cell_off_ptr, cells_ptr = tables.cell_off.ctypes.data, tables.cells.ctypes.data
+    return _lib.ArenaTables(tables.count, cell_off_ptr, cells_ptr)
+
+
+def arena_layout_host(cfg, layout: ArenaLayout, pose, goal, acc, pick=None):
+    """rlca_layout_arena_host: the arena layout of every world of `cfg` written into copies of the host arrays pose,
+    goal, acc (N, 4) float32; `pick` overrides the layout's.  Returns (pose, goal, acc, status (num_worlds,) int32)."""
+    import ctypes as C
+    from . import _lib
+    lib = _lib.load()
+    pose, goal, acc = (np.array(a, np.float32, order='C', copy=True) for a in (pose, goal, acc))
+    n = int(cfg.robots_per_world) * int(cfg.num_worlds)
+    if any(a.shape != (n, 4) for a in (pose, goal, acc)):
+        raise ValueError(f'pose, goal and acc must be ({n}, 4)')
+    status = np.full(int(cfg.num_worlds), -1, np.int32)
+    params = _lib.LayoutParams(layout.side, layout.separation, layout.min_travel)
+    tab = arena_tables_struct(layout.tables)
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    _lib.check(lib.rlca_layout_arena_host(C.byref(cfg), C.byref(params), C.byref(tab),
+                                          layout.pick if pick is None else pick, vp(pose), vp(goal), vp(acc),
+                                          vp(status)))
+    return pose, goal, acc, status
+
+
+def arena_relayout_host(cfg, layout: ArenaLayout, pose, goal, acc, meta, flags, pick=None):
+    """rlca_layout_arena_respawn_host: relayout_host with the arena sampler.  Returns (pose, goal, acc, meta, flags,
+    live (N,) uint8, status (num_worlds,) int32)."""
+    import ctypes as C
+    from . import _lib
+    lib = _lib.load()
+    pose, goal, acc = (np.array(a, np.float32, order='C', copy=True) for a in (pose, goal, acc))
+    meta = np.array(meta, np.int32, order='C', copy=True)
+    flags = np.array(flags, np.uint8, order='C', copy=True)
+    n = int(cfg.robots_per_world) * int(cfg.num_worlds)
+    if any(a.shape != (n, 4) for a in (pose, goal, acc, meta, flags)):
+        raise ValueError(f'pose, goal, acc, meta and flags must be ({n}, 4)')
+    live = np.full(n, 0xFF, np.uint8)
+    status = np.full(int(cfg.num_worlds), -1, np.int32)
+    params = _lib.LayoutParams(layout.side, layout.separation, layout.min_travel)
+    tab = arena_tables_struct(layout.tables)
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    _lib.check(lib.rlca_layout_arena_respawn_host(C.byref(cfg), C.byref(params), C.byref(tab),
+                                                  layout.pick if pick is None else pick, vp(pose), vp(goal), vp(acc),
+                                                  vp(meta), vp(flags), vp(live), vp(status)))
     return pose, goal, acc, meta, flags, live, status
 
 
@@ -245,9 +318,109 @@ def random_scenario_from_arguments(ap, args):
     return sc
 
 
+ARENA_FLAGS = ('--arena-robots', '--arena-count', '--arena-side', '--arena-obstacles', '--arena-seed',
+               '--arena-separation', '--arena-min-travel')
+
+
+def add_arena_arguments(ap, timeout=False):
+    """The --arena-* flags of an arena scenario on an argparse parser; `timeout` adds --arena-timeout (training)."""
+    from .arenas import ARENA_DEFAULTS as A
+    ap.add_argument('--arena-robots', type=int, default=None, metavar='K',
+                    help='arena: robots per world, 2..64 (default %d)' % RANDOM_DEFAULTS['robots_per_world'])
+    ap.add_argument('--arena-count', type=int, default=None, metavar='T',
+                    help='arena: arenas on the generated map (default %d)' % A['count'])
+    ap.add_argument('--arena-side', type=float, default=None, metavar='S',
+                    help='arena: side of an arena\'s interior, m (default %g)' % A['side'])
+    ap.add_argument('--arena-obstacles', default=None, metavar='LO,HI',
+                    help='arena: obstacles per arena, uniform in LO..HI (default %d,%d)' % A['obstacles'])
+    ap.add_argument('--arena-seed', type=int, default=None, metavar='N',
+                    help='arena: seed of the generated arenas; another seed gives held-out arenas (default %d)'
+                         % A['seed'])
+    ap.add_argument('--arena-separation', type=float, default=None, metavar='D',
+                    help='arena: least start-start and goal-goal distance, m (default %g)' % A['separation'])
+    ap.add_argument('--arena-min-travel', type=float, default=None, metavar='L',
+                    help='arena: least start-goal distance, m (default S / 2)')
+    if timeout:
+        ap.add_argument('--arena-timeout', type=int, default=None, metavar='T',
+                        help='arena: ticks after which an episode times out (default 3 ceil(S sqrt(2) / (v_max dt)))')
+
+
+def check_arena_arguments(ap, args, arena_component=False):
+    """ap.error when an --arena-* flag is given without --scenario arena (or an arena component of a trainer's --mix),
+    and when a --random-* flag is given with it."""
+    flags = ARENA_FLAGS + (('--arena-timeout',) if hasattr(args, 'arena_timeout') else ())
+    given = lambda fl: [f for f in fl if getattr(args, f[2:].replace('-', '_'), None) is not None]
+    arena = args.scenario == 'arena' or arena_component
+    if not arena and given(flags):
+        if getattr(args, 'mix', None) is not None:
+            ap.error('%s apply to --scenario arena or an arena component of --mix only' % ' / '.join(flags))
+        ap.error('%s apply to --scenario arena only' % ' / '.join(flags))
+    rnd = RANDOM_FLAGS + (('--random-timeout',) if hasattr(args, 'random_timeout') else ())
+    if args.scenario == 'arena' and given(rnd):
+        ap.error('%s: not with --scenario arena, whose layouts the --arena-* flags shape' % ' / '.join(given(rnd)))
+
+
+def arena_scenario_from_arguments(ap, args, pick):
+    """The arena Scenario the --arena-* flags describe, with `pick` (0 evaluation, 1 training); ap.error for values
+    make_scenario rejects and for an --arena-timeout below 1.  With --arena-timeout defined (a trainer) and not given,
+    the timeout is random_max_ticks(side)."""
+    timeout = getattr(args, 'arena_timeout', None)
+    if timeout is not None and timeout < 1:
+        ap.error('--arena-timeout must be >= 1, got %d' % timeout)
+    obstacles = None
+    if args.arena_obstacles is not None:
+        try:
+            lo, hi = (int(v) for v in args.arena_obstacles.split(','))
+        except ValueError:
+            ap.error('--arena-obstacles must be LO,HI (two integers), got %r' % args.arena_obstacles)
+        obstacles = (lo, hi)
+    try:
+        sc = make_scenario('arena', robots_per_world=args.arena_robots, arenas=args.arena_count,
+                           arena_side=args.arena_side, obstacles=obstacles, arena_seed=args.arena_seed,
+                           separation=args.arena_separation, min_travel=args.arena_min_travel, pick=pick,
+                           timeout=timeout)
+    except ValueError as e:
+        ap.error(str(e))
+    if hasattr(args, 'arena_timeout') and timeout is None:
+        sc = dataclasses.replace(sc, timeout=random_max_ticks(sc.layout.side))
+    return sc
+
+
+def _arena_scenario(robots_per_world, arenas, arena_side, obstacles, arena_seed, separation, min_travel, pick,
+                    timeout) -> Scenario:
+    from .arenas import ARENA_DEFAULTS as A, generate_arenas
+    K = RANDOM_DEFAULTS['robots_per_world'] if robots_per_world is None else robots_per_world
+    if not (int(K) == K and 2 <= K <= 64):
+        raise ValueError(f'arena: robots_per_world must be in 2..64, got {robots_per_world}')
+    K = int(K)
+    S = float(np.float32(A['side'] if arena_side is None else arena_side))
+    if not (math.isfinite(S) and S >= 2.0):
+        raise ValueError(f'arena: side must be finite and >= 2 m, got {arena_side}')
+    D = float(np.float32(A['separation'] if separation is None else separation))
+    L = float(np.float32(0.5 * S if min_travel is None else min_travel))
+    if not 0 <= L <= S * math.sqrt(2.0):
+        raise ValueError(f'arena: min_travel must be in [0, side * sqrt(2)] = [0, {S * math.sqrt(2.0):.4g}], '
+                         f'got {min_travel}')
+    from .arenas import RESOLUTION
+    _check_separation('arena', RESOLUTION, D, separation)
+    if pick not in (0, 1):
+        raise ValueError(f'arena: pick must be 0 (world) or 1 (draw), got {pick}')
+    if timeout is not None and not (int(timeout) == timeout and 1 <= timeout < 2 ** 31):
+        raise ValueError(f'arena: timeout must be an integer >= 1, got {timeout}')
+    T = A['count'] if arenas is None else arenas
+    ob = tuple(A['obstacles'] if obstacles is None else obstacles)
+    seed = A['seed'] if arena_seed is None else int(arena_seed)
+    m, tables = generate_arenas(T, S, ob, seed, K, D)
+    zero = np.zeros((K, 4), np.float32)
+    lay = ArenaLayout(D, L, int(pick), tables, int(T), S, ob, seed)
+    return Scenario('arena', 2, K, 10000 if timeout is None else int(timeout), 0.7, 1, m, zero, zero.copy(), layout=lay)
+
+
 def make_scenario(name: str, map_: WorldMap | None = None, robots_per_world: int | None = None,
                   radius: float | None = None, *, side: float | None = None, separation: float | None = None,
-                  min_travel: float | None = None, timeout: int | None = None) -> Scenario:
+                  min_travel: float | None = None, timeout: int | None = None, arenas: int | None = None,
+                  arena_side: float | None = None, obstacles: tuple | None = None, arena_seed: int | None = None,
+                  pick: int = 0) -> Scenario:
     """`robots_per_world` and `radius` shape the circle scenario (see circle_layout); both None, or 50 robots with no
     radius, keep the shipped 50-row table of the reference's circle.world.
 
@@ -256,11 +429,27 @@ def make_scenario(name: str, map_: WorldMap | None = None, robots_per_world: int
     10), starts and goals at least `separation` m apart (default 1), each goal at least `min_travel` m from its start
     (default side / 2).  `timeout` is the tick budget of an episode (default 10000, the circle's; a training run
     passes random_max_ticks(side)).  The tables are zero; ValueError for parameters rlca_layout_random rejects or a
-    square that leaves the map's free cells."""
+    square that leaves the map's free cells.
+
+    'arena' (DESIGN.md §9v): `robots_per_world` robots (default 8) per world in one of `arenas` walled arenas (default
+    64) of `arena_side` m (default 10) with U{lo..hi} = `obstacles` (default 4..10) random obstacles each, generated from
+    `arena_seed` (default 0; arenas.generate_arenas), on that map with the circle's tick constants.  Starts and goals
+    lie in the arena's placeable cells, `separation` (default 1.2: at 0.2 m rlca_layout_random's bound
+    2 (r_c + sqrt(2) res) is 1.147 m) and `min_travel` (default arena_side / 2) as for random; `pick` 0 puts world w in arena (world_offset + w) mod T (evaluation), 1 draws an arena at every layout
+    (training).  `timeout` as for random.  ValueError for parameters rlca_layout_arena rejects and for arenas the
+    generator refuses, a map off the small-map path included."""
     name = name.lower()
-    if name != 'random' and (side is not None or separation is not None or min_travel is not None or
-                             timeout is not None):
-        raise ValueError('side, separation, min_travel and timeout shape the random scenario only')
+    arena_args = (arenas, arena_side, obstacles, arena_seed)
+    if name not in ('random', 'arena') and (side is not None or separation is not None or min_travel is not None or
+                                            timeout is not None):
+        raise ValueError('side, separation, min_travel and timeout shape the random scenario only (and, but for side, '
+                         'the arena scenario)')
+    if name != 'arena' and (any(a is not None for a in arena_args) or pick != 0):
+        raise ValueError('arenas, arena_side, obstacles, arena_seed and pick shape the arena scenario only')
+    if name == 'arena':
+        if radius is not None or side is not None or map_ is not None:
+            raise ValueError('radius, side and map_ do not shape the arena scenario: it generates its map')
+        return _arena_scenario(robots_per_world, *arena_args, separation, min_travel, pick, timeout)
     if name == 'random':
         if radius is not None:
             raise ValueError('radius shapes the circle scenario only')

@@ -32,7 +32,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .scenarios import Scenario, fill_config, make_scenario
+from .scenarios import ArenaLayout, Scenario, arena_tables_struct, fill_config, make_scenario
 
 RESULT_STRINGS = {0: 0, 1: 'Reach Goal', 2: 'Crashed', 3: 'Time out'}
 
@@ -92,6 +92,14 @@ class StageWorld:
             self._relayout_status = torch.zeros(self.num_worlds, dtype=torch.int32, device=dev)
             self._layout_params = _lib.LayoutParams(self.sc.layout.side, self.sc.layout.separation,
                                                     self.sc.layout.min_travel)
+            self._arena = None
+            if isinstance(self.sc.layout, ArenaLayout):
+                # the arena tables, checked on the host and uploaded once (DESIGN.md §9v)
+                t = self.sc.layout.tables
+                _lib.check(self.lib.rlca_arena_tables_check(C.byref(self.cfg), C.byref(arena_tables_struct(t))))
+                self._arena_off = torch.from_numpy(np.ascontiguousarray(t.cell_off, np.int32)).to(dev)
+                self._arena_cells = torch.from_numpy(np.ascontiguousarray(t.cells, np.int32)).to(dev)
+                self._arena = arena_tables_struct(t, self._arena_off.data_ptr(), self._arena_cells.data_ptr())
         self.reset_world()
 
     # ------------------------------------------------------------------ plumbing
@@ -187,7 +195,8 @@ class StageWorld:
 
     def random_layout(self):
         """A random layout (DESIGN.md §9i) in every world of the current state: starts, goals and headings drawn on the
-        device from the scenario's Layout (rlca_layout_random), then the scan and local goal from the new poses.  One
+        device from the scenario's Layout (rlca_layout_random) or, on an arena scenario, in the world's arena
+        (rlca_layout_arena, §9v), then the scan and local goal from the new poses.  One
         synchronisation reads the per-world status; ValueError names the first world whose robots could not all be
         placed, and that world keeps its rows."""
         lay = self.sc.layout
@@ -196,8 +205,12 @@ class StageWorld:
         params = _lib.LayoutParams(lay.side, lay.separation, lay.min_travel)
         status = torch.empty(self.num_worlds, dtype=torch.int32, device=self.device)
         st = self._state_struct(self._cur)
-        _lib.check(self.lib.rlca_layout_random(C.byref(self.cfg), C.byref(params), C.byref(st), _ptr(status),
-                                               self._stream()))
+        if self._arena is not None:
+            _lib.check(self.lib.rlca_layout_arena(C.byref(self.cfg), C.byref(params), C.byref(self._arena), lay.pick,
+                                                  C.byref(st), _ptr(status), self._stream()))
+        else:
+            _lib.check(self.lib.rlca_layout_random(C.byref(self.cfg), C.byref(params), C.byref(st), _ptr(status),
+                                                   self._stream()))
         self._observe()
         self.live.fill_(1)
         self._relayout_status.zero_()
@@ -207,13 +220,17 @@ class StageWorld:
         bad = torch.nonzero(status).flatten().cpu()
         if len(bad):
             w = int(bad[0])
-            raise ValueError(f'world {int(self.cfg.world_offset) + w}: robot {int(status[w]) - 1} not placed in '
+            where = ''
+            if self._arena is not None:
+                where = ' in its arena' + (f' {(int(self.cfg.world_offset) + w) % self.sc.layout.count}'
+                                           if self.sc.layout.pick == 0 else '')
+            raise ValueError(f'world {int(self.cfg.world_offset) + w}: robot {int(status[w]) - 1} not placed{where} in '
                              f'{int(self.cfg.max_reject)} tries; lower the density')
 
     def relayout_finished(self, stack_out, out=None):
         """After a tick of a random scenario with auto_reset 0 (DESIGN.md §9k), on the env's stream with no
         synchronisation: park the robots whose episode ended (last command 0, `live` 0), give every world whose robots
-        have all ended a new layout (rlca_layout_respawn), scan the new state (rlca_env_observe into the env's own obs /
+        have all ended a new layout (rlca_layout_respawn; rlca_layout_arena_respawn on arenas), scan the new state (rlca_env_observe into the env's own obs /
         gs), and make the re-laid robots' rows of stack_out (N, 3, beams) three copies of the new scan and their
         out['gs'] rows the new local goal and speed (rlca_stack_refresh).  `out` holds the 'flags' and 'gs' buffers the
         tick wrote (default the env's own); re-laid robots get flags[:, 3] (was_reset) = 1.  Pass `live` to the next
@@ -224,8 +241,14 @@ class StageWorld:
         flags, gs = o.get('flags', self.flags), o.get('gs', self.gs)
         st = self._state_struct(self._cur)
         stream = self._stream()
-        _lib.check(self.lib.rlca_layout_respawn(C.byref(self.cfg), C.byref(self._layout_params), C.byref(st),
-                                                _ptr(flags), _ptr(self.live), _ptr(self._relayout_status), stream))
+        if self._arena is not None:
+            _lib.check(self.lib.rlca_layout_arena_respawn(C.byref(self.cfg), C.byref(self._layout_params),
+                                                          C.byref(self._arena), self.sc.layout.pick, C.byref(st),
+                                                          _ptr(flags), _ptr(self.live), _ptr(self._relayout_status),
+                                                          stream))
+        else:
+            _lib.check(self.lib.rlca_layout_respawn(C.byref(self.cfg), C.byref(self._layout_params), C.byref(st),
+                                                    _ptr(flags), _ptr(self.live), _ptr(self._relayout_status), stream))
         self._observe()
         _lib.check(self.lib.rlca_stack_refresh(C.byref(self.cfg), _ptr(flags), _ptr(self.obs), _ptr(self.gs),
                                                _ptr(stack_out), _ptr(gs), stream))
