@@ -43,6 +43,11 @@ every tick, inf one offset per episode), and the speed it reads carries white no
 --baseline dwa drives every robot with the dynamic-window baseline, which reads what the policy reads (the newest scan,
 the local goal and its speed), so every sensing perturbation applies to it; --dwa-radius, --dwa-horizon,
 --dwa-heading-time, --dwa-samples V,W, --dwa-accel A[,B], --dwa-brake and --dwa-weights H,C,S set it (DESIGN.md §9u).
+--planner steers the policy (or --baseline dwa) by a global planner on the device: where a robot's goal is out of sight
+its local goal is the farthest visible cell of the geodesic path; it prints the share of robot-ticks that saw the goal,
+followed a waypoint or had no plan, and the geodesic metrics.  --geodesic prints only the geodesic metrics (the
+geodesic length of every episode and the extra geodesic distance), for any controller (DESIGN.md §9w).  Neither works
+on a map too big to plan on (circle.world).
 
     python evaluate.py --scenario stage1 --policy tests/golden/checkpoints/stage1_2.pth --num-worlds 8 --episodes 3
     python evaluate.py --scenario circle --policy tests/golden/checkpoints/stage2.pth --num-worlds 2 --episodes 1 \\
@@ -89,6 +94,9 @@ from rl_collision_avoidance_b200.latency import LATENCY_FLAGS, Latency, add_late
 from rl_collision_avoidance_b200.localization import LOCALIZATION_FLAGS, Localization, add_localization_arguments, \
     localization_from_arguments
 from rl_collision_avoidance_b200.model.net import CNNPolicy
+from rl_collision_avoidance_b200.planner import PARTIALS as GEODESIC_COLUMNS, Planner, \
+    add_arguments as add_planner_arguments, build_plan_tables, check_arguments as check_planner_arguments, \
+    from_arguments as planner_from_arguments
 from rl_collision_avoidance_b200.noise import NOISE_FLAGS, Noise, add_noise_arguments, noise_from_arguments
 from rl_collision_avoidance_b200.orca import HYBRID_DEFAULTS, Hybrid, NonCooperative, \
     add_arguments as add_controller_arguments, check_arguments as check_controller_arguments, check_hybrid, \
@@ -155,6 +163,7 @@ def main(argv=None):
     add_latency_arguments(ap)
     add_dynamics_arguments(ap)
     add_localization_arguments(ap)
+    add_planner_arguments(ap)
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -197,6 +206,8 @@ def main(argv=None):
     if localization_params is not None and (orca or args.hybrid):
         ap.error('--pose-error / --heading-error / --speed-error apply to --policy without --hybrid only: the ORCA '
                  'baselines and the hybrid driver read the true state')
+    check_planner_arguments(ap, args, localization=localization_params is not None)
+    steer = planner_from_arguments(args)
     hybrid_params = None
     if args.hybrid:
         hybrid_params = dict(HYBRID_DEFAULTS)
@@ -221,6 +232,12 @@ def main(argv=None):
         ap.error('--crowd must be in 1..%d on %s' % (sc.robots_per_world, args.scenario))
     crowd_params = crowd_from_arguments(ap, args, v_max)
     dwa_params = dwa_from_arguments(ap, args)
+    plan_tables = None
+    if steer is not None:
+        try:
+            plan_tables = build_plan_tables(sc.map)
+        except ValueError as e:
+            ap.error('--%s: %s' % ('planner' if steer else 'geodesic', e))
     env = StageWorld(LASER_BEAM, index=0, scenario=sc, num_worlds=args.num_worlds, seed=args.seed,
                      auto_reset=AUTO_RESET[args.scenario])
     if dwa_params is not None:
@@ -254,9 +271,10 @@ def main(argv=None):
     latency = Latency(env, latency_params) if latency_params is not None else None
     dynamics = Dynamics(env, dynamics_params) if dynamics_params is not None else None
     localization = Localization(env, localization_params) if localization_params is not None else None
+    planner = Planner(env, steer, tables=plan_tables) if steer is not None else None
     out = evaluate(env, policy, args.episodes, max_ticks, check_every=args.check_every, non_cooperative=nc, hybrid=hy,
                    safety=safety, progress=progress, noise=noise, latency=latency, dynamics=dynamics,
-                   localization=localization, crowd=crowd)
+                   localization=localization, crowd=crowd, planner=planner)
 
     def line(m, robots, role=''):
         f = lambda k: '%.3f +- %.3f' % m[k]
@@ -294,6 +312,22 @@ def main(argv=None):
         k = int(masked.mask.count_nonzero())
         line(out['by_role']['cooperative'], env.N - k, 'cooperative  ')
         line(out['by_role'][role], k, label)
+    if planner is not None and planner.steer:
+        p = out['planner']
+        print('planner over %d %srobot-ticks: goal visible %.4f  waypoint %.4f  no plan %.4f  (%d components, '
+              'largest field %d cells)' % (p['robot_ticks'], 'cooperative ' if masked is not None else '',
+                                           p['goal_visible'], p['waypoint'], p['no_plan'], p['components'],
+                                           p['max_area']))
+
+    def geodesic_line(g, role=''):
+        print('geodesic  %sreached with a path %d  mean geodesic length %.3f m  extra geodesic distance %.3f +- %.3f m  '
+              'no path %d' % (role, g['reached'], g['mean_length'], *g['extra_geodesic_distance'], g['no_path']))
+
+    if planner is not None:
+        geodesic_line(out['geodesic'])
+        if masked is not None:
+            geodesic_line(out['geodesic_by_role']['cooperative'], 'cooperative  ')
+            geodesic_line(out['geodesic_by_role'][role], label)
     if hy is not None:
         s = out['modes']
         print('hybrid modes over %d %srobot-ticks: policy %.4f  driver %.4f  safe %.4f'
@@ -336,7 +370,8 @@ def main(argv=None):
             (() if dynamics is not None else tuple(f[2:].replace('-', '_') for f in DYNAMICS_FLAGS)) + \
             (() if localization is not None else tuple(f[2:].replace('-', '_') for f in LOCALIZATION_FLAGS)) + \
             (() if crowd is not None else ('crowd',) + tuple(f[2:].replace('-', '_') for f in CROWD_FLAGS)) + \
-            (() if dwa_params is not None else tuple(f[2:].replace('-', '_') for f in DWA_FLAGS))
+            (() if dwa_params is not None else tuple(f[2:].replace('-', '_') for f in DWA_FLAGS)) + \
+            (() if planner is not None else ('planner', 'geodesic'))
         shown = {k: v for k, v in vars(args).items() if k not in hidden}
         res = {'args': shown, 'controller': controller or 'policy', 'robots': env.N,
                'ticks': out['ticks'], 'metrics': m,
@@ -354,6 +389,14 @@ def main(argv=None):
             res['crowd'] = crowd.settings()
         if dwa_params is not None:
             res['dwa'] = out['dwa']
+        if planner is not None:
+            if planner.steer:
+                res['planner'] = out['planner']
+            res['geodesic'] = {'metrics': out['geodesic'], 'columns': list(GEODESIC_COLUMNS),
+                               'totals': out['geodesic_totals'].tolist(), 'partials': out['geodesic_partials'].tolist()}
+            if masked is not None:
+                res['geodesic']['by_role'] = out['geodesic_by_role']
+                res['geodesic']['partials_split'] = out['geodesic_partials_split'].tolist()
         if masked is not None:
             res['by_role'] = out['by_role']
             res['partials_split'] = out['partials_split'].tolist()

@@ -1263,6 +1263,120 @@ int rlca_dwa_action_host(const rlca_env_config *cfg, const rlca_dwa_params *p, c
                          const float *stack_host, const float *gs_host, float *action_host, int32_t *status_host,
                          float *clearance_host, float *score_host);
 
+/* =====================================================================================
+ * Global planner (DESIGN.md §9w), csrc/rlca_plan.cu: geodesic fields to each robot's goal, line-of-sight waypoints as
+ * the policy's local goal, and the geodesic length of every episode.
+ *
+ * Graph: the traversable cells (rl_collision_avoidance_b200/planner.py: no non-free cell within r_c + res sqrt(2) / 2
+ * of the cell's centre, cells outside the grid non-free), 8-neighbour moves of cost 70 (orthogonal) and 99 (diagonal,
+ * allowed only when both orthogonal neighbours are traversable).  D(c) is the least path cost from cell c to a row's
+ * goal entry cell; 0xFFFFFFFF where there is no path.  Cells are the tick's: cx = floor(x ppm) + origin_cx, the same
+ * for y; an index is cy grid_w + cx.
+ *   goal entry   the goal's cell if traversable, else the traversable cell of its 5 x 5 neighbourhood whose centre is
+ *                nearest the goal point (float32, cell units), ties in row-major order; none = no plan
+ *   robot entry  the robot's cell if it lies in the goal entry's component, else the cell of least D in its 5 x 5
+ *                neighbourhood, ties in row-major order; none = no plan
+ *   visible      every cell the closed segment from the robot's centre to a target point meets is traversable, but
+ *                for cells within chessboard distance 1 of either end point's cell (a float32 supercover walk, column
+ *                by column in cell units)
+ * ===================================================================================== */
+/* shared memory of one CTA on sm_90a (227 KB) at 4 bytes per cell: the largest component rectangle a field may span */
+#define RLCA_PLAN_MAX_CELLS 58112
+
+/* The planning graph of a map: label (grid_h, grid_w) int32, the component of each traversable cell and -1 elsewhere;
+ * rects (num_components, 4) int32, each component's bounding rectangle cx0, cy0, cx1, cy1 (inclusive); max_area the
+ * largest rectangle's cell count.  Device pointers for the device entries, host pointers for the host twins. */
+typedef struct rlca_plan_tables {
+    int32_t num_components;
+    int32_t max_area;            /* 1..RLCA_PLAN_MAX_CELLS */
+    const int32_t *label;
+    const int32_t *rects;
+} rlca_plan_tables;
+
+/* RLCA_OK when host tables hold what the device entries rely on: labels in -1..num_components - 1, every rectangle
+ * non-empty, inside the grid and at most max_area cells, every labelled cell inside its component's rectangle,
+ * max_area in 1..RLCA_PLAN_MAX_CELLS.  RLCA_ERR_INVALID otherwise.  Run it on the host copy before uploading. */
+int rlca_plan_tables_check(const rlca_env_config *cfg, const rlca_plan_tables *tables_host);
+
+/* The planner's per-row state, N = num_worlds R rows; device pointers for the device entries, host pointers for the
+ * host twins.  The caller sets entry to -1 before the first rlca_plan_fields and zeroes status_count.
+ *   entry         (N) int32 goal entry cell of the row's field, -1 = no plan
+ *   rect          (N, 4) int32 the field's rectangle (its component's)
+ *   field         (N, max_area) uint32 D over the rectangle, row-major, row width cx1 - cx0 + 1
+ *   list          (N + 1) int32 the rows the last rlca_plan_fields re-planned: count, then the rows (device: in any
+ *                 order; host: ascending)
+ *   status        (N) uint8 of the last rlca_plan_waypoints: 0 goal visible, 1 waypoint, 2 no plan
+ *   status_count  (N, 3) int32, incremented per row and status by every rlca_plan_waypoints
+ *   length        (N) float geodesic length L = D(start entry) res / 70 of the running episode, -1 = no path
+ *   records       (N, episodes) float L of the tracker's records, slot for slot
+ * The tracker fields (length, records, episodes) are read by rlca_plan_track and rlca_plan_reduce only. */
+typedef struct rlca_plan_state {
+    int32_t *entry;
+    int32_t *rect;
+    uint32_t *field;
+    int32_t *list;
+    uint8_t *status;
+    int32_t *status_count;
+    float *length;
+    float *records;
+    int32_t episodes;
+} rlca_plan_state;
+
+/* Re-plan the rows whose goal entry (from state->goal_dev) differs from ps->entry: their field over the component's
+ * rectangle and their entry and rect.  A goal with no entry sets entry -1.  RLCA_ERR_INVALID for a NULL pointer,
+ * robots_per_world outside 1..64, num_worlds < 1, a config without a map, tables with no component or max_area outside
+ * 1..RLCA_PLAN_MAX_CELLS. */
+int rlca_plan_fields(const rlca_env_config *cfg, const rlca_plan_tables *tables, const rlca_plan_state *ps,
+                     const rlca_env_state *state, void *stream);
+/* The same on HOST buffers by a serial loop over the same code; equal to rlca_plan_fields bit for bit.  Also
+ * RLCA_ERR_INVALID for what rlca_plan_tables_check rejects. */
+int rlca_plan_fields_host(const rlca_env_config *cfg, const rlca_plan_tables *tables_host,
+                          const rlca_plan_state *ps_host, const rlca_env_state *state_host);
+
+/* gs_out (N, 4) from the poses and goals of `state` (the state a tick just wrote), the fields and gs_in (N, 4), the gs
+ * the tick wrote: status 0 (goal visible) and 2 (no plan) copy gs_in; status 1 writes goal_speed of the pose and the
+ * centre of the farthest visible cell of a chain of up to 64 steepest-descent steps from the robot's entry cell (ties
+ * E, N, W, S, NE, NW, SW, SE; the first chain cell when none is visible; the entry cell itself when it is the goal
+ * entry), with gs_in's speed half.  RLCA_ERR_INVALID as rlca_plan_fields, and for gs_in equal to gs_out. */
+int rlca_plan_waypoints(const rlca_env_config *cfg, const rlca_plan_tables *tables, const rlca_plan_state *ps,
+                        const rlca_env_state *state, const float *gs_in_dev, float *gs_out_dev, void *stream);
+int rlca_plan_waypoints_host(const rlca_env_config *cfg, const rlca_plan_tables *tables_host,
+                             const rlca_plan_state *ps_host, const rlca_env_state *state_host, const float *gs_in_host,
+                             float *gs_out_host);
+
+/* After rlca_plan_fields of a tick and BEFORE that tick's rlca_eval_track, with the tick's state_in, state_out and
+ * flags: an episode the tracker tracks (closed != meta_in.y) that ends (flags.z != 0) writes its length into the record
+ * slot the tracker fills next; then a re-spawn (flags.w) sets length from the init pose (state_out acc.zw) and the row's
+ * current field.  flags NULL (a run's start, state_in unused): every row's length from its init pose.  RLCA_ERR_INVALID
+ * as rlca_plan_fields, for episodes < 1 or different from the tracker's, or a NULL buffer. */
+int rlca_plan_track(const rlca_env_config *cfg, const rlca_plan_tables *tables, const rlca_plan_state *ps,
+                    const rlca_env_state *state_in, const rlca_env_state *state_out, const uint8_t *flags_dev,
+                    const rlca_eval_state *ev, void *stream);
+int rlca_plan_track_host(const rlca_env_config *cfg, const rlca_plan_tables *tables_host,
+                         const rlca_plan_state *ps_host, const rlca_env_state *state_in_host,
+                         const rlca_env_state *state_out_host, const uint8_t *flags_host, const int32_t *closed_host,
+                         const int32_t *count_host, int32_t episodes);
+
+/* Per-world float64 partials of worlds [world_begin, world_begin + world_count), one thread per world (and role) in
+ * agent-then-record order, no atomics: partials_dev (world_count, RLCA_PLAN_NPARTIALS), or (world_count, 2, ...) split
+ * by an agent mask as rlca_eval_reduce_split splits.  Over recorded episodes that reached the goal with a path, with
+ * the straight-line metric's goal radius: extra = path - max(L - goal_radius, 0). */
+#define RLCA_PLAN_REACHED 0          /* episodes with result 1 and a path */
+#define RLCA_PLAN_SUM_LENGTH 1       /* sum of their L */
+#define RLCA_PLAN_SUM_EXTRA 2        /* sum, sum of squares of their extra geodesic distance */
+#define RLCA_PLAN_SUM_EXTRA_SQ 3
+#define RLCA_PLAN_NO_PATH 4          /* recorded episodes, any result, whose start had no path to the goal */
+#define RLCA_PLAN_NPARTIALS 5
+int rlca_plan_reduce(const rlca_env_config *cfg, const rlca_plan_state *ps, const rlca_eval_state *ev,
+                     int32_t world_begin, int32_t world_count, double *partials_dev, void *stream);
+int rlca_plan_reduce_split(const rlca_env_config *cfg, const rlca_plan_state *ps, const rlca_eval_state *ev,
+                           const uint8_t *mask_dev, int32_t world_begin, int32_t world_count, double *partials_dev,
+                           void *stream);
+/* The same from HOST buffers: geo_records (N, episodes), the tracker's records and count, mask NULL or (N). */
+int rlca_plan_reduce_host(const rlca_env_config *cfg, const float *geo_records_host, const float *eval_records_host,
+                          const int32_t *count_host, const uint8_t *mask_host, int32_t episodes, int32_t world_begin,
+                          int32_t world_count, double *partials_host);
+
 /* sizeof(rlca_env_config) as compiled, so bindings can verify their struct layout. */
 int rlca_sizeof_env_config(void);
 

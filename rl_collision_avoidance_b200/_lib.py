@@ -152,6 +152,18 @@ class DwaParams(C.Structure):
                                   'heading_weight', 'clearance_weight', 'speed_weight', 'clearance_cap')]
 
 
+class PlanTables(C.Structure):
+    """Mirror of rlca_plan_tables (include/rlca.h)."""
+    _fields_ = [('num_components', C.c_int32), ('max_area', C.c_int32), ('label', C.c_void_p), ('rects', C.c_void_p)]
+
+
+class PlanState(C.Structure):
+    """Mirror of rlca_plan_state (include/rlca.h): device pointers, or host pointers for the host twins."""
+    _fields_ = [('entry', C.c_void_p), ('rect', C.c_void_p), ('field', C.c_void_p), ('list', C.c_void_p),
+                ('status', C.c_void_p), ('status_count', C.c_void_p), ('length', C.c_void_p), ('records', C.c_void_p),
+                ('episodes', C.c_int32)]
+
+
 class LocalizationState(C.Structure):
     """Mirror of rlca_localization_state (include/rlca.h): device pointers, or host pointers for the host twin."""
     _fields_ = [('err', C.c_void_p), ('sigma', C.c_void_p)]
@@ -173,6 +185,8 @@ PROGRESS_PARTIALS = tuple(g + '_' + k for g in ('timeout', 'unfinished')
                                     'sum_closest_sq')) + \
     ('sum_still_ticks', 'sum_ticks', 'reached', 'sum_rotation', 'sum_rotation_sq')
 
+# rlca_plan_reduce partials per world (the RLCA_PLAN_* columns of include/rlca.h), all sums
+PLAN_PARTIALS = ('reached', 'sum_length', 'sum_extra', 'sum_extra_sq', 'no_path')
 
 # every symbol include/rlca.h declares: (name, restype, argtypes)
 _P = C.c_void_p
@@ -328,6 +342,24 @@ SYMBOLS = {
                                                  _P, _P]),
     'rlca_dwa_action': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(DwaParams), _P, _P, _P, _P, _P, _P]),
     'rlca_dwa_action_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(DwaParams), _P, _P, _P, _P, _P, _P, _P]),
+    'rlca_plan_tables_check': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables)]),
+    'rlca_plan_fields': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState),
+                                   C.POINTER(EnvState), _P]),
+    'rlca_plan_fields_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState),
+                                        C.POINTER(EnvState)]),
+    'rlca_plan_waypoints': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState),
+                                      C.POINTER(EnvState), _P, _P, _P]),
+    'rlca_plan_waypoints_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState),
+                                           C.POINTER(EnvState), _P, _P]),
+    'rlca_plan_track': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState),
+                                  C.POINTER(EnvState), C.POINTER(EnvState), _P, C.POINTER(EvalState), _P]),
+    'rlca_plan_track_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState),
+                                       C.POINTER(EnvState), C.POINTER(EnvState), _P, _P, _P, C.c_int32]),
+    'rlca_plan_reduce': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanState), C.POINTER(EvalState), C.c_int32,
+                                   C.c_int32, _P, _P]),
+    'rlca_plan_reduce_split': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanState), C.POINTER(EvalState), _P,
+                                         C.c_int32, C.c_int32, _P, _P]),
+    'rlca_plan_reduce_host': (C.c_int, [C.POINTER(EnvConfig), _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
     'rlca_last_error': (C.c_char_p, []),
     'rlca_version': (C.c_char_p, []),
 }

@@ -144,6 +144,26 @@ def _blocked_structure(res=RESOLUTION):
     return gap[:, None] ** 2 + gap[None, :] ** 2 <= rp * rp
 
 
+def placeable_mask(cells, res=RESOLUTION):
+    """(grid_h, grid_w) bool of the placeable cells of a map: no non-free cell (value != 0) within placeable_radius of
+    the cell's centre, cells outside the grid counted as non-free.  The one copy of the rule, for the arena cell lists
+    here and the planner's traversable cells (planner.py, DESIGN.md §9w)."""
+    # the dilation of the non-free cells by _blocked_structure, border 1, one row of the structure at a time: each row
+    # is a symmetric run of offsets, a running maximum along x (seconds instead of minutes on circle.world's 36 M cells)
+    st = _blocked_structure(res)
+    k = st.shape[0] // 2
+    h, w = np.shape(cells)
+    pad = np.ones((h + 2 * k, w + 2 * k), np.uint8)
+    pad[k:k + h, k:k + w] = np.asarray(cells) != 0
+    blocked = np.zeros((h, w), bool)
+    for dj in range(-k, k + 1):
+        run = int(st[dj + k].sum())
+        if run:
+            grown = ndimage.maximum_filter1d(pad[k + dj:k + dj + h], size=run, axis=1)
+            blocked |= grown[:, k:k + w] != 0
+    return ~blocked
+
+
 def _holds(xs, ys, robots, separation):
     """True when a greedy pass in row-major order finds `robots` cell centres at least `separation` apart."""
     px, py = [], []
@@ -179,7 +199,6 @@ def generate_arenas(count=64, side=10.0, obstacles=(4, 10), seed=0, robots_per_w
     res = RESOLUTION
     ocx, ocy = used_w // 2, grid_h // 2
     cells = np.zeros((grid_h, grid_w), np.uint8)
-    structure = _blocked_structure()
     rects = np.zeros((T, 4), np.int32)
     offs, lists = [0], []
     for a in range(T):
@@ -200,7 +219,7 @@ def generate_arenas(count=64, side=10.0, obstacles=(4, 10), seed=0, robots_per_w
                 else:
                     _mark_disc(block, ocx - bx, ocy - by, x, y, rng.uniform(*DISC_RADII))
             block[0, :] = block[-1, :] = block[:, 0] = block[:, -1] = CELL_STATIC
-            ok = ~ndimage.binary_dilation(block != 0, structure=structure, border_value=1)
+            ok = placeable_mask(block)
             lab, k = ndimage.label(ok)                       # 4-connected
             if k == 0:
                 continue

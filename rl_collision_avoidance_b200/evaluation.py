@@ -21,6 +21,7 @@ from . import _lib
 from .dwa import DwaController
 from .model.ppo import generate_action_no_sampling
 from .orca import NhOrcaController, OrcaController, mode_shares
+from .planner import geodesic_metrics, geodesic_totals
 
 COLUMNS = _lib.EVAL_PARTIALS
 NPARTIALS = len(COLUMNS)
@@ -473,7 +474,7 @@ def metrics(tot):
 
 
 def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None,
-             progress=None, noise=None, latency=None, dynamics=None, localization=None, crowd=None):
+             progress=None, noise=None, latency=None, dynamics=None, localization=None, crowd=None, planner=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans
     through the env's FIFO), or with the actions of `policy` when it is an OrcaController or NhOrcaController (orca.py, map-blind or map-aware), until each has `episodes` recorded episodes or `max_ticks` ticks have run, and reduce
     the records.  The episode mechanics are the env's: auto_reset 1 (stage 1) and 2 (stage 2) re-spawn inside the
@@ -540,7 +541,18 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     localization, env.gs otherwise.  Everything after it is the policy's chain: the masked override, the circle rule,
     latency, noise and dynamics, so every sensing perturbation applies to it.  The result then also holds 'dwa' (the
     settings and 'fallback_share': the robot-ticks, over all robot-ticks, on which no candidate was admissible and it
-    commanded (0, 0)).  ValueError together with `hybrid`, which switches a policy."""
+    commanded (0, 0)).  ValueError together with `hybrid`, which switches a policy.
+
+    With `planner` (a planner.Planner on `env`, DESIGN.md §9w) the planner is updated at the start and after every
+    tick, after any latency and noise have touched the stack and before the trackers: it re-plans the robots whose goal
+    changed and keeps every episode's geodesic length.  With planner.steer the policy (or the DWA baseline) reads the
+    planner's gs: a waypoint on the geodesic path as the local goal where the goal is out of sight.  The result then
+    also holds 'geodesic_partials' (num_worlds, planner.NPARTIALS), 'geodesic_totals' and 'geodesic'
+    (planner.geodesic_metrics), with `non_cooperative` or `crowd` also 'geodesic_partials_split' and
+    'geodesic_by_role'; with steer also 'planner': the settings and the share of robot-ticks of the cooperative robots
+    with each status (goal visible, waypoint, no plan).  Without steer it works with every controller.  ValueError for
+    steer with the ORCA baselines or `hybrid` (they read the true goal) and with `localization` (the planner plans from
+    the true pose)."""
     dwa = isinstance(policy, DwaController)
     if dwa:
         if policy.env is not env:
@@ -562,6 +574,18 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             raise ValueError('localization error changes what a policy reads; the ORCA baselines read the true state')
         if hybrid is not None:
             raise ValueError('localization error changes what a policy reads; the hybrid driver reads the true state')
+    if planner is not None:
+        if planner.env is not env:
+            raise ValueError('the planner belongs to another env')
+        if planner.steer:
+            if isinstance(policy, (OrcaController, NhOrcaController)):
+                raise ValueError('the planner steers what a policy reads; the ORCA baselines read the true goal '
+                                 'through their own kernels')
+            if hybrid is not None:
+                raise ValueError('the planner steers what a policy reads; the hybrid driver reads the true goal')
+            if localization is not None:
+                raise ValueError('the planner plans from the true pose; localization error needs a planner on the '
+                                 'believed pose')
     if latency is not None:
         if latency.env is not env:
             raise ValueError('the latency belongs to another env')
@@ -597,6 +621,11 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     if noise is not None:
         noise.scan(stacks[0])
     gs = localization.observe() if localization is not None else None
+    if planner is not None:
+        planner.attach(tracker)
+        pgs = planner.update()
+        if planner.steer:
+            gs = pgs
     terminal = torch.zeros(N, dtype=torch.bool, device=dev)
     fallbacks = torch.zeros(N, dtype=torch.int64, device=dev) if dwa else None
     goal_done = 1 if circle else E
@@ -631,6 +660,10 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             noise.scan(stacks[1 - k], env.flags)
         if localization is not None:
             gs = localization.observe(env.flags)
+        if planner is not None:
+            pgs = planner.update(env.flags)
+            if planner.steer:
+                gs = pgs
         if safe is not None:
             safe.track()
         if prog is not None:
@@ -670,6 +703,18 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             out['progress_partials_split'] = ps
             out['progress_by_role'] = {'cooperative': progress_metrics(progress_totals(ps[:, 0])),
                                        role: progress_metrics(progress_totals(ps[:, 1]))}
+    if planner is not None:
+        gp = planner.partials()
+        out.update(geodesic_partials=gp, geodesic_totals=geodesic_totals(gp))
+        out['geodesic'] = geodesic_metrics(out['geodesic_totals'])
+        if masked is not None:
+            gsp = planner.partials(role_mask=masked.mask)
+            out['geodesic_partials_split'] = gsp
+            out['geodesic_by_role'] = {'cooperative': geodesic_metrics(geodesic_totals(gsp[:, 0])),
+                                       role: geodesic_metrics(geodesic_totals(gsp[:, 1]))}
+        if planner.steer:
+            out['planner'] = dict(planner.settings(),
+                                  **planner.status_shares(None if masked is None else masked.mask))
     if noise is not None:
         out['noise'] = noise.settings()
     if latency is not None:
