@@ -1344,6 +1344,26 @@ int rlca_plan_waypoints_host(const rlca_env_config *cfg, const rlca_plan_tables 
                              const rlca_plan_state *ps_host, const rlca_env_state *state_host, const float *gs_in_host,
                              float *gs_out_host);
 
+/* Training with the planner (DESIGN.md §9x): rlca_plan_waypoints' rows (gs_out, status, status_count, the same rule)
+ * and, in the same launch, a geodesic progress reward.  Per row, from the state the tick (and any re-layout) left:
+ *   psi = 0 for status 0 and 2; for status 1, with w the waypoint (the centre of chain cell c_w),
+ *   psi = (sqrtf(fmaf(dx, dx, dy dy)) + D(c_w) res / 70) - pose.w     (dx, dy = w - pose, float32; D res / 70 as in
+ *         the geodesic length), so that pose.w + psi is the distance to the waypoint plus its geodesic length
+ * With flags (N, 4) of the tick (after rlca_layout_*respawn): flags.x == 0 (a non-terminal tick): reward += progress_gain
+ * (psi_prev - psi) in place; flags.x != 0: the reward is left as it is, and where the tick wrote the row's eplog
+ * (flags.z != 0) its return column eplog[8 a + 2] += progress_gain (psi_start - psi_prev) when eplog is not NULL.  Then
+ * psi_prev = psi, and psi_start = psi where flags.w != 0.  flags NULL (a run's start; reward and eplog unused): psi_prev
+ * = psi_start = psi for every row.  psi_prev and psi_start (N) float are the caller's, as are reward (N) and eplog
+ * (N, 8).  gs_in may equal gs_out (in place).  RLCA_ERR_INVALID as rlca_plan_waypoints, for a NULL psi buffer, psi_prev
+ * equal to psi_start, or flags without reward.  The host twin equals the kernel bit for bit. */
+int rlca_plan_shape(const rlca_env_config *cfg, const rlca_plan_tables *tables, const rlca_plan_state *ps,
+                    float *psi_prev_dev, float *psi_start_dev, const rlca_env_state *state, const uint8_t *flags_dev,
+                    float *reward_dev, float *eplog_dev, const float *gs_in_dev, float *gs_out_dev, void *stream);
+int rlca_plan_shape_host(const rlca_env_config *cfg, const rlca_plan_tables *tables_host,
+                         const rlca_plan_state *ps_host, float *psi_prev_host, float *psi_start_host,
+                         const rlca_env_state *state_host, const uint8_t *flags_host, float *reward_host,
+                         float *eplog_host, const float *gs_in_host, float *gs_out_host);
+
 /* After rlca_plan_fields of a tick and BEFORE that tick's rlca_eval_track, with the tick's state_in, state_out and
  * flags: an episode the tracker tracks (closed != meta_in.y) that ends (flags.z != 0) writes its length into the record
  * slot the tracker fills next; then a re-spawn (flags.w) sets length from the init pose (state_out acc.zw) and the row's

@@ -351,6 +351,10 @@ SYMBOLS = {
                                       C.POINTER(EnvState), _P, _P, _P]),
     'rlca_plan_waypoints_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState),
                                            C.POINTER(EnvState), _P, _P]),
+    'rlca_plan_shape': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState), _P, _P,
+                                  C.POINTER(EnvState), _P, _P, _P, _P, _P, _P]),
+    'rlca_plan_shape_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState), _P, _P,
+                                       C.POINTER(EnvState), _P, _P, _P, _P, _P]),
     'rlca_plan_track': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState),
                                   C.POINTER(EnvState), C.POINTER(EnvState), _P, C.POINTER(EvalState), _P]),
     'rlca_plan_track_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(PlanTables), C.POINTER(PlanState),

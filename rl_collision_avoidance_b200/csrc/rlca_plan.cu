@@ -282,7 +282,7 @@ __global__ void __launch_bounds__(FIELD_THREADS) rlca_plan_field_kernel(PlanMap 
 
 // ------------------------------------------------------------------------------------------------ waypoints
 // One row's plan; lane `lane` of 32 tests chain cells lane and lane + 32 (the host twin passes lane -1 and tests all).
-// Returns the status; gs is written for status 1 only.
+// Returns the status; gs and the waypoint's cell (wx, wy) are written for status 1 only.
 struct RowIn {
     float4 pose, goal;
     int e;
@@ -295,7 +295,7 @@ __host__ __device__ inline bool chain_visible(const PlanMap &m, const RowIn &q, 
     return segment_clear(m, q.pose.x * m.ppm, q.pose.y * m.ppm, centre_u(cx, m.ocx), centre_u(cy, m.ocy));
 }
 
-__device__ __forceinline__ int warp_row(const PlanMap &m, const RowIn &q, int lane, float4 &gs)
+__device__ __forceinline__ int warp_row(const PlanMap &m, const RowIn &q, int lane, float4 &gs, int &wx, int &wy)
 {
     int cx, cy, ex, ey;
     if (q.e < 0 || !cell_of(m, q.pose.x, q.pose.y, cx, cy)) return 2;
@@ -319,8 +319,8 @@ __device__ __forceinline__ int warp_row(const PlanMap &m, const RowIn &q, int la
     const unsigned b0 = __ballot_sync(0xFFFFFFFFu, v0), b1 = __ballot_sync(0xFFFFFFFFu, v1);
     const int best = b1 ? 63 - __clz(b1) : b0 ? 31 - __clz(b0) : 0;
     const int src = best & 31;
-    const int wx = __shfl_sync(0xFFFFFFFFu, best >= 32 ? c1x : c0x, src);
-    const int wy = __shfl_sync(0xFFFFFFFFu, best >= 32 ? c1y : c0y, src);
+    wx = __shfl_sync(0xFFFFFFFFu, best >= 32 ? c1x : c0x, src);
+    wy = __shfl_sync(0xFFFFFFFFu, best >= 32 ? c1y : c0y, src);
     float s, c;
     dev_sincosf(q.pose.z, s, c);
     gs = goal_speed(q.pose, make_float4(centre_u(wx, m.ocx) * m.res, centre_u(wy, m.ocy) * m.res, q.goal.z, q.goal.w),
@@ -329,7 +329,7 @@ __device__ __forceinline__ int warp_row(const PlanMap &m, const RowIn &q, int la
 }
 
 // the host twin of warp_row: the same functions, the chain in one array
-static int host_row(const PlanMap &m, const RowIn &q, float4 &gs)
+static int host_row(const PlanMap &m, const RowIn &q, float4 &gs, int &wx, int &wy)
 {
     int cx, cy, ex, ey;
     if (q.e < 0 || !cell_of(m, q.pose.x, q.pose.y, cx, cy)) return 2;
@@ -352,11 +352,54 @@ static int host_row(const PlanMap &m, const RowIn &q, float4 &gs)
     int best = 0;
     for (int k = 0; k < len; ++k)
         if (chain_visible(m, q, chx[k], chy[k])) best = k;
+    wx = chx[best];
+    wy = chy[best];
     float s, c;
     dev_sincosf(q.pose.z, s, c);
-    gs = goal_speed(q.pose, make_float4(centre_u(chx[best], m.ocx) * m.res, centre_u(chy[best], m.ocy) * m.res,
-                                        q.goal.z, q.goal.w), s, c);
+    gs = goal_speed(q.pose, make_float4(centre_u(wx, m.ocx) * m.res, centre_u(wy, m.ocy) * m.res, q.goal.z, q.goal.w),
+                    s, c);
     return 1;
+}
+
+// ------------------------------------------------------------------------------------------------ shaped reward
+// The geodesic progress potential phi = pose.w + psi of a row after a tick: psi = 0 for status 0 (goal visible) and 2
+// (no plan), and for status 1 the distance to the waypoint w plus the waypoint cell's remaining geodesic length, less
+// the straight-line distance pose.w the tick stored: psi = (|p - w| + D(c_w) res / 70) - pose.w.
+__host__ __device__ inline float psi_excess(const PlanMap &m, const RowIn &q, int st, int wx, int wy)
+{
+    if (st != 1) return 0.0f;
+    const float dx = centre_u(wx, m.ocx) * m.res - q.pose.x, dy = centre_u(wy, m.ocy) * m.res - q.pose.y;
+    const float L = (float)((double)field_at(q.f, q.r, wx, wy) * (double)m.res / 70.0);
+    return (sqrtf(fmaf(dx, dx, dy * dy)) + L) - q.pose.w;
+}
+
+// The per-row buffers and outputs of the shaping launch; flags NULL at a run's start (reward and eplog unused)
+struct ShapeIo {
+    float gain;
+    const uchar4 *flags;
+    float *reward, *eplog, *psi_prev, *psi_start;
+};
+
+// Row a's shaping with its new psi: a non-terminal tick (flags.x == 0) adds gain (psi_prev - psi) to the tick's reward;
+// a tick that wrote the row's eplog (flags.x and flags.z) adds gain (psi_start - psi_prev) to its return, the sum of
+// the episode's shaping terms; every other reward stays the tick's.  Then psi_prev = psi, and psi_start = psi at an
+// episode start (flags.w, or every row at a run's start).
+__host__ __device__ inline void shape_row(const ShapeIo &sh, int a, float psi)
+{
+    bool start = true;
+    if (sh.flags) {
+        const uchar4 fl = sh.flags[a];
+        const float pp = sh.psi_prev[a];
+        if (fl.x == 0) {
+            sh.reward[a] = sh.reward[a] + sh.gain * (pp - psi);
+        } else if (fl.z != 0 && sh.eplog) {
+            float &ret = sh.eplog[(size_t)a * 8 + 2];
+            ret = ret + sh.gain * (sh.psi_start[a] - pp);
+        }
+        start = fl.w != 0;
+    }
+    sh.psi_prev[a] = psi;
+    if (start) sh.psi_start[a] = psi;
 }
 
 __global__ void __launch_bounds__(WP_THREADS) rlca_plan_waypoints_kernel(
@@ -373,11 +416,65 @@ __global__ void __launch_bounds__(WP_THREADS) rlca_plan_waypoints_kernel(
     q.r = q.e >= 0 ? rect[a] : make_int4(0, 0, -1, -1);
     q.f = field + (size_t)a * m.max_area;
     float4 gs = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-    const int st = warp_row(m, q, lane, gs);
+    int wx, wy;
+    const int st = warp_row(m, q, lane, gs, wx, wy);
     if (lane == 0) {
         gs_out[a] = st == 1 ? gs : gs_in[a];
         status[a] = (uint8_t)st;
         status_count[3 * a + st] += 1;
+    }
+}
+
+// rlca_plan_waypoints_kernel's rows and, on lane 0, the row's psi and shaping.  Lane 0 reads the row's gs_in before it
+// writes gs_out, so gs_in and gs_out may be one buffer: neither is __restrict__.  (The waypoint kernel keeps its own
+// copy of these few lines: sharing them through a template body reorders two of its instructions.)
+__global__ void __launch_bounds__(WP_THREADS) rlca_plan_shape_kernel(
+    PlanMap m, int n, ShapeIo sh, const float4 *__restrict__ pose, const float4 *__restrict__ goal,
+    const int32_t *__restrict__ entry, const int4 *__restrict__ rect, const uint32_t *__restrict__ field,
+    const float4 *gs_in, float4 *gs_out, uint8_t *__restrict__ status, int32_t *__restrict__ status_count)
+{
+    const int a = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (a >= n) return;                                 // warp-uniform
+    RowIn q;
+    q.pose = pose[a];
+    q.goal = goal[a];
+    q.e = entry[a];
+    q.r = q.e >= 0 ? rect[a] : make_int4(0, 0, -1, -1);
+    q.f = field + (size_t)a * m.max_area;
+    float4 gs = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    int wx, wy;                                         // written for status 1, the only status psi_excess reads
+    const int st = warp_row(m, q, lane, gs, wx, wy);
+    if (lane == 0) {
+        gs_out[a] = st == 1 ? gs : gs_in[a];
+        status[a] = (uint8_t)st;
+        status_count[3 * a + st] += 1;
+        shape_row(sh, a, psi_excess(m, q, st, wx, wy));
+    }
+}
+
+// the host twin of both kernels over every row (sh NULL: rlca_plan_waypoints_kernel)
+static void host_rows(const PlanMap &m, int n, const rlca_plan_state *ps, const rlca_env_state *state,
+                      const float *gs_in_host, float *gs_out_host, const ShapeIo *sh)
+{
+    const float4 *pose = reinterpret_cast<const float4 *>(state->pose_dev);
+    const float4 *goal = reinterpret_cast<const float4 *>(state->goal_dev);
+    const int4 *rect = reinterpret_cast<const int4 *>(ps->rect);
+    const float4 *gs_in = reinterpret_cast<const float4 *>(gs_in_host);
+    float4 *gs_out = reinterpret_cast<float4 *>(gs_out_host);
+    for (int a = 0; a < n; ++a) {
+        RowIn q;
+        q.pose = pose[a];
+        q.goal = goal[a];
+        q.e = ps->entry[a];
+        q.r = q.e >= 0 ? rect[a] : make_int4(0, 0, -1, -1);
+        q.f = ps->field + (size_t)a * m.max_area;
+        float4 gs = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        int wx = 0, wy = 0;
+        const int st = host_row(m, q, gs, wx, wy);
+        gs_out[a] = st == 1 ? gs : gs_in[a];
+        ps->status[a] = (uint8_t)st;
+        ps->status_count[3 * a + st] += 1;
+        if (sh) shape_row(*sh, a, psi_excess(m, q, st, wx, wy));
     }
 }
 
@@ -642,25 +739,70 @@ extern "C" int rlca_plan_waypoints_host(const rlca_env_config *cfg, const rlca_p
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_plan_waypoints_host: a buffer is NULL");
     if (gs_in_host == gs_out_host)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_plan_waypoints_host: gs_in and gs_out alias");
+    host_rows(m, cfg->robots_per_world * cfg->num_worlds, ps_host, state_host, gs_in_host, gs_out_host, nullptr);
+    return RLCA_OK;
+}
+
+static int shape_args(const char *who, const rlca_plan_state *ps, const float *psi_prev, const float *psi_start,
+                      const rlca_env_state *state, const uint8_t *flags, const float *reward, const float *gs_in,
+                      const float *gs_out)
+{
+    if (!state || !state->pose_dev || !state->goal_dev || !gs_in || !gs_out || !ps->entry || !ps->rect ||
+        !ps->field || !ps->status || !ps->status_count || !psi_prev || !psi_start)
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: a buffer is NULL", who);
+    if (psi_prev == psi_start) return rlca_set_err(RLCA_ERR_INVALID, "%s: psi_prev and psi_start alias", who);
+    if (flags && !reward) return rlca_set_err(RLCA_ERR_INVALID, "%s: after a tick the reward is needed", who);
+    return RLCA_OK;
+}
+
+extern "C" int rlca_plan_shape(const rlca_env_config *cfg, const rlca_plan_tables *tables, const rlca_plan_state *ps,
+                               float *psi_prev_dev, float *psi_start_dev, const rlca_env_state *state,
+                               const uint8_t *flags_dev, float *reward_dev, float *eplog_dev, const float *gs_in_dev,
+                               float *gs_out_dev, void *stream)
+{
+    PlanMap m;
+    int rc = plan_args("rlca_plan_shape", cfg, tables, ps, m);
+    if (rc) return rc;
+    if ((rc = shape_args("rlca_plan_shape", ps, psi_prev_dev, psi_start_dev, state, flags_dev, reward_dev, gs_in_dev,
+                         gs_out_dev)))
+        return rc;
+    ShapeIo sh;
+    sh.gain = cfg->progress_gain;
+    sh.flags = reinterpret_cast<const uchar4 *>(flags_dev);
+    sh.reward = reward_dev;
+    sh.eplog = eplog_dev;
+    sh.psi_prev = psi_prev_dev;
+    sh.psi_start = psi_start_dev;
     const int n = cfg->robots_per_world * cfg->num_worlds;
-    const float4 *pose = reinterpret_cast<const float4 *>(state_host->pose_dev);
-    const float4 *goal = reinterpret_cast<const float4 *>(state_host->goal_dev);
-    const int4 *rect = reinterpret_cast<const int4 *>(ps_host->rect);
-    const float4 *gs_in = reinterpret_cast<const float4 *>(gs_in_host);
-    float4 *gs_out = reinterpret_cast<float4 *>(gs_out_host);
-    for (int a = 0; a < n; ++a) {
-        RowIn q;
-        q.pose = pose[a];
-        q.goal = goal[a];
-        q.e = ps_host->entry[a];
-        q.r = q.e >= 0 ? rect[a] : make_int4(0, 0, -1, -1);
-        q.f = ps_host->field + (size_t)a * m.max_area;
-        float4 gs = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-        const int st = host_row(m, q, gs);
-        gs_out[a] = st == 1 ? gs : gs_in[a];
-        ps_host->status[a] = (uint8_t)st;
-        ps_host->status_count[3 * a + st] += 1;
-    }
+    const int rows_per_cta = WP_THREADS / 32;
+    rlca_plan_shape_kernel<<<(n + rows_per_cta - 1) / rows_per_cta, WP_THREADS, 0, (cudaStream_t)stream>>>(
+        m, n, sh, reinterpret_cast<const float4 *>(state->pose_dev), reinterpret_cast<const float4 *>(state->goal_dev),
+        ps->entry, reinterpret_cast<const int4 *>(ps->rect), ps->field, reinterpret_cast<const float4 *>(gs_in_dev),
+        reinterpret_cast<float4 *>(gs_out_dev), ps->status, ps->status_count);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_plan_shape_host(const rlca_env_config *cfg, const rlca_plan_tables *tables_host,
+                                    const rlca_plan_state *ps_host, float *psi_prev_host, float *psi_start_host,
+                                    const rlca_env_state *state_host, const uint8_t *flags_host, float *reward_host,
+                                    float *eplog_host, const float *gs_in_host, float *gs_out_host)
+{
+    PlanMap m;
+    int rc = plan_args("rlca_plan_shape_host", cfg, tables_host, ps_host, m);
+    if (rc) return rc;
+    if ((rc = rlca_plan_tables_check(cfg, tables_host))) return rc;
+    if ((rc = shape_args("rlca_plan_shape_host", ps_host, psi_prev_host, psi_start_host, state_host, flags_host,
+                         reward_host, gs_in_host, gs_out_host)))
+        return rc;
+    ShapeIo sh;
+    sh.gain = cfg->progress_gain;
+    sh.flags = reinterpret_cast<const uchar4 *>(flags_host);
+    sh.reward = reward_host;
+    sh.eplog = eplog_host;
+    sh.psi_prev = psi_prev_host;
+    sh.psi_start = psi_start_host;
+    host_rows(m, cfg->robots_per_world * cfg->num_worlds, ps_host, state_host, gs_in_host, gs_out_host, &sh);
     return RLCA_OK;
 }
 

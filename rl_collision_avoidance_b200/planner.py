@@ -4,13 +4,18 @@ as the policy's local goal where the goal is out of sight, and the geodesic leng
     planner = Planner(env, steer=True)        # the map's planning graph, uploaded once
     gs = planner.update(flags)                # after each tick (None at a run's start): the gs the policy reads
 
+Training with the planner (DESIGN.md §9x): Planner(env, reward=True).update(flags, reward, eplog, gs) also adds the
+geodesic progress shaping to the tick's reward (and to the return of the episodes the tick ended) and writes the
+waypoint gs into gs in place, in one launch (rlca_plan_shape).
+
 The graph (build_plan_tables, host, numpy and scipy, once per map): the traversable cells are the arena generator's
 placeable cells (arenas.placeable_mask: a footprint centred anywhere in the cell, at any heading, covers free cells
 only), moves go to the 8 neighbours at cost 70 (orthogonal) or 99 (diagonal, only where both orthogonal neighbours
 are traversable), and every 4-connected component keeps its bounding rectangle.  A goal's field spans its component's
 rectangle in one CTA's shared memory, so a map whose largest rectangle exceeds RLCA_PLAN_MAX_CELLS cells is refused.
 
-Kernels: csrc/rlca_plan.cu (rlca_plan_fields, rlca_plan_waypoints, rlca_plan_track, rlca_plan_reduce).  The host
+Kernels: csrc/rlca_plan.cu (rlca_plan_fields, rlca_plan_waypoints, rlca_plan_shape, rlca_plan_track,
+rlca_plan_reduce).  The host
 twins below run the same code on the CPU and equal the kernels bit for bit.
 """
 from __future__ import annotations
@@ -96,10 +101,14 @@ class Planner:
     or there is no plan, the waypoint's local goal elsewhere (one buffer reused by every call); without `steer` it
     returns env.gs.  `tables` are build_plan_tables(env.sc.map), built when None.  With a tracker attached (`attach`,
     as evaluate() does) it also keeps every episode's geodesic length, read at the tracker's episode boundaries: call
-    update before the tracker's own track()."""
+    update before the tracker's own track().
+    With `reward` (which needs `steer`) update also shapes the tick's reward by geodesic progress (DESIGN.md §9x):
+    psi_prev and psi_start (N) hold each row's potential excess after the last update and at its episode's start."""
 
-    def __init__(self, env, steer=True, tables=None):
-        self.env, self.steer = env, bool(steer)
+    def __init__(self, env, steer=True, tables=None, reward=False):
+        if reward and not steer:
+            raise ValueError('the planner shapes the reward towards the waypoint it steers by: reward needs steer')
+        self.env, self.steer, self.reward = env, bool(steer), bool(reward)
         self.tables = build_plan_tables(env.sc.map) if tables is None else tables
         check_tables(env.cfg, self.tables)
         N, dev = env.N, env.device
@@ -113,6 +122,8 @@ class Planner:
         self._status = torch.zeros(N, dtype=torch.uint8, device=dev)
         self.status_count = torch.zeros(N, 3, dtype=torch.int32, device=dev)
         self.gs = torch.zeros(N, 4, device=dev)
+        self.psi_prev = torch.zeros(N, device=dev) if self.reward else None
+        self.psi_start = torch.zeros(N, device=dev) if self.reward else None
         self.tracker = self.length = self.records = None
         self._build_state()
 
@@ -133,16 +144,34 @@ class Planner:
         self.status_count.zero_()
         self._build_state()
 
-    def update(self, flags=None):
+    def update(self, flags=None, reward=None, eplog=None, gs=None):
         """After a tick, with its env.flags (None at a run's start, before any tick): fields, waypoints (with steer)
-        and the geodesic tracker (when attached), on the env's stream."""
+        and the geodesic tracker (when attached), on the env's stream.  `gs` (N, 4), the buffer the tick (and any
+        re-layout) wrote the gs into, is read in place of env.gs and receives the waypoint gs in place; it is then what
+        update returns.  With `reward` the same launch shapes `reward` (N) and the return column of `eplog` (N, 8) in
+        place, the tick's buffers (env.reward and env.eplog when None); None flags only set psi_prev = psi_start."""
         env = self.env
         cfg, stream = C.byref(env.cfg), env._stream()
         s_out = env._state_struct(env._cur)
         _lib.check(env.lib.rlca_plan_fields(cfg, C.byref(self._t), C.byref(self._st), C.byref(s_out), stream))
-        if self.steer:
+        if self.reward:
+            if flags is not None:
+                reward = env.reward if reward is None else reward
+                eplog = env.eplog if eplog is None else eplog
+                _check_rows(reward, (env.N,), 'reward')
+                _check_rows(eplog, (env.N, 8), 'eplog')
+            else:
+                reward = eplog = None
+            gs_in = env.gs if gs is None else _check_rows(gs, (env.N, 4), 'gs')
+            _lib.check(env.lib.rlca_plan_shape(cfg, C.byref(self._t), C.byref(self._st), _ptr(self.psi_prev),
+                                               _ptr(self.psi_start), C.byref(s_out), _ptr(flags), _ptr(reward),
+                                               _ptr(eplog), _ptr(gs_in), _ptr(self.gs if gs is None else gs), stream))
+        elif self.steer:
             _lib.check(env.lib.rlca_plan_waypoints(cfg, C.byref(self._t), C.byref(self._st), C.byref(s_out),
-                                                   _ptr(env.gs), _ptr(self.gs), stream))
+                                                   _ptr(env.gs if gs is None else _check_rows(gs, (env.N, 4), 'gs')),
+                                                   _ptr(self.gs), stream))
+            if gs is not None:
+                gs.copy_(self.gs)
         if self.tracker is not None:
             if flags is not None and not env._ticked:
                 raise RuntimeError('Planner.update(flags) needs a tick: call env.control_vel first')
@@ -150,6 +179,8 @@ class Planner:
             _lib.check(env.lib.rlca_plan_track(cfg, C.byref(self._t), C.byref(self._st),
                                                C.byref(s_in) if s_in is not None else None, C.byref(s_out),
                                                _ptr(flags), C.byref(self.tracker._st), stream))
+        if gs is not None and self.steer:
+            return gs
         return self.gs if self.steer else env.gs
 
     def status(self):
@@ -253,6 +284,13 @@ class HostState:
         return self.field[a, :w * h].reshape(h, w)
 
 
+def _check_rows(t, shape, name):
+    """t when it is a contiguous float32 tensor of `shape` on the planner's device rows; ValueError otherwise."""
+    if t.dtype != torch.float32 or tuple(t.shape) != shape or not t.is_contiguous() or not t.is_cuda:
+        raise ValueError(f'{name} must be a contiguous float32 device tensor of shape {shape}')
+    return t
+
+
 def _f32(a, shape, name):
     a = np.ascontiguousarray(a, np.float32)
     if a.shape != shape:
@@ -278,6 +316,38 @@ def waypoints_host(cfg, tables, state: HostState, pose, goal, gs_in):
     st = _lib.EnvState(p.ctypes.data, g.ctypes.data, None, None)
     _lib.check(_lib.load().rlca_plan_waypoints_host(C.byref(cfg), C.byref(tables.struct()), C.byref(state.struct()),
                                                     C.byref(st), _vp(s), _vp(out)))
+    return out
+
+
+def shape_host(cfg, tables, state: HostState, psi_prev, psi_start, pose, goal, gs_in, flags=None, reward=None,
+               eplog=None, in_place=False):
+    """rlca_plan_shape_host: gs_out (N, 4) float32 (gs_in itself, written in place, with `in_place`: gs_in must then be
+    a contiguous float32 array).  psi_prev, psi_start (N), reward (N) and eplog (N, 8), contiguous float32 numpy arrays,
+    are updated in place; flags (N, 4) uint8 or None (a run's start); state.status and state.status_count updated."""
+    N = len(state.entry)
+    p, g = _f32(pose, (N, 4), 'pose'), _f32(goal, (N, 4), 'goal')
+    bufs = [(psi_prev, (N,), 'psi_prev'), (psi_start, (N,), 'psi_start')]
+    if flags is not None:
+        bufs.append((reward, (N,), 'reward'))
+        if eplog is not None:
+            bufs.append((eplog, (N, 8), 'eplog'))
+    if in_place:
+        bufs.append((gs_in, (N, 4), 'gs_in'))
+    for a, shape, name in bufs:
+        if not (isinstance(a, np.ndarray) and a.dtype == np.float32 and a.shape == shape and a.flags.c_contiguous):
+            raise ValueError(f'{name} must be a contiguous float32 array of shape {shape}, updated in place')
+    s = gs_in if in_place else _f32(gs_in, (N, 4), 'gs_in')
+    out = s if in_place else np.zeros_like(s)
+    fl = None
+    if flags is not None:
+        fl = np.ascontiguousarray(flags, np.uint8)
+        if fl.shape != (N, 4):
+            raise ValueError('flags must be (N, 4)')
+    st = _lib.EnvState(p.ctypes.data, g.ctypes.data, None, None)
+    _lib.check(_lib.load().rlca_plan_shape_host(C.byref(cfg), C.byref(tables.struct()), C.byref(state.struct()),
+                                                _vp(psi_prev), _vp(psi_start), C.byref(st), _vp(fl),
+                                                _vp(reward if flags is not None else None),
+                                                _vp(eplog if flags is not None else None), _vp(s), _vp(out)))
     return out
 
 

@@ -24,6 +24,7 @@ from .latency import Latency
 from .localization import Localization
 from .noise import Noise
 from .orca import NonCooperative
+from .planner import Planner
 from .stage_world import RESULT_STRINGS
 
 
@@ -61,6 +62,7 @@ class _Component:
         self.dynamics = dynamics                        # dynamics.Dynamics of the env, or None
         self.localization = localization                # localization.Localization of the env, or None
         self.masked = None                              # orca.NonCooperative or crowd.Crowd of the env, or None
+        self.planner = None                             # planner.Planner of the env (steering), or None
         self.ticked = False                             # a tick has run, so self.flags holds its flags
         self.name = env.sc.name
         self.relayout = env.sc.layout is not None
@@ -93,6 +95,8 @@ class _Component:
         self.gs[0] = e.gs
         if self.localization is not None:
             self.localization.observe(gs=self.gs[0], out=self.gs[0])    # every row starts an episode
+        if self.planner is not None:
+            self.planner.update(None, gs=self.gs[0])    # the first waypoints; every row starts an episode
 
     def tick(self, t):
         """Tick t on the component's slices, after the policy has written ro.scaled.  With noise the robots execute
@@ -103,7 +107,9 @@ class _Component:
         command, last of all, is limited in acceleration, with the same flags of the tick before.  With localization
         the gs the tick and the re-layout wrote becomes, in place and last of all, the gs the robot believes, with the
         flags of this tick.  With masked agents their rows of ro.scaled are overwritten first, before any latency; PPO
-        keeps the policy's sampled action in ro.actions."""
+        keeps the policy's sampled action in ro.actions.  With a planner the gs the tick and the re-layout wrote becomes,
+        in place and last of all, the waypoint gs, and a reward planner shapes the tick's reward and the returns of the
+        episodes it ended in place, with the flags as the re-layout left them."""
         e = self.env
         if self.masked is not None:
             self.masked.apply(self.scaled)
@@ -128,6 +134,8 @@ class _Component:
             self.noise.scan(self.stacks[t + 1], self.flags[t])
         if self.localization is not None:
             self.localization.observe(self.flags[t], gs=self.gs[t + 1], out=self.gs[t + 1])
+        if self.planner is not None:
+            self.planner.update(self.flags[t], reward=self.rewards[t], eplog=self.eplog[t], gs=self.gs[t + 1])
 
 
 def compose(envs, ro, noise=None, latency=None, dynamics=None, localization=None):
@@ -149,6 +157,41 @@ def compose(envs, ro, noise=None, latency=None, dynamics=None, localization=None
         for c in comps:
             c.check_aligned()
     return comps
+
+
+PLANNERS = ('geodesic', 'straight')
+
+
+def attach_planners(comps, planner, localization=None, tables=None):
+    """Give every component a planner.Planner of its env that steers by waypoints: 'geodesic' also shapes the reward by
+    geodesic progress, 'straight' keeps the tick's reward.  None attaches nothing.  `tables`: one
+    planner.PlannerTables per component (build_plan_tables of its env's map), or None to build them here.  ValueError
+    for another value, with localization error (the planner plans from the true pose) and, naming the map and the
+    limit, for a map the planner refuses (build_plan_tables)."""
+    if planner is None:
+        return
+    if planner not in PLANNERS:
+        raise ValueError('planner must be None or one of %s, got %r' % (', '.join(PLANNERS), planner))
+    if localization is not None:
+        raise ValueError('the planner plans from the true pose; localization error needs a planner on the believed '
+                         'pose')
+    if tables is not None and len(tables) != len(comps):
+        raise ValueError('planner tables: %d given for %d components' % (len(tables), len(comps)))
+    for k, c in enumerate(comps):
+        c.planner = Planner(c.env, steer=True, reward=planner == 'geodesic',
+                            tables=None if tables is None else tables[k])
+
+
+def _status_shares(comps):
+    """The share of robot-ticks of each planner status since the last call, over every component's rows; zeroes the
+    counts."""
+    tot = sum(c.planner.status_count.to(torch.int64).sum(0) for c in comps).cpu().numpy()
+    for c in comps:
+        c.planner.status_count.zero_()
+    n = int(tot.sum())
+    out = {k: (int(v) / n if n else float('nan')) for k, v in zip(('goal_visible', 'waypoint', 'no_plan'), tot)}
+    out['robot_ticks'] = n
+    return out
 
 
 def masked_agents(comps, non_cooperative=None, crowd=None):
@@ -206,7 +249,8 @@ def _check_mix(envs, stage):
 
 def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logger_cal=None, stage=1, max_updates=None,
         process_group=None, rank=0, save_every=20, generator=None, start_update=0, diagnostics=False, target_kl=None,
-        noise=None, latency=None, dynamics=None, localization=None, non_cooperative=None, crowd=None):
+        noise=None, latency=None, dynamics=None, localization=None, non_cooperative=None, crowd=None, planner=None,
+        planner_tables=None):
     """hp: dict with HORIZON, GAMMA, LAMDA, BATCH_SIZE, EPOCH, COEFF_ENTROPY, CLIP_VALUE, NUM_ENV, OBS_SIZE, ACT_SIZE,
     LASER_HIST, MAX_EPISODES.  `start_update` continues the checkpoint numbering of a resumed run.
     A random scenario (env.sc.layout, DESIGN.md §9k) trains with stage 2's update on per-world layouts: the env runs
@@ -237,6 +281,12 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     masked agents into every world of every component (masked_agents); their rows of the action are overwritten before
     any latency, and every row of their columns is left out of every PPO update (stage 1: filter_index; stage 2:
     united with get_filter_index).  The stats then also hold 'by_role' {'cooperative', 'non_cooperative' or 'crowd'}.
+    `planner` ('geodesic' or 'straight', DESIGN.md §9x) gives component k a planner.Planner (attach_planners): every
+    gs the policy reads (ro.gs, slot 0 and every slot a tick wrote, after any re-layout) is the waypoint gs, so PPO
+    stores and re-evaluates what the policy read; 'geodesic' also shapes ro.rewards and the episodes' returns by
+    geodesic progress, 'straight' keeps the tick's reward.  The stats then also hold 'planner', the status shares of the
+    update's robot-ticks.  Refused with localization error and on maps the planner refuses.  None launches nothing.
+    `planner_tables` (one planner.PlannerTables per env, in order) saves building the planning graphs again.
     Returns per-update stats (for tests / benchmarks); 'by_scenario' splits the episodes by component."""
     envs = list(env) if isinstance(env, (list, tuple)) else [env]
     if not envs:
@@ -252,6 +302,7 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     dev = envs[0].device
     ro = Rollout(H, N, envs[0].beam_mum, dev)
     comps = compose(envs, ro, noise, latency, dynamics, localization)
+    attach_planners(comps, planner, localization, planner_tables)
     col_mask = masked_agents(comps, non_cooperative, crowd)
     role = 'crowd' if crowd is not None else 'non_cooperative'
     col_comp = np.repeat(np.arange(len(comps)), [e.N for e in envs])     # component of every agent column
@@ -347,6 +398,8 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
         if col_mask is not None:
             ep_masked = col_mask[idx[:, 1]]
             stats[-1]['by_role'] = {'cooperative': _episode_stats(ep[~ep_masked]), role: _episode_stats(ep[ep_masked])}
+        if planner is not None:
+            stats[-1]['planner'] = _status_shares(comps)
         if diag is not None:
             stats[-1]['diagnostics'] = diag.metrics()
             if rank == 0:
