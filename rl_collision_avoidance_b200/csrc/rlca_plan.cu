@@ -411,7 +411,8 @@ __global__ void __launch_bounds__(WP_THREADS) rlca_plan_waypoints_kernel(
     if (a >= n) return;                                 // warp-uniform
     RowIn q;
     q.pose = pose[a];
-    q.goal = goal[a];
+    const float4 g = goal[a], in = gs_in[a];            // a waypoint replaces the local goal, never the speed
+    q.goal = make_float4(g.x, g.y, in.z, in.w);
     q.e = entry[a];
     q.r = q.e >= 0 ? rect[a] : make_int4(0, 0, -1, -1);
     q.f = field + (size_t)a * m.max_area;
@@ -419,7 +420,7 @@ __global__ void __launch_bounds__(WP_THREADS) rlca_plan_waypoints_kernel(
     int wx, wy;
     const int st = warp_row(m, q, lane, gs, wx, wy);
     if (lane == 0) {
-        gs_out[a] = st == 1 ? gs : gs_in[a];
+        gs_out[a] = st == 1 ? gs : in;
         status[a] = (uint8_t)st;
         status_count[3 * a + st] += 1;
     }
@@ -445,7 +446,9 @@ __global__ void __launch_bounds__(WP_THREADS) rlca_plan_shape_kernel(
     int wx, wy;                                         // written for status 1, the only status psi_excess reads
     const int st = warp_row(m, q, lane, gs, wx, wy);
     if (lane == 0) {
-        gs_out[a] = st == 1 ? gs : gs_in[a];
+        float4 out = gs_in[a];                          // a waypoint replaces the local goal, never the speed
+        if (st == 1) { out.x = gs.x; out.y = gs.y; }
+        gs_out[a] = out;
         status[a] = (uint8_t)st;
         status_count[3 * a + st] += 1;
         shape_row(sh, a, psi_excess(m, q, st, wx, wy));
@@ -471,7 +474,9 @@ static void host_rows(const PlanMap &m, int n, const rlca_plan_state *ps, const 
         float4 gs = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         int wx = 0, wy = 0;
         const int st = host_row(m, q, gs, wx, wy);
-        gs_out[a] = st == 1 ? gs : gs_in[a];
+        float4 out = gs_in[a];
+        if (st == 1) { out.x = gs.x; out.y = gs.y; }
+        gs_out[a] = out;
         ps->status[a] = (uint8_t)st;
         ps->status_count[3 * a + st] += 1;
         if (sh) shape_row(*sh, a, psi_excess(m, q, st, wx, wy));

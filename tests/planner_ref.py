@@ -1,5 +1,6 @@
 """An independent numpy / scipy restatement of the global planner (DESIGN.md §9w) for the CPU tests: traversable
-cells, goal entries, the geodesic field by scipy's Dijkstra, the robot entry, the descent chain, a float64 supercover
+cells, goal entries, the geodesic field by scipy's Dijkstra (one graph per field, or each component's graph built once:
+Graphs), the robot entry, the descent chain, a float64 supercover
 walk, the waypoint and the geodesic tracker."""
 import math
 
@@ -84,6 +85,52 @@ def field(label, rect, entry):
     ok = np.isfinite(d) & ins.ravel()
     out[ok] = d[ok].astype(np.uint32)
     return out.reshape(h, w)
+
+
+class Graphs:
+    """field's graph of every component of `label`, built once per component with numpy shifts over its bounding
+    rectangle (rects (K, 4): x0, y0, x1, y1 inclusive), so that each field is one dijkstra call; field(entry) equals
+    field(label, rects[comp], entry)."""
+
+    def __init__(self, label, rects):
+        self.label = label
+        self.rects = [tuple(int(v) for v in r) for r in rects]
+        self._graphs = {}
+
+    def graph(self, comp):
+        """(csr, (h, w) bool of the component's cells) over the rectangle of component comp"""
+        if comp not in self._graphs:
+            x0, y0, x1, y1 = self.rects[comp]
+            ins = self.label[y0:y1 + 1, x0:x1 + 1] == comp
+            h, w = ins.shape
+            idx = np.arange(h * w).reshape(h, w)
+            rows, cols, wts = [], [], []
+            for dx, dy in NB:
+                src = (slice(max(0, -dy), h - max(0, dy)), slice(max(0, -dx), w - max(0, dx)))
+                dst = (slice(max(0, dy), h + min(0, dy)), slice(max(0, dx), w + min(0, dx)))
+                ok = ins[src] & ins[dst]
+                diag = dx != 0 and dy != 0
+                if diag:
+                    ok &= ins[src[0], dst[1]] & ins[dst[0], src[1]]     # both orthogonal neighbours
+                rows.append(idx[src][ok])
+                cols.append(idx[dst][ok])
+                wts.append(np.full(int(ok.sum()), 99 if diag else 70))
+            g = coo_matrix((np.concatenate(wts), (np.concatenate(rows), np.concatenate(cols))),
+                           shape=(h * w, h * w)).tocsr()
+            self._graphs[comp] = (g, ins)
+        return self._graphs[comp]
+
+    def field(self, entry):
+        """(rect, (h, w) uint32 D over rect) of the goal entry (cx, cy)"""
+        comp = int(self.label[entry[1], entry[0]])
+        rect = self.rects[comp]
+        g, ins = self.graph(comp)
+        h, w = ins.shape
+        d = dijkstra(g, indices=(entry[1] - rect[1]) * w + entry[0] - rect[0])
+        out = np.full(h * w, INF, np.uint32)
+        ok = np.isfinite(d) & ins.ravel()
+        out[ok] = d[ok].astype(np.uint32)
+        return rect, out.reshape(h, w)
 
 
 def field_at(D, rect, x, y):

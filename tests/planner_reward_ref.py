@@ -9,12 +9,18 @@ import planner_ref as ref
 def psi(label, ocx, ocy, ppm, res, D, rect, entry_ok, pose, goal):
     """(status, psi) of one row in float64: 0 unless the row steers by a waypoint w (status 1), else the distance to w
     plus D(w's cell) res / 70, less the straight-line distance pose[3] the tick stored."""
-    s, wp, ch, k = ref.waypoint(label, ocx, ocy, ppm, res, D, rect, entry_ok, pose, goal)
+    w = ref.waypoint(label, ocx, ocy, ppm, res, D, rect, entry_ok, pose, goal)
+    return w[0], psi_of(w, res, D, rect, pose)
+
+
+def psi_of(w, res, D, rect, pose):
+    """psi of one row from its ref.waypoint result w = (status, waypoint, chain, chain index)"""
+    s, wp, ch, k = w
     if s != 1:
-        return s, 0.0
+        return 0.0
     x, y = ch[k]
     L = ref.field_at(D, rect, x, y) * res / 70.0
-    return s, math.hypot(wp[0] - float(pose[0]), wp[1] - float(pose[1])) + L - float(pose[3])
+    return math.hypot(wp[0] - float(pose[0]), wp[1] - float(pose[1])) + L - float(pose[3])
 
 
 def shaped_reward(reward, flags, psi_prev, psi_now, gain):

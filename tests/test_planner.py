@@ -153,6 +153,29 @@ def test_field_twin_equals_dijkstra(built, kind):
     assert (st.entry >= 0).any() and (st.entry == -1).any()
 
 
+@pytest.mark.parametrize('kind', ['stage1', 'stage2', 'spiral', 'comb', 'gaps'])
+def test_component_graphs_equal_per_field_dijkstra(kind):
+    """planner_ref.Graphs, each component's graph built once with numpy shifts, gives ref.field's D for entries in
+    every component (a few cells of the big components of the shipped maps, whose per-field graph takes a second)."""
+    m = make_scenario(kind).map if kind in ('stage1', 'stage2') else _synthetic(kind)
+    t = build_plan_tables(m)
+    graphs = ref.Graphs(t.label, t.rects)
+    rng = np.random.default_rng(len(kind))
+    area = (t.rects[:, 2] - t.rects[:, 0] + 1) * (t.rects[:, 3] - t.rects[:, 1] + 1)
+    checked = 0
+    for comp in np.argsort(-area):
+        ys, xs = np.nonzero(t.label == comp)
+        for i in rng.choice(len(xs), size=min(2, len(xs)), replace=False):
+            e = (int(xs[i]), int(ys[i]))
+            rect, D = graphs.field(e)
+            assert rect == tuple(t.rects[comp])
+            assert np.array_equal(D, ref.field(t.label, rect, e)), (comp, e)
+            checked += 1
+        if checked >= 6:
+            break
+    assert checked >= min(6, 2 * t.count)
+
+
 def test_only_changed_goal_entries_are_replanned(built):
     sc = make_scenario('stage1')
     t = build_plan_tables(sc.map)
@@ -301,6 +324,22 @@ def test_waypoint_properties(built):
         assert _bits_equal(out[st.status != 1], gs[st.status != 1])
     assert n1 > 0
     assert st.status_count.sum() == len(states) * cfg.robots_per_world * cfg.num_worlds
+
+
+def test_waypoint_keeps_the_speed_of_gs_in(built):
+    """A waypoint replaces the local goal only: where gs_in's speed is not the env's goal.zw (a robot parked by a
+    re-layout after the tick wrote its gs), every row keeps gs_in's speed."""
+    sc = _arena_sc(8, 4)
+    cfg, t, st, states = _waypoint_case(sc, 4, 5, 0, 3)
+    n1 = 0
+    for pose, goal, gs in states:
+        gs = gs.copy()
+        gs[:, 2:] = goal[:, 2:] + np.float32(0.25)
+        fields_host(cfg, t, st, goal)
+        out = waypoints_host(cfg, t, st, pose, goal, gs)
+        assert _bits_equal(out[:, 2:], gs[:, 2:])
+        n1 += int((st.status == 1).sum())
+    assert n1 > 0
 
 
 def test_convex_open_map_sees_every_clear_goal(built):

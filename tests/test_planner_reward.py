@@ -21,6 +21,18 @@ F = np.float32
 EPS = float(np.finfo(np.float32).eps)
 
 
+def psi_bound(psi, w):
+    """psi's bound against the float64 restatement: 8 ulp of |psi| + 2 |pose.w| + 1 (psi and the straight-line distance
+    pose.w it subtracts, float32)"""
+    return 8 * EPS * (abs(float(psi)) + 2.0 * abs(float(w)) + 1.0)
+
+
+def shaped_bound(reward, term):
+    """the shaped reward's bound against its float64 value from the same psi: 3 ulp of |reward| + |term|, term =
+    gain (psi_prev - psi)"""
+    return 3 * EPS * (abs(float(reward)) + abs(float(term)))
+
+
 def _cfg(sc, W=1, auto_reset=0, seed=0):
     return fill_config(_lib.EnvConfig(), sc, num_worlds=W, beams=512, auto_reset=auto_reset, seed=seed)
 
@@ -101,8 +113,7 @@ def test_shape_twin_matches_float64_restatement(built, name, W, ticks):
             if s_ref != hs.status[a]:
                 counts['skipped'] += 1
             else:
-                mag = abs(float(pp[a])) + 2.0 * abs(float(orc.pose[a, 3])) + 1.0
-                if abs(float(pp[a]) - psi_ref) > 8 * EPS * mag:
+                if abs(float(pp[a]) - psi_ref) > psi_bound(pp[a], orc.pose[a, 3]):
                     counts['skipped'] += 1          # another waypoint on the chain (a corner case of the walk)
                 else:
                     counts['psi'] += 1
@@ -114,7 +125,7 @@ def test_shape_twin_matches_float64_restatement(built, name, W, ticks):
             fl = flags[a]
             if fl[0] == 0:
                 want = rref.shaped_reward(orc.reward[a], fl, pp_before[a], pp[a], gain)
-                tol = 3 * EPS * (abs(float(orc.reward[a])) + abs(gain * (float(pp_before[a]) - float(pp[a]))))
+                tol = shaped_bound(orc.reward[a], gain * (float(pp_before[a]) - float(pp[a])))
                 assert abs(float(reward[a]) - want) <= tol, (a, reward[a], want)
                 counts['shaped'] += 1
                 if st_before[a] == 0 and hs.status[a] == 0:

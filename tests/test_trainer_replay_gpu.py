@@ -2,19 +2,30 @@
 trainer imports and of the optimizer instance, then every update replayed against independent references.
 
 a. The environment, bit for bit: one CPU oracle per component, driven by the executed commands, with the scan deque of
-   tests/trainer_ref.py, the re-layout host twin (random layouts) and the noise host twins.  Stacks, goal | speed,
-   rewards, flags and the eplog rows of ended episodes equal the device rollout's.  The perturbation chain is restated
+   tests/trainer_ref.py, the layout and re-layout host twins (random layouts; arenas with the layout's own pick) and
+   the noise host twins.  Stacks, goal | speed, rewards, flags and the eplog rows of ended episodes equal the device
+   rollout's.  The perturbation chain is restated
    per component and tick: the executed command is the sampled one with the masked rows overridden (the crowd and
    straight-driver host twins on the oracle's state, themselves within their float64 restatements' bounds), then
    latency_ref's command ring, the noise twin and dynamics_ref's limits, the last two links with the flags of the tick
    before; it equals what the env's control_vel received, bit for bit.  The stack is the deque after the re-layout
    refresh, then latency_ref's scan ring and the noise twin; the gs the policy reads is localization_ref's believed gs
    on the oracle's pose and goal after the re-layout.
-b. The policy per tick, at the weights of the update's start: values against the float64 forward within
+   With a planner, restated from tests/planner_ref.py alone (PlanReplay), last of all: after the run's start and
+   every tick each row whose goal entry changed is re-planned by scipy's Dijkstra, and the device's status equals
+   ref.waypoint's on the oracle's pose and goal; the gs the policy reads is the tick's bit for bit where the goal is in
+   sight or there is no plan, and the waypoint's local goal within 1e-4 (its speed bit for bit) elsewhere
+   (test_waypoint_twin_matches_float64_restatement).  Rows where a tested segment passes within 1e-5 m of a cell
+   corner are exempt, at most one in 1000, and carry the device's gs.  With 'geodesic' the device's psi is within
+   test_planner_reward's bound of planner_reward_ref.psi, a non-terminal tick's reward within its bound of
+   shaped_reward on the tick's reward and the device's psi before and after it, a terminal tick's reward is the tick's
+   bit for bit, and an ended episode's return lies within float32 rounding of the float64 sum of the rewards PPO
+   trained on (psi_start restarting on flags[:, 3] and at the run's start); its other eplog columns stay bit for bit.
+   With 'straight' rewards and eplog stay the tick's., at the weights of the update's start: values against the float64 forward within
    learner_ref.check_forward's bound for the tensor-core mode, means within the bound at _forward64; actions,
    log-probabilities and the clip against sample_ref (test_sample_gpu's bounds); the stored action is the sampled,
    un-noised one; last_v is the float64 value of the replayed state after the horizon.
-c. The update: GAE targets and advantages against the float64 recurrence on the replayed rewards and dones (1 float32
+c. The update: GAE targets and advantages against the float64 recurrence on the rewards checked in a and dones (1 float32
    ulp, test_learner_shapes_gpu.test_gae_vs_float64_recurrence); filter_index exactly; the epochs' permutations drawn
    again from the generator state at entry give the restated minibatch schedule (a ragged last minibatch in stage 1,
    the tail dropped in stage 2) over the rows the restated filter keeps (stage 2: get_filter_index united with every
@@ -24,7 +35,9 @@ c. The update: GAE targets and advantages against the float64 recurrence on the 
    Adam step against trainer_ref.adam_step in float64 from the device's gradient (bounds at step_checks and
    adam_bounds).  Every replayed PPO ratio is asserted to be learner_ref.MARGIN away from 1 +- clip.
 d. The Env log lines against the replay's own episode bookkeeping, and the stats run returns (episodes, success rate,
-   mean episode reward, by_scenario and, with masked agents, by_role) against the replay's eplog rows of ended episodes.
+   mean episode reward, by_scenario and, with masked agents, by_role) against the eplog rows of ended episodes checked
+   in a; with a planner the returns in the lines within a's bound of the float64 sums, and the status shares against
+   the replay's statuses over the update's robot-ticks (update 0's with the start's rows).
 
 Real rollouts are not decisive batches (learner_ref): a pre-activation within fp32 rounding of zero can flip its ReLU
 mask between the kernels and float64, which moves that tower's gradients by ~1e-3 of their scale.  A tower's tensors are
@@ -49,10 +62,13 @@ import dynamics_ref
 import latency_ref
 import localization_ref
 import orca_ref
+import planner_ref
+import planner_reward_ref as rref
 import sample_ref
 import trainer_ref as ref
 from learner_ref import (CLIP, COEFF, MARGIN, VCOEF, Checks, layer_scale, maxabs, ref_forward, ref_logprob, ref_losses)
 from test_crowd import TOL as CROWD_TOL
+from test_planner_reward import psi_bound, shaped_bound
 from test_sample_gpu import action_bound, lp_bound
 
 pytestmark = pytest.mark.gpu
@@ -72,10 +88,24 @@ CHAIN_SEED = 1            # the chain's localization seed: with LOCALIZATION's, 
 NONCOOP_TOL = 1e-5       # the straight driver's twin against orca_ref's preferred velocity and tracker (test_noncoop)
 MIX = [('stage2', 1, 2, 25, {}), ('circle', 2, 2, 100, dict(robots_per_world=8, radius=1.5)),
        ('random', 4, 0, 60, dict(robots_per_world=8, side=6.0))]
+# 8 worlds of 8 robots in 16 obstacle arenas of generator seed 2, an arena drawn at every layout (pick 1, as training
+# draws them); with a 25-tick time-out every world is re-laid on ticks 25, 51 = H - 1, 77 and 103
+ARENA = ('arena', 8, 0, 25, dict(robots_per_world=8, arenas=16, pick=1, arena_seed=2))
 
-# (scenario, worlds, auto_reset, timeout, extra make_scenario arguments) per component; the perturbations are the
+
+def _stage1_pillar():
+    """stage 1's map with a 2 m square pillar at its centre: stage 1's room is convex, so only goals behind the
+    pillar are out of sight"""
+    from rl_collision_avoidance_b200.scenarios import make_scenario
+    m = make_scenario('stage1').map
+    c = m.cells.copy()
+    k = int(round(1.0 / m.resolution))
+    c[m.origin_cy - k:m.origin_cy + k, m.origin_cx - k:m.origin_cx + k] = 254
+    return dataclasses.replace(m, cells=c, name='stage1 with a pillar')
+
+# (scenario, worlds, auto_reset, timeout, extra make_scenario arguments, a callable one called) per component; the perturbations are the
 # keyword arguments of latency.LatencyParams, dynamics.DynamicsParams and localization.LocalizationParams, 'crowd' the
-# k of crowd=(k, CrowdParams(), True) and 'non_cooperative' the (k, speed) of trainer.run
+# k of crowd=(k, CrowdParams(), True), 'non_cooperative' the (k, speed) and 'planner' the planner of trainer.run
 CASES = {
     # 2 x 24 robots; episodes time out after 20 ticks, so the first ones end on tick 19 and 39 = the horizon's last;
     # H N = 1920 is 7.5 minibatches of 256: a ragged last minibatch
@@ -104,13 +134,27 @@ CASES = {
     # the mix with every link of the chain on and a crowd that sees the map
     'chain': dict(stage=2, comps=MIX, H=52, batch=256, ckpt='stage2.pth', noise=True, latency=LATENCY,
                   dynamics=DYNAMICS, localization=dict(LOCALIZATION, seed=CHAIN_SEED), crowd=2),
+    # arena worlds re-laid inside the horizon and across it; robots parked until their world's last episode ends
+    'arena': dict(stage=2, comps=[ARENA], H=52, batch=128, ckpt='stage2.pth', noise=False),
+    # stage 1's shape on its map with a pillar, steered and rewarded by the geodesic planner: every re-spawn re-plans, episodes end on tick
+    # 39 = H - 1 and others straddle the boundary, their returns corrected in update 2
+    'planner_stage1': dict(stage=1, comps=[('stage1', 2, 1, 19, dict(map_=_stage1_pillar))], H=40, batch=256,
+                           ckpt='stage1_2.pth', noise=False, planner='geodesic'),
+    # the arena case steered by waypoints, with the tick's own rewards
+    'planner_straight': dict(stage=2, comps=[ARENA], H=52, batch=128, ckpt='stage2.pth', noise=False,
+                             planner='straight'),
+    # stage 2 | arena with every link of the chain the planner accepts (localization error it refuses), the planner
+    # last; a 28-tick arena time-out, so that arena episodes straddle the boundary
+    'planner_chain': dict(stage=2, comps=[('stage2', 1, 2, 25, {}), ARENA[:3] + (28,) + ARENA[4:]], H=52, batch=256,
+                          ckpt='stage2.pth', noise=True, latency=LATENCY, dynamics=DYNAMICS, crowd=2,
+                          planner='geodesic'),
 }
 SEED = 3
 
 
 def _scenario(name, timeout, extra):
     from rl_collision_avoidance_b200.scenarios import make_scenario
-    sc = make_scenario(name, **extra)
+    sc = make_scenario(name, **{k: v() if callable(v) else v for k, v in extra.items()})
     return dataclasses.replace(sc, timeout=timeout)
 
 
@@ -134,10 +178,13 @@ class Recorder:
         from rl_collision_avoidance_b200 import trainer
         from rl_collision_avoidance_b200.crowd import Crowd
         from rl_collision_avoidance_b200.orca import NonCooperative
+        from rl_collision_avoidance_b200.planner import Planner
         self.policy, self.opt, self.gen = policy, optimizer, generator
         self.ticks, self.fv, self.noise_cmds, self.gtd, self.updates = [], [], [], [], []
         self.executed = [[] for _ in envs]          # per component and tick: the command control_vel received
         self.overrides = [[] for _ in envs]         # per component and tick: the action after the masked override
+        self.plans = [[] for _ in envs]             # per component, the start's then each tick's Planner.update: the
+                                                    # status and psi_prev (psi) it left
         self.ro = self.comps = self.stats = None
         rec = self
 
@@ -164,6 +211,15 @@ class Recorder:
                 rec.overrides[index(self_.env)].append(out.clone())
                 return out
             monkeypatch.setattr(cls, 'apply', apply)
+
+        up0 = Planner.update
+
+        def update(self_, flags=None, reward=None, eplog=None, gs=None):
+            out = up0(self_, flags, reward, eplog, gs)
+            rec.plans[index(self_.env)].append(dict(status=self_.status().clone(),
+                                                    psi=None if self_.psi_prev is None else self_.psi_prev.clone()))
+            return out
+        monkeypatch.setattr(Planner, 'update', update)
 
         fv0 = policy.forward_values
 
@@ -231,8 +287,8 @@ class Recorder:
 
 
 def _perturbations(c):
-    """The perturbation settings of case c: noise, latency, dynamics and localization params (or None) and the
-    masked agents ('crowd', k, CrowdParams) / ('non_cooperative', k, speed) (or None)."""
+    """The perturbation settings of case c: noise, latency, dynamics and localization params (or None), the masked
+    agents ('crowd', k, CrowdParams) / ('non_cooperative', k, speed) (or None) and the planner (or None)."""
     from rl_collision_avoidance_b200.crowd import CrowdParams
     from rl_collision_avoidance_b200.dynamics import DynamicsParams
     from rl_collision_avoidance_b200.latency import LatencyParams
@@ -247,7 +303,7 @@ def _perturbations(c):
                 latency=LatencyParams(**c['latency']) if 'latency' in c else None,
                 dynamics=DynamicsParams(**c['dynamics']) if 'dynamics' in c else None,
                 localization=LocalizationParams(**c['localization']) if 'localization' in c else None,
-                masked=masked)
+                masked=masked, planner=c.get('planner'))
 
 
 def _train(case, monkeypatch):
@@ -282,7 +338,8 @@ def _train(case, monkeypatch):
                         stage=c['stage'], max_updates=2, generator=gen, noise=pt['noise'], latency=pt['latency'],
                         dynamics=pt['dynamics'], localization=pt['localization'],
                         non_cooperative=masked[1:] if masked and masked[0] == 'non_cooperative' else None,
-                        crowd=(masked[1], masked[2], True) if masked and masked[0] == 'crowd' else None)
+                        crowd=(masked[1], masked[2], True) if masked and masked[0] == 'crowd' else None,
+                        planner=pt['planner'])
     finally:
         lg.removeHandler(hl)
         lc.removeHandler(hc)
@@ -291,25 +348,120 @@ def _train(case, monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ a. environment
+class PlanReplay:
+    """The planner of one component restated from planner_ref alone: build_plan_tables' graph, each row's goal entry
+    (ref.goal_entry) re-planned by scipy's Dijkstra when it changes (ref.Graphs), the row's status and waypoint
+    (ref.waypoint) and psi (planner_reward_ref) on the oracle's pose and goal, then with 'geodesic' the shaped reward
+    and the episodes' shaping.  `plans` are the device's records of the component (Recorder.plans): the status and psi
+    each Planner.update left, the start's first."""
+
+    def __init__(self, kind, sc, cfg, plans, n):
+        from rl_collision_avoidance_b200.planner import build_plan_tables
+        t = build_plan_tables(sc.map)
+        self.kind, self.m, self.label, self.graphs = kind, sc.map, t.label, planner_ref.Graphs(t.label, t.rects)
+        self.ppm, self.res, self.gain = (float(np.float32(x)) for x in (cfg.ppm, cfg.resolution, cfg.progress_gain))
+        self.plans = plans
+        self.entry = [False] * n                     # the goal entry each row's field was planned for (None: no entry)
+        self.field = [None] * n                      # (rect, D) of the row's field
+        self.count = np.zeros(3, np.int64)           # the rows of each status since the update's stats were checked
+        self.exempt = np.zeros(n, bool)              # rows whose waypoint the float64 walk may place elsewhere
+        self.psi_prev = self.psi_start = None        # the device's psi after the last update / at the episode's start
+
+    def update(self, i, pose, goal, gs_in, gs_dev, what, ev):
+        """Planner.update number i (0: the run's start, g + 1: tick g) on the state the tick and any re-layout left:
+        re-plan, then each row's status against the device's, its gs (gs_dev, what the policy read) against the
+        waypoint's and psi against the float64 one.  Returns the gs the replay carries: the tick's where the goal is in
+        sight or there is no plan, the device's checked waypoint gs elsewhere and on exempt rows."""
+        m, ppm = self.m, self.ppm
+        dev = self.plans[i]
+        status, psi = _np(dev['status']), None if dev['psi'] is None else _np(dev['psi'])
+        self.exempt[:] = False
+        for a in range(len(pose)):
+            e = planner_ref.goal_entry(self.label, m.origin_cx, m.origin_cy, ppm, goal[a, 0], goal[a, 1])
+            if e != self.entry[a]:
+                self.entry[a] = e
+                self.field[a] = None if e is None else self.graphs.field(e)
+                ev['replanned'] += int(e is not None)
+            rect, D = self.field[a] or (None, None)
+            w = planner_ref.waypoint(self.label, m.origin_cx, m.origin_cy, ppm, self.res, D, rect, e is not None,
+                                     pose[a], goal[a])
+            s = int(status[a])
+            if s != 1:
+                assert _bits_equal(gs_dev[a], gs_in[a]), f'{what} row {a}: status {s} and another gs than the tick\'s'
+            ok = s == w[0]
+            if ok and s == 1:
+                dx, dy = w[1][0] - float(pose[a, 0]), w[1][1] - float(pose[a, 1])
+                c, sn = math.cos(float(pose[a, 2])), math.sin(float(pose[a, 2]))
+                ok = abs(dx * c + dy * sn - gs_dev[a, 0]) < 1e-4 and abs(dy * c - dx * sn - gs_dev[a, 1]) < 1e-4
+                assert _bits_equal(gs_dev[a, 2:], gs_in[a, 2:]), f'{what} row {a}: the waypoint gs\'s speed'
+            if not ok:
+                # allowed only where a tested segment passes within 1e-5 m of a cell corner (test_planner)
+                u, v = float(pose[a, 0]) * ppm, float(pose[a, 1]) * ppm
+                near = planner_ref.corner_dist(u, v, float(goal[a, 0]) * ppm, float(goal[a, 1]) * ppm) < 1e-5 * ppm
+                for (x, y) in (w[2] or []):
+                    near |= planner_ref.corner_dist(u, v, x - m.origin_cx + 0.5, y - m.origin_cy + 0.5) < 1e-5 * ppm
+                assert near, f'{what} row {a}: status {s}, waypoint gs {gs_dev[a]}; float64 status {w[0]} at {w[1]}'
+                self.exempt[a] = True
+            elif psi is not None:
+                want = rref.psi_of(w, self.res, D, rect, pose[a])
+                assert abs(float(psi[a]) - want) <= psi_bound(psi[a], pose[a, 3]), \
+                    f'{what} row {a}: psi {psi[a]!r}, float64 {want!r}'
+                ev['psi_checked'] += 1
+            self.count[s] += 1
+            ev[f'status_{s}'] += 1
+        ev['plan_rows'] += len(pose)
+        ev['exempt'] += int(self.exempt.sum())
+        if i == 0 and psi is not None:
+            self.psi_prev, self.psi_start = psi, psi.copy()       # every row starts an episode
+        return np.where((status == 1)[:, None], gs_dev, gs_in)
+
+    def shape(self, i, flags, reward, reward_dev, what, ev):
+        """With 'geodesic', after update(i): the device's reward against the tick's plus gain (psi_prev - psi) on a
+        non-terminal tick (rref.shaped_reward, test_planner_reward's bound, from the device's psi checked in update) and
+        the tick's bit for bit on a terminal one.  Returns the device's rewards, their float64 values and, per row, the
+        shaping gain (psi_start - psi_prev) the return of an episode the tick ended gets; then psi_prev = psi and
+        psi_start restarts where flags[:, 3] is set."""
+        psi = _np(self.plans[i]['psi'])
+        r64 = reward.astype(np.float64)
+        for a in range(len(reward)):
+            if flags[a, 0] != 0:
+                assert _bits_equal(reward_dev[a], reward[a]), f'{what} row {a}: terminal reward {reward_dev[a]!r} ' \
+                                                              f'is not the tick\'s {reward[a]!r}'
+                continue
+            r64[a] = rref.shaped_reward(reward[a], flags[a], self.psi_prev[a], psi[a], self.gain)
+            term = self.gain * (float(self.psi_prev[a]) - float(psi[a]))
+            assert abs(float(reward_dev[a]) - r64[a]) <= shaped_bound(reward[a], term), \
+                f'{what} row {a}: shaped reward {reward_dev[a]!r}, float64 {r64[a]!r}'
+            ev['shaped_changed'] += int(reward_dev[a] != reward[a])
+        corr = self.gain * (self.psi_start.astype(np.float64) - self.psi_prev.astype(np.float64))
+        self.psi_prev = psi
+        restart = flags[:, 3] != 0
+        self.psi_start[restart] = psi[restart]
+        return reward_dev.copy(), r64, corr
+
+
 class OracleComponent:
     """The CPU oracle of one component, the restated scan deque and the episode bookkeeping of its robots."""
 
-    def __init__(self, k, comp, sc, W, ar, pt):
+    def __init__(self, k, comp, sc, W, ar, pt, plans):
         from oracle.oracle import OracleWorld, OrcConfig
         from rl_collision_avoidance_b200.noise import scan_host
         from rl_collision_avoidance_b200.orca import ObstacleSet
-        from rl_collision_avoidance_b200.scenarios import fill_config, random_layout_host
+        from rl_collision_avoidance_b200.scenarios import ArenaLayout, arena_layout_host, fill_config, \
+            random_layout_host
         self.k, self.c, self.sc, self.noise = k, comp, sc, pt['noise']
         self.cfg = cfg = comp.env.cfg                # the product's config struct, for the host twins
         ocfg = fill_config(OrcConfig(), sc, num_worlds=W, beams=512, auto_reset=ar, seed=SEED)
         o = self.o = OracleWorld(ocfg, sc.map.cells, sc.init_tab, sc.goal_tab)
         self.relayout = sc.layout is not None
+        self.arena = isinstance(sc.layout, ArenaLayout)
         o.reset_world()
         o.reset_pose()
         o.generate_goal_point()
         if self.relayout:
-            o.pose[...], o.goal[...], o.acc[...], status = random_layout_host(self.cfg, sc.layout, o.pose, o.goal,
-                                                                              o.acc)
+            # the first layout: the random one, or the arena layout with the layout's own pick
+            first = arena_layout_host if self.arena else random_layout_host
+            o.pose[...], o.goal[...], o.acc[...], status = first(self.cfg, sc.layout, o.pose, o.goal, o.acc)
             assert not status.any()
             o.observe()
         n = o.N
@@ -355,6 +507,14 @@ class OracleComponent:
         self.init = o.pose[:, 0:2].copy()
         self.idle = np.zeros(n, bool)                 # stage 2's liveflag false / a parked random robot
         self.last_r = np.zeros(n, np.float32)
+        self.ep_sabs = np.zeros(n)                    # sum of |shaped reward| in float64, for the float64 sum's rounding
+        self.ep_update = np.zeros(n, np.int64)        # the update an episode started in
+        self.plan = None if pt['planner'] is None else PlanReplay(pt['planner'], sc, cfg, plans, n)
+
+    def start_plan(self, gs_dev, ev):
+        """The planner's update at the run's start, against slot 0 of update 0 (gs_dev)."""
+        if self.plan is not None:
+            self.gs = self.plan.update(0, self.o.pose, self.o.goal, self.gs, gs_dev, f'start {self.c.name}', ev)
 
     def state(self):
         return self.stacks.array(), self.gs.copy()
@@ -427,10 +587,12 @@ class OracleComponent:
             assert np.abs(act[a] - want).max() <= tol, (self.c.name, a, act[a], want)
             ev['masked_checked'] += 1
 
-    def tick(self, cmd, g, ev):
-        """one tick at global tick g: reward, flags, eplog, the rows that were idle on it and those that ended"""
+    def tick(self, cmd, g, ev, dev):
+        """one tick at global tick g of update dev['u']: reward, flags, eplog, the rows that were idle on it and those
+        that ended.  dev holds the device's gs, reward and eplog of the tick: with a planner the replay checks them and
+        carries the device's where it may not restate them bit for bit."""
         from rl_collision_avoidance_b200.noise import scan_host
-        from rl_collision_avoidance_b200.scenarios import relayout_host
+        from rl_collision_avoidance_b200.scenarios import arena_relayout_host, relayout_host
         o = self.o
         idle = self.idle | (self.live == 0)
         o.step(cmd, live=self.live if self.relayout else None)
@@ -440,7 +602,8 @@ class OracleComponent:
         restart = flags[:, 3] != 0
         self.stacks.tick(obs, restart)
         if self.relayout:
-            o.pose[...], o.goal[...], o.acc[...], o.meta[...], flags, self.live, status = relayout_host(
+            relay = arena_relayout_host if self.arena else relayout_host
+            o.pose[...], o.goal[...], o.acc[...], o.meta[...], flags, self.live, status = relay(
                 self.cfg, self.sc.layout, o.pose, o.goal, o.acc, o.meta, flags)
             assert not status.any()
             o.observe()
@@ -471,22 +634,48 @@ class OracleComponent:
             self.believed = (believed != gs).any(1)
             ev['believed'] += int(self.believed.sum())
             gs = believed
+        # the planner last, on the state and flags the re-layout left
+        tick_reward, r64, corr = reward, reward.astype(np.float64), None
+        what = f'update {dev["u"]} tick {g} {self.c.name}'
+        if self.plan is not None:
+            gs = self.plan.update(g + 1, o.pose, o.goal, gs, dev['gs'], what, ev)
+            if self.plan.kind == 'geodesic':
+                reward, r64, corr = self.plan.shape(g + 1, flags, reward, dev['reward'], what, ev)
         self.gs = gs
         self.prev = flags
         # bookkeeping
         lines = []
         live_now = ~idle
         self.steps[live_now] += 1
-        self.ep_reward[live_now] += reward[live_now].astype(np.float64)
-        self.ep_abs[live_now] += np.abs(reward[live_now].astype(np.float64))
+        self.ep_reward[live_now] += r64[live_now]
+        self.ep_abs[live_now] += np.abs(tick_reward[live_now].astype(np.float64))
+        self.ep_sabs[live_now] += np.abs(r64[live_now])
         for i in np.nonzero(ended)[0]:
-            lines.append((i, self.episode[i], self.steps[i], self.ep_reward[i], self.ep_abs[i], self.goal[i].copy(),
+            # the tick's return is a float32 running sum of `steps` terms: within steps u sum |r| of the float64 sum
+            tol = self.steps[i] * U * self.ep_abs[i]
+            if corr is not None:
+                # the planner adds c = gain (psi_start - psi_prev) to it: E = fl(R + fl(gain fl(psi_start - psi_prev)))
+                # with R the tick's return.  The two inner roundings put fl(...) within (2u + u^2) |c| of c, the
+                # addition E within u |E| (1 + u) of R + fl(...); the float64 sum of the shaped rewards is R's float64
+                # sum plus c (the shaping terms of the non-terminal ticks telescope to c), up to its own rounding, <=
+                # steps 2^-52 sum |shaped reward|
+                E, c = float(dev['eplog'][i, 2]), float(corr[i])
+                tol += (2 * U + U * U) * abs(c) + U * (1 + U) * abs(E) + self.steps[i] * 2.0 ** -52 * self.ep_sabs[i]
+                assert _bits_equal(np.delete(dev['eplog'][i], 2), np.delete(eplog[i], 2)), \
+                    f'{what} row {i}: eplog columns but the return'
+                assert abs(E - self.ep_reward[i]) <= tol + 1e-30, \
+                    f'{what} row {i}: return {E!r}, float64 sum of the shaped rewards {self.ep_reward[i]!r}, bound {tol}'
+                eplog[i, 2] = dev['eplog'][i, 2]
+                ev['corrected'] += int(c != 0)
+                ev['straddled'] += int(dev['u'] == 1 and self.ep_update[i] == 0)
+            lines.append((i, self.episode[i], self.steps[i], self.ep_reward[i], tol, self.goal[i].copy(),
                           self.init[i].copy(), int(flags[i, 2])))
         self.idle = (self.idle | ended) & ~restart
         for i in np.nonzero(restart)[0]:
             self.episode[i] += 1
             self.steps[i] = 0
-            self.ep_reward[i] = self.ep_abs[i] = 0.0
+            self.ep_reward[i] = self.ep_abs[i] = self.ep_sabs[i] = 0.0
+            self.ep_update[i] = dev['u'] if g % dev['H'] != dev['H'] - 1 else dev['u'] + 1
             self.goal[i] = o.goal[i, 0:2]
             self.init[i] = o.pose[i, 0:2]
         out = dict(reward=reward, flags=flags, eplog=eplog, idle=idle, ended=ended, lines=lines,
@@ -703,7 +892,9 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
     assert len(rec.updates) == 2 and len(rec.gtd) == 2 and len(rec.ticks) == 2 * H and len(rec.stats) == 2
     assert all(len(x) == 2 * H for x in rec.executed)
     assert all(len(x) == (2 * H if pt['masked'] else 0) for x in rec.overrides)
-    oc = [OracleComponent(k, comp, sc, W, ar, pt) for k, (comp, (sc, W, ar)) in enumerate(zip(comps, scs))]
+    assert all(len(x) == (2 * H + 1 if pt['planner'] else 0) for x in rec.plans)
+    oc = [OracleComponent(k, comp, sc, W, ar, pt, rec.plans[k])
+          for k, (comp, (sc, W, ar)) in enumerate(zip(comps, scs))]
     col_mask = np.concatenate([o.mask for o in oc]) != 0
     col_comp = np.concatenate([np.full(o.o.N, k) for k, o in enumerate(oc)])
     check = Checks()
@@ -711,6 +902,8 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
     for key in ('ended', 'ended_last_tick', 'idle', 'respawn', 'relaid', 'filtered', 'boundary_runs', 'noised_rows',
                 'steps', 'clipped', 'undecided_conv', 'undecided_fc', 'worst_mean_factor', 'worst_value_factor'):
         ev[key] = 0
+    for o in oc:
+        o.start_plan(rec.updates[0]['snap']['gs'][0, o.c.a:o.c.b], ev)
     expected_lines = []
     for u, up in enumerate(rec.updates):
         snap = up['snap']
@@ -736,7 +929,9 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
                 if u == 1 and t == 0 and o.lat is not None and o.lat.cr[1] > 0:
                     # rows whose episode ended on update 1's last tick restart their command rings here
                     ev['ring_restart_on_boundary'] += int((o.prev[:, 3] != 0).sum())
-                r = o.tick(o.command(scaled[a:b], g, rec, ev), g, ev)
+                dev = dict(u=u, H=H, gs=snap['gs'][t + 1, a:b], reward=snap['rewards'][t, a:b],
+                           eplog=snap['eplog'][t, a:b])
+                r = o.tick(o.command(scaled[a:b], g, rec, ev), g, ev, dev)
                 s, gsn = o.state()
                 what = f'update {u} tick {t} {o.c.name}'
                 assert _bits_equal(snap['stacks'][t + 1, a:b], s), f'{what}: stack'
@@ -758,8 +953,8 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
                 ev['respawn' if not o.relayout else 'relaid'] += int((r['flags'][:, 3] != 0).sum())
                 dones[t, a:b] = r['flags'][:, 0] != 0
                 rewards[t, a:b] = r['reward']
-                for (i, epi, steps, rsum, rabs, goal, init, res) in r['lines']:
-                    upd_lines.append((t, a + i, o, i, epi, steps, rsum, rabs, goal, init, res))
+                for (i, epi, steps, rsum, tol, goal, init, res) in r['lines']:
+                    upd_lines.append((t, a + i, o, i, epi, steps, rsum, tol, goal, init, res))
         # ---- b. the policy per tick, at the weights of the update's start
         P = _params64(policy, up['flat'])
         logstd = _np(up['flat'][policy.offsets[0]:policy.offsets[0] + 2])
@@ -792,7 +987,7 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
         lv64, _, _ = _forward64(P, torch.from_numpy(sH).cuda(), torch.from_numpy(gH).cuda())
         check(f'update {u} last_v', maxabs(torch.from_numpy(gt['last_value']).cuda().double() - lv64),
               2e-5 * max(1.0, maxabs(lv64)))
-        # ---- c. the update
+        # ---- c. the update, on the device's rewards checked in a
         assert _bits_equal(gt['rewards'], rewards), f'update {u}: GAE rewards'
         assert _bits_equal(gt['values'], snap['values']), f'update {u}: GAE values'
         assert np.array_equal(gt['dones'] != 0, dones), f'update {u}: GAE dones are not flag 0 (done)'
@@ -858,12 +1053,25 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
             assert _same(s['by_role'], want), f'update {u}: by_role {s["by_role"]} != {want}'
             ev['episodes_cooperative'] += int((~m).sum())
             ev['episodes_masked'] += int(m.sum())
+        # the planner's status shares over the update's robot-ticks (update 0's with the start's rows), in the replay's
+        # statuses
+        if pt['planner'] is None:
+            assert 'planner' not in s
+        else:
+            tot = sum(o.plan.count for o in oc)
+            n = int(tot.sum())
+            want = {k: int(v) / n for k, v in zip(('goal_visible', 'waypoint', 'no_plan'), tot)}
+            want['robot_ticks'] = n
+            assert n == (H + (u == 0)) * N and _same(s['planner'], want), \
+                f'update {u}: planner {s["planner"]} != {want}'
+            for o in oc:
+                o.plan.count[:] = 0
     # ---- d. log lines against the bookkeeping
     from rl_collision_avoidance_b200.stage_world import RESULT_STRINGS
     env_lines = [l for l in lines if isinstance(l, str) and l.startswith('Env ')]
     assert len(env_lines) == len(expected_lines) == len(cal), (len(env_lines), len(expected_lines), len(cal))
     mixed = len(oc) > 1
-    for line, calv, (t, col, o, i, epi, steps, rsum, rabs, goal, init, res) in zip(env_lines, cal, expected_lines):
+    for line, calv, (t, col, o, i, epi, steps, rsum, tol, goal, init, res) in zip(env_lines, cal, expected_lines):
         robot = i % o.c.env.num_env
         head = 'Env %02d, Goal (%05.1f, %05.1f), Episode %05d, setp %03d, Reward ' % (
             robot, goal[0], goal[1], epi + 1 if stage == 1 else epi, steps + 1 if stage == 1 else steps)
@@ -877,22 +1085,23 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
             assert rest[1:] == [RESULT_STRINGS[res], o.c.name], line
         else:
             assert rest[1:] == [RESULT_STRINGS[res] + ','], line
-        # float32 running sum of `steps` terms: <= steps u sum |r| from the float64 sum
-        tol = steps * U * rabs
+        # the float32 return against the float64 sum of the rewards PPO trained on, within OracleComponent.tick's bound
         assert abs(float(calv) - rsum) <= tol + 1e-30, (line, float(calv), rsum, tol)
         assert abs(got_r - rsum) <= 0.05 + tol + 1e-9, (line, rsum)
     check.done()
     # ---- the events each case exists for
     print(f'[events] {case}: {dict(ev)}, train {t_train:.1f} s, total {time.perf_counter() - t_start:.1f} s')
     assert ev['ended'] > 0 and len(env_lines) > 0 and ev['steps'] > 0
-    if case in ('stage1', 'noise', 'latency'):
+    if case in ('stage1', 'noise', 'latency', 'planner_stage1'):
         assert ev['ended_last_tick'] > 0 and ev['respawn'] > 0
     if noise is not None:
         assert ev['noised_rows'] > 0
     if case in ('stage2', 'mix', 'dynamics'):
         assert ev['filtered'] > 0 and ev['idle'] > 0 and ev['respawn'] > 0
-    if case in ('random', 'mix', 'localization'):
+    if case in ('random', 'mix', 'localization', 'planner_straight'):
         assert ev['relaid'] > 0
+    if case in ('arena', 'planner_chain'):
+        assert ev['relaid'] > 0 and ev['idle'] > 0 and ev['filtered'] > 0
     if case == 'mix':
         assert ev['boundary_runs'] > 0, 'no filter run crossed a component boundary'
     if case == 'latency':
@@ -914,3 +1123,14 @@ def test_trainer_replays_against_the_reference_loop(built, monkeypatch, case):
             assert ev[link] > 0, f'{link}: this link changed no row'
         assert ev['masked_checked'] > 0 and ev['episodes_masked'] > 0
         assert ev['masked_boundary_rows'] > 0, 'no masked row in a filter run crossing a component boundary'
+    if pt['planner'] is not None:
+        assert ev['replanned'] > 0 and ev['status_0'] > 0 and ev['status_1'] > 0, 'no re-plan, or a status unseen'
+        assert ev['exempt'] <= max(1, ev['plan_rows'] // 1000), 'too many rows whose waypoint the walks disagree on'
+    if pt['planner'] == 'geodesic':
+        assert ev['shaped_changed'] > 0, 'no shaped reward differed from the tick\'s'
+        assert ev['corrected'] > 0, 'no ended episode had its return corrected'
+        assert ev['straddled'] > 0, 'no episode straddled the update boundary'
+    if case == 'planner_chain':
+        for link in ('masked_changed', 'command_delayed', 'noised_rows', 'limited', 'scan_delayed', 'noised_scans'):
+            assert ev[link] > 0, f'{link}: this link changed no row'
+        assert ev['masked_checked'] > 0 and ev['episodes_masked'] > 0
