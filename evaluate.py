@@ -363,12 +363,11 @@ def main(argv=None):
             progress_line(out['progress_by_role']['cooperative'], 'cooperative  ')
             progress_line(out['progress_by_role'][role], label)
     if args.json:
+        perturbations = (('noise', NOISE_FLAGS), ('latency', LATENCY_FLAGS), ('dynamics', DYNAMICS_FLAGS),
+                         ('localization', LOCALIZATION_FLAGS))
         hidden = (() if safety is not None else ('safety', 'near_miss')) + \
             (() if progress is not None else ('timeouts', 'stall_window')) + \
-            (() if noise is not None else tuple(f[2:].replace('-', '_') for f in NOISE_FLAGS)) + \
-            (() if latency is not None else tuple(f[2:].replace('-', '_') for f in LATENCY_FLAGS)) + \
-            (() if dynamics is not None else tuple(f[2:].replace('-', '_') for f in DYNAMICS_FLAGS)) + \
-            (() if localization is not None else tuple(f[2:].replace('-', '_') for f in LOCALIZATION_FLAGS)) + \
+            tuple(f[2:].replace('-', '_') for name, flags in perturbations if name not in out for f in flags) + \
             (() if crowd is not None else ('crowd',) + tuple(f[2:].replace('-', '_') for f in CROWD_FLAGS)) + \
             (() if dwa_params is not None else tuple(f[2:].replace('-', '_') for f in DWA_FLAGS)) + \
             (() if planner is not None else ('planner', 'geodesic'))
@@ -377,14 +376,7 @@ def main(argv=None):
                'ticks': out['ticks'], 'metrics': m,
                'columns': list(COLUMNS), 'totals': out['totals'].tolist(),
                'partials': out['partials'].tolist()}
-        if noise is not None:
-            res['noise'] = out['noise']
-        if latency is not None:
-            res['latency'] = out['latency']
-        if dynamics is not None:
-            res['dynamics'] = out['dynamics']
-        if localization is not None:
-            res['localization'] = out['localization']
+        res.update((name, out[name]) for name, _ in perturbations if name in out)
         if crowd is not None:
             res['crowd'] = crowd.settings()
         if dwa_params is not None:

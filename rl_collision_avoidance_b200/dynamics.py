@@ -22,8 +22,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .latency import _host_flags, _ptr, check_flags
-from .noise import check_stream_id
+from .perturbation import as_command, check_flags, check_seed, check_stream_id, device_of, host_flags, pair_argument, \
+    ptr
 
 MAX_ACCEL = 100.0               # RLCA_DYNAMICS_MAX_ACCEL, m/s^2 and rad/s^2
 
@@ -54,9 +54,7 @@ class DynamicsParams:
     def __post_init__(self):
         object.__setattr__(self, 'linear', _accel_range('linear', self.linear))
         object.__setattr__(self, 'angular', _accel_range('angular', self.angular))
-        if isinstance(self.seed, bool) or int(self.seed) != self.seed or not 0 <= int(self.seed) < 1 << 64:
-            raise ValueError(f'the dynamics seed must be an integer in 0 .. 2^64 - 1, got {self.seed!r}')
-        object.__setattr__(self, 'seed', int(self.seed))
+        object.__setattr__(self, 'seed', check_seed('dynamics', self.seed))
 
     @property
     def linear_on(self):
@@ -85,8 +83,7 @@ class Dynamics:
             raise TypeError('params must be a DynamicsParams')
         self.env, self.params, self.stream_id = env, params, check_stream_id(stream_id)
         self._p = params.struct(self.stream_id)
-        d = torch.device(env.device)
-        self._dev = d if d.index is not None or d.type != 'cuda' else torch.device('cuda', torch.cuda.current_device())
+        self._dev = device_of(env)
         N = env.N
         self.calls = 0
         self._vel = torch.zeros(N, 2, device=env.device)
@@ -111,14 +108,11 @@ class Dynamics:
         Returns `self.executed`, one buffer reused by every call."""
         env = self.env
         check_flags(env, self._dev, flags)
-        a = cmd if (cmd.device == self._dev and cmd.dtype == torch.float32 and cmd.is_contiguous()) \
-            else cmd.to(device=env.device, dtype=torch.float32).contiguous()
-        if tuple(a.shape) != (env.N, 2):
-            raise ValueError(f'the command must have shape ({env.N}, 2)')
+        a = as_command(env, self._dev, cmd)
         draw = self.calls
         self.calls += 1
         _lib.check(env.lib.rlca_dynamics_action(C.byref(env.cfg), C.byref(self._p), C.byref(self._state),
-                                                draw & 0xFFFFFFFF, _ptr(flags), _ptr(a), _ptr(self.executed),
+                                                draw & 0xFFFFFFFF, ptr(flags), ptr(a), ptr(self.executed),
                                                 env._stream()))
         return self.executed
 
@@ -143,7 +137,7 @@ def action_host(cfg, params: DynamicsParams, state: HostState, draw, cmd, flags=
     a = np.ascontiguousarray(cmd, np.float32)
     if a.shape != (N, 2):
         raise ValueError('cmd must have one (v, w) row per agent')
-    f = _host_flags(flags, N)
+    f = host_flags(flags, N)
     out = np.empty_like(a)
     _lib.check(_lib.load().rlca_dynamics_action_host(C.byref(cfg), C.byref(params.struct(stream_id)),
                                                      C.byref(state.struct()), int(draw),
@@ -167,14 +161,6 @@ def add_dynamics_arguments(ap):
                     help='seed of the limit draws (default: --seed)')
 
 
-def _limits(text):
-    parts = text.split(',')
-    if len(parts) not in (1, 2):
-        raise ValueError('takes A or A,A_MAX')
-    vals = [float(p) for p in parts]
-    return (vals[0], vals[0]) if len(vals) == 1 else tuple(vals)
-
-
 def dynamics_from_arguments(ap, args):
     """DynamicsParams of the acceleration-limit flags, or None when none is given; ap.error for a bad value (a limit
     of 0 included: leave the flag out instead) and for --dynamics-seed on its own.  The seed is --dynamics-seed, else
@@ -184,14 +170,10 @@ def dynamics_from_arguments(ap, args):
             ap.error('--dynamics-seed applies with --accel-limit or --angular-accel-limit only')
         return None
     ranges = {}
-    for name, flag in (('linear', 'accel_limit'), ('angular', 'angular_accel_limit')):
-        text = getattr(args, flag)
-        try:
-            ranges[name] = _limits(text) if text is not None else (0.0, 0.0)
-        except ValueError as e:
-            ap.error('--%s: %s' % (flag.replace('_', '-'), e))
-        if text is not None and ranges[name][0] <= 0.0:
-            ap.error('--%s: a limit must be > 0' % flag.replace('_', '-'))
+    for name, flag in (('linear', '--accel-limit'), ('angular', '--angular-accel-limit')):
+        ranges[name] = pair_argument(ap, args, flag)
+        if getattr(args, flag[2:].replace('-', '_')) is not None and ranges[name][0] <= 0.0:
+            ap.error('%s: a limit must be > 0' % flag)
     seed = args.dynamics_seed if args.dynamics_seed is not None else getattr(args, 'seed', 0)
     try:
         return DynamicsParams(seed=seed, **ranges)

@@ -21,6 +21,7 @@ from . import _lib
 from .dwa import DwaController
 from .model.ppo import generate_action_no_sampling
 from .orca import NhOrcaController, OrcaController, mode_shares
+from .perturbation import Chain
 from .planner import geodesic_metrics, geodesic_totals
 
 COLUMNS = _lib.EVAL_PARTIALS
@@ -506,29 +507,15 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     'progress_totals', 'progress' (progress_metrics) and 'progress_tracker'; with `non_cooperative` also
     'progress_partials_split' and 'progress_by_role'.  With None nothing of this is allocated or launched.
 
-    With `noise` (a noise.Noise on `env`, DESIGN.md §9p) the robots sense and act under noise: the first stack and,
-    after every tick, the stack the tick wrote get `noise.scan` (with env.flags), and the command, after the
-    non-cooperative override and the circle rule, becomes `noise.action`'s executed command before control_vel.
-    env.obs, env.gs and the state are never perturbed, so the trackers keep measuring the true scan and poses.  The
-    result then also holds 'noise' (the settings).  Scan noise needs a policy: the ORCA baselines do not read the scan.
-
-    With `latency` (a latency.Latency on `env`, DESIGN.md §9q) the robots read old scans and execute old commands: the
-    first stack and, after every tick, the stack the tick wrote get `latency.scan` (with env.flags) before any noise,
-    and the command, after the circle rule and before noise, becomes `latency.action`'s executed command, with the
-    flags of the previous tick (None on the first).  A circle robot stopped by the circle rule still runs out the
-    commands already queued.  The result then also holds 'latency' (the settings).  Scan delay needs a policy.
-
-    With `dynamics` (a dynamics.Dynamics on `env`, DESIGN.md §9r) the robots have acceleration limits: the command,
-    last of all, after any noise, becomes `dynamics.action`'s executed command, with the flags of the previous tick
-    (None on the first).  A circle robot stopped by the circle rule brakes at its limit instead of stopping on the
-    spot.  The ORCA baselines command velocities like the policy, so the limits apply to them too.  The result then
-    also holds 'dynamics' (the settings).
-
-    With `localization` (a localization.Localization on `env`, DESIGN.md §9s) the policy reads its local goal from a
-    believed pose and its speed with odometry noise: at the start (flags None) and after every tick, after any latency
-    and noise have touched the stack, `localization.observe` with env.flags turns env.gs into the gs the policy reads
-    next.  env.gs and the state stay the truth, so success, crashes and every tracker measure the true poses.  The
-    result then also holds 'localization' (the settings).  Policies only, not hybrid: the ORCA baselines and the hybrid
+    With `noise`, `latency`, `dynamics` or `localization` (a noise.Noise, latency.Latency, dynamics.Dynamics or
+    localization.Localization on `env`, DESIGN.md §9p-§9s) the robots sense and act through a perturbation.Chain of
+    them, which fixes their order (§9y): the command, after the masked override and the circle rule, becomes the
+    chain's executed command, and the first stack and every stack a tick wrote are perturbed before the policy reads
+    them.  A circle robot stopped by the circle rule still runs out its queued commands and brakes at its limit.
+    env.obs, env.gs and the state are never perturbed, so the trackers keep measuring the truth.  The result then also
+    holds each one's settings under its name.  Scan noise and scan delay need a policy: the ORCA baselines do not read
+    the scan.  The ORCA baselines command velocities like the policy, so command latency, actuation noise and the
+    limits apply to them.  Localization error is for policies only, not hybrid: the ORCA baselines and the hybrid
     driver read the true state through their own kernels; non-cooperative robots keep the truth.
 
     With `crowd` (a crowd.Crowd on `env`, DESIGN.md §9t) its agents follow the social force instead, applied where the
@@ -543,9 +530,9 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     settings and 'fallback_share': the robot-ticks, over all robot-ticks, on which no candidate was admissible and it
     commanded (0, 0)).  ValueError together with `hybrid`, which switches a policy.
 
-    With `planner` (a planner.Planner on `env`, DESIGN.md §9w) the planner is updated at the start and after every
-    tick, after any latency and noise have touched the stack and before the trackers: it re-plans the robots whose goal
-    changed and keeps every episode's geodesic length.  With planner.steer the policy (or the DWA baseline) reads the
+    With `planner` (a planner.Planner on `env`, DESIGN.md §9w), the chain's last link, the planner is updated at the
+    start and after every tick, before the trackers: it re-plans the robots whose goal changed and keeps every
+    episode's geodesic length.  With planner.steer the policy (or the DWA baseline) reads the
     planner's gs: a waypoint on the geodesic path as the local goal where the goal is out of sight.  The result then
     also holds 'geodesic_partials' (num_worlds, planner.NPARTIALS), 'geodesic_totals' and 'geodesic'
     (planner.geodesic_metrics), with `non_cooperative` or `crowd` also 'geodesic_partials_split' and
@@ -554,6 +541,7 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
     steer with the ORCA baselines or `hybrid` (they read the true goal) and with `localization` (the planner plans from
     the true pose)."""
     dwa = isinstance(policy, DwaController)
+    orca = isinstance(policy, (OrcaController, NhOrcaController))
     if dwa:
         if policy.env is not env:
             raise ValueError('the DWA controller belongs to another env')
@@ -565,42 +553,27 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         if crowd.env is not env:
             raise ValueError('the crowd belongs to another env')
     masked, role = (crowd, 'crowd') if crowd is not None else (non_cooperative, 'non_cooperative')
-    if dynamics is not None and dynamics.env is not env:
-        raise ValueError('the dynamics belongs to another env')
+    chain = Chain(env, noise, latency, dynamics, localization, planner)
     if localization is not None:
-        if localization.env is not env:
-            raise ValueError('the localization belongs to another env')
-        if isinstance(policy, (OrcaController, NhOrcaController)):
+        if orca:
             raise ValueError('localization error changes what a policy reads; the ORCA baselines read the true state')
         if hybrid is not None:
             raise ValueError('localization error changes what a policy reads; the hybrid driver reads the true state')
-    if planner is not None:
-        if planner.env is not env:
-            raise ValueError('the planner belongs to another env')
-        if planner.steer:
-            if isinstance(policy, (OrcaController, NhOrcaController)):
-                raise ValueError('the planner steers what a policy reads; the ORCA baselines read the true goal '
-                                 'through their own kernels')
-            if hybrid is not None:
-                raise ValueError('the planner steers what a policy reads; the hybrid driver reads the true goal')
-            if localization is not None:
-                raise ValueError('the planner plans from the true pose; localization error needs a planner on the '
-                                 'believed pose')
-    if latency is not None:
-        if latency.env is not env:
-            raise ValueError('the latency belongs to another env')
-        if latency.params.scan_on and isinstance(policy, (OrcaController, NhOrcaController)):
-            raise ValueError('scan delay changes what a policy reads; the ORCA baselines do not read the scan')
+    if planner is not None and planner.steer:
+        if orca:
+            raise ValueError('the planner steers what a policy reads; the ORCA baselines read the true goal through '
+                             'their own kernels')
+        if hybrid is not None:
+            raise ValueError('the planner steers what a policy reads; the hybrid driver reads the true goal')
+    if latency is not None and latency.params.scan_on and orca:
+        raise ValueError('scan delay changes what a policy reads; the ORCA baselines do not read the scan')
     E = int(episodes)
     if int(check_every) < 1:
         raise ValueError('check_every must be >= 1')
-    if hybrid is not None and isinstance(policy, (OrcaController, NhOrcaController)):
+    if hybrid is not None and orca:
         raise ValueError('hybrid switches a policy; the ORCA baselines are not switched')
-    if noise is not None:
-        if noise.env is not env:
-            raise ValueError('the noise belongs to another env')
-        if noise.params.scan_on and isinstance(policy, (OrcaController, NhOrcaController)):
-            raise ValueError('scan noise perturbs what a policy reads; the ORCA baselines do not read the scan')
+    if noise is not None and noise.params.scan_on and orca:
+        raise ValueError('scan noise perturbs what a policy reads; the ORCA baselines do not read the scan')
     tracker = EpisodeTracker(env, E)
     safe = SafetyTracker(env, tracker, safety) if safety is not None else None
     prog = ProgressTracker(env, tracker, progress) if progress is not None else None
@@ -616,23 +589,16 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         hybrid.reset()
     obs = env.get_laser_observation()
     stacks = [obs[:, None, :].repeat(1, 3, 1).contiguous(), torch.empty(N, 3, env.beam_mum, device=dev)]
-    if latency is not None:
-        latency.scan(stacks[0])
-    if noise is not None:
-        noise.scan(stacks[0])
-    gs = localization.observe() if localization is not None else None
     if planner is not None:
         planner.attach(tracker)
-        pgs = planner.update()
-        if planner.steer:
-            gs = pgs
+    gs = chain.sense(stacks[0])
     terminal = torch.zeros(N, dtype=torch.bool, device=dev)
     fallbacks = torch.zeros(N, dtype=torch.int64, device=dev) if dwa else None
     goal_done = 1 if circle else E
     ticks = 0
     for tick in range(int(max_ticks)):
         k = tick & 1
-        if isinstance(policy, (OrcaController, NhOrcaController)):
+        if orca:
             scaled = policy()
         elif dwa:
             scaled = policy(stacks[k], env.gs if gs is None else gs)
@@ -647,23 +613,9 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
             masked.apply(scaled)
         if circle:
             scaled = torch.stack((torch.where(terminal, 0.0, scaled[:, 0]), scaled[:, 1]), 1)
-        if latency is not None:
-            scaled = latency.action(scaled, env.flags if tick > 0 else None)
-        if noise is not None:
-            scaled = noise.action(scaled)
-        if dynamics is not None:
-            scaled = dynamics.action(scaled, env.flags if tick > 0 else None)
+        scaled = chain.command(scaled, env.flags if tick > 0 else None)
         env.control_vel(scaled, stack_in=stacks[k], stack_out=stacks[1 - k])
-        if latency is not None:
-            latency.scan(stacks[1 - k], env.flags)
-        if noise is not None:
-            noise.scan(stacks[1 - k], env.flags)
-        if localization is not None:
-            gs = localization.observe(env.flags)
-        if planner is not None:
-            pgs = planner.update(env.flags)
-            if planner.steer:
-                gs = pgs
+        gs = chain.sense(stacks[1 - k], env.flags)
         if safe is not None:
             safe.track()
         if prog is not None:
@@ -715,14 +667,7 @@ def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=N
         if planner.steer:
             out['planner'] = dict(planner.settings(),
                                   **planner.status_shares(None if masked is None else masked.mask))
-    if noise is not None:
-        out['noise'] = noise.settings()
-    if latency is not None:
-        out['latency'] = latency.settings()
-    if dynamics is not None:
-        out['dynamics'] = dynamics.settings()
-    if localization is not None:
-        out['localization'] = localization.settings()
+    out.update(chain.settings())
     if dwa:
         out['dwa'] = dict(policy.settings(), fallback_share=int(fallbacks.sum()) / (ticks * N) if ticks else math.nan)
     return out

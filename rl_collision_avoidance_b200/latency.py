@@ -23,7 +23,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .noise import check_stream_id
+from .perturbation import as_command, check_flags, check_seed, check_stack, check_stream_id, device_of, host_flags, \
+    pair_argument, ptr
 
 MAX_DELAY = 8                   # RLCA_LATENCY_MAX_DELAY: 0.8 s at dt = 0.1 s
 
@@ -54,9 +55,7 @@ class LatencyParams:
     def __post_init__(self):
         object.__setattr__(self, 'scan_delay', _delay_range('scan_delay', self.scan_delay))
         object.__setattr__(self, 'command_delay', _delay_range('command_delay', self.command_delay))
-        if isinstance(self.seed, bool) or int(self.seed) != self.seed or not 0 <= int(self.seed) < 1 << 64:
-            raise ValueError(f'the latency seed must be an integer in 0 .. 2^64 - 1, got {self.seed!r}')
-        object.__setattr__(self, 'seed', int(self.seed))
+        object.__setattr__(self, 'seed', check_seed('latency', self.seed))
 
     @property
     def scan_on(self):
@@ -75,17 +74,6 @@ class LatencyParams:
                                   self.command_delay[1], self.seed, check_stream_id(stream_id))
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
-def check_flags(env, dev, flags):
-    """ValueError unless `flags` is None or a contiguous (env.N, 4) uint8 tensor on the device `dev` of `env`"""
-    if flags is not None and (tuple(flags.shape) != (env.N, 4) or flags.dtype != torch.uint8 or
-                              not flags.is_contiguous() or flags.device != dev):
-        raise ValueError(f'flags must be a contiguous ({env.N}, 4) uint8 tensor on {env.device}')
-
-
 class Latency:
     """The latency of one env handle: its rings and per-robot delays.  `stream_id` tells apart the handles of one run
     (a mix component's index); the handle's world_offset tells apart the shards of a data-parallel run.  Every `scan`
@@ -96,8 +84,7 @@ class Latency:
             raise TypeError('params must be a LatencyParams')
         self.env, self.params, self.stream_id = env, params, check_stream_id(stream_id)
         self._p = params.struct(self.stream_id)
-        d = torch.device(env.device)
-        self._dev = d if d.index is not None or d.type != 'cuda' else torch.device('cuda', torch.cuda.current_device())
+        self._dev = device_of(env)
         N, B = env.N, env.beam_mum
         self.scan_calls = 0
         self.action_calls = 0
@@ -133,15 +120,13 @@ class Latency:
         and every row when `flags` is None, start an episode: their delay is redrawn and their stack kept.  Returns
         `stack`."""
         env = self.env
-        if tuple(stack.shape) != (env.N, 3, env.beam_mum) or stack.dtype != torch.float32 or \
-                not stack.is_contiguous() or stack.device != self._dev:
-            raise ValueError(f'stack must be a contiguous ({env.N}, 3, {env.beam_mum}) float32 tensor on {env.device}')
+        check_stack(env, self._dev, stack)
         check_flags(env, self._dev, flags)
         draw = self.scan_calls
         self.scan_calls += 1
         if self.params.scan_on:
             _lib.check(env.lib.rlca_latency_scan(C.byref(env.cfg), C.byref(self._p), C.byref(self._state),
-                                                 draw & 0xFFFFFFFF, _ptr(flags), _ptr(stack), env._stream()))
+                                                 draw & 0xFFFFFFFF, ptr(flags), ptr(stack), env._stream()))
         return stack
 
     def action(self, cmd, flags=None):
@@ -155,12 +140,9 @@ class Latency:
         self.action_calls += 1
         if not self.params.command_on:
             return cmd
-        a = cmd if (cmd.device == self._dev and cmd.dtype == torch.float32 and cmd.is_contiguous()) \
-            else cmd.to(device=env.device, dtype=torch.float32).contiguous()
-        if tuple(a.shape) != (env.N, 2):
-            raise ValueError(f'the command must have shape ({env.N}, 2)')
+        a = as_command(env, self._dev, cmd)
         _lib.check(env.lib.rlca_latency_action(C.byref(env.cfg), C.byref(self._p), C.byref(self._state),
-                                               draw & 0xFFFFFFFF, _ptr(flags), _ptr(a), _ptr(self.executed),
+                                               draw & 0xFFFFFFFF, ptr(flags), ptr(a), ptr(self.executed),
                                                env._stream()))
         return self.executed
 
@@ -180,20 +162,13 @@ class HostState:
         return _lib.LatencyState(vp(self.scan_ring), vp(self.cmd_ring), vp(self.scan_delay), vp(self.cmd_delay))
 
 
-def _host_flags(flags, N):
-    f = None if flags is None else np.ascontiguousarray(flags, np.uint8)
-    if f is not None and f.shape != (N, 4):
-        raise ValueError(f'flags must have shape ({N}, 4)')
-    return f
-
-
 def scan_host(cfg, params: LatencyParams, state: HostState, draw, stack, flags=None, stream_id=0):
     """rlca_latency_scan_host on a host stack (N, 3, beams) float32, changed in place, and the HostState `state`
     (the kernel's code, run by the CPU); returns the stack."""
     N = int(cfg.robots_per_world) * int(cfg.num_worlds)
     if stack.dtype != np.float32 or not stack.flags.c_contiguous or stack.shape != (N, 3, int(cfg.beams)):
         raise ValueError(f'stack must be a contiguous ({N}, 3, {int(cfg.beams)}) float32 array')
-    f = _host_flags(flags, N)
+    f = host_flags(flags, N)
     _lib.check(_lib.load().rlca_latency_scan_host(C.byref(cfg), C.byref(params.struct(stream_id)),
                                                   C.byref(state.struct()), int(draw),
                                                   f.ctypes.data_as(C.c_void_p) if f is not None else None,
@@ -207,7 +182,7 @@ def action_host(cfg, params: LatencyParams, state: HostState, draw, cmd, flags=N
     a = np.ascontiguousarray(cmd, np.float32)
     if a.shape != (N, 2):
         raise ValueError('cmd must have one (v, w) row per agent')
-    f = _host_flags(flags, N)
+    f = host_flags(flags, N)
     out = np.empty_like(a)
     _lib.check(_lib.load().rlca_latency_action_host(C.byref(cfg), C.byref(params.struct(stream_id)),
                                                     C.byref(state.struct()), int(draw),
@@ -231,14 +206,6 @@ def add_latency_arguments(ap):
                     help='seed of the delay draws (default: --seed)')
 
 
-def _ticks(text):
-    parts = text.split(',')
-    if len(parts) not in (1, 2):
-        raise ValueError('takes T or T,T_MAX')
-    vals = [int(p) for p in parts]
-    return (vals[0], vals[0]) if len(vals) == 1 else tuple(vals)
-
-
 def latency_from_arguments(ap, args):
     """LatencyParams of the latency flags, or None when none is given; ap.error for a bad value and for
     --latency-seed on its own.  The seed is --latency-seed, else --seed, else 0."""
@@ -246,13 +213,8 @@ def latency_from_arguments(ap, args):
         if args.latency_seed is not None:
             ap.error('--latency-seed applies with --scan-delay or --command-delay only')
         return None
-    ranges = {}
-    for name in ('scan_delay', 'command_delay'):
-        text = getattr(args, name)
-        try:
-            ranges[name] = _ticks(text) if text is not None else (0, 0)
-        except ValueError as e:
-            ap.error('--%s: %s' % (name.replace('_', '-'), e))
+    ranges = {name: pair_argument(ap, args, '--' + name.replace('_', '-'), int)
+              for name in ('scan_delay', 'command_delay')}
     seed = args.latency_seed if args.latency_seed is not None else getattr(args, 'seed', 0)
     try:
         return LatencyParams(seed=seed, **ranges)

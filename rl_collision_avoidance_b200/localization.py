@@ -23,9 +23,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .dynamics import _limits
-from .latency import _host_flags, _ptr, check_flags
-from .noise import check_stream_id
+from .perturbation import check_flags, check_seed, check_stream_id, device_of, host_flags, pair_argument, ptr
 
 DEFAULT_CORRELATION_TIME = 2.0  # s
 
@@ -69,9 +67,7 @@ class LocalizationParams:
         if not tau >= 0.0:
             raise ValueError(f'correlation_time must be >= 0 s or inf, got {self.correlation_time!r}')
         object.__setattr__(self, 'correlation_time', tau)
-        if isinstance(self.seed, bool) or int(self.seed) != self.seed or not 0 <= int(self.seed) < 1 << 64:
-            raise ValueError(f'the localization seed must be an integer in 0 .. 2^64 - 1, got {self.seed!r}')
-        object.__setattr__(self, 'seed', int(self.seed))
+        object.__setattr__(self, 'seed', check_seed('localization', self.seed))
 
     @property
     def on(self):
@@ -99,8 +95,7 @@ class Localization:
             raise TypeError('params must be a LocalizationParams')
         self.env, self.params, self.stream_id = env, params, check_stream_id(stream_id)
         self._p = params.struct(self.stream_id)
-        d = torch.device(env.device)
-        self._dev = d if d.index is not None or d.type != 'cuda' else torch.device('cuda', torch.cuda.current_device())
+        self._dev = device_of(env)
         self.calls = 0
         self._err = self._sigma = self.believed = None
         if params.on:
@@ -150,8 +145,8 @@ class Localization:
             return out.copy_(g)
         o = self.believed if out is None else out
         _lib.check(env.lib.rlca_localization_observe(C.byref(env.cfg), C.byref(self._p), C.byref(self._state),
-                                                     draw & 0xFFFFFFFF, _ptr(flags),
-                                                     C.byref(env._state_struct(env._cur)), _ptr(g), _ptr(o),
+                                                     draw & 0xFFFFFFFF, ptr(flags),
+                                                     C.byref(env._state_struct(env._cur)), ptr(g), ptr(o),
                                                      env._stream()))
         return o
 
@@ -180,7 +175,7 @@ def observe_host(cfg, params: LocalizationParams, state: HostState, draw, pose, 
             raise ValueError(f'{name} must have one row of 4 per agent')
         arrs.append(a)
     p, g, s = arrs
-    f = _host_flags(flags, N)
+    f = host_flags(flags, N)
     out = np.empty_like(s)
     st = _lib.EnvState(p.ctypes.data, g.ctypes.data, None, None)
     _lib.check(_lib.load().rlca_localization_observe_host(C.byref(cfg), C.byref(params.struct(stream_id)),
@@ -223,14 +218,8 @@ def localization_from_arguments(ap, args):
         if args.localization_seed is not None:
             ap.error('--localization-seed applies with --pose-error, --heading-error or --speed-error only')
         return None
-    vals = {}
-    for name, flag in (('pose_sigma', 'pose_error'), ('heading_sigma', 'heading_error'),
-                       ('speed_sigma', 'speed_error')):
-        text = getattr(args, flag)
-        try:
-            vals[name] = _limits(text) if text is not None else (0.0, 0.0)
-        except ValueError as e:
-            ap.error('--%s: %s' % (flag.replace('_', '-'), e))
+    vals = {name: pair_argument(ap, args, flag) for name, flag in
+            (('pose_sigma', '--pose-error'), ('heading_sigma', '--heading-error'), ('speed_sigma', '--speed-error'))}
     seed = args.localization_seed if args.localization_seed is not None else getattr(args, 'seed', 0)
     tau = args.pose_error_time if pose_time else DEFAULT_CORRELATION_TIME
     try:

@@ -20,8 +20,8 @@ import numpy as np
 import torch
 
 from . import _lib
-
-MAX_STREAM_ID = (1 << 24) - 1
+from .perturbation import as_command, check_flags, check_seed, check_stack, check_stream_id, device_of, host_flags, \
+    pair_argument, ptr
 
 
 def _finite_nonneg(name, v):
@@ -49,9 +49,7 @@ class NoiseParams:
         if not 0.0 <= p <= 1.0:
             raise ValueError(f'dropout must be in [0, 1], got {self.dropout!r}')
         object.__setattr__(self, 'dropout', p)
-        if isinstance(self.seed, bool) or int(self.seed) != self.seed or not 0 <= int(self.seed) < 1 << 64:
-            raise ValueError(f'the noise seed must be an integer in 0 .. 2^64 - 1, got {self.seed!r}')
-        object.__setattr__(self, 'seed', int(self.seed))
+        object.__setattr__(self, 'seed', check_seed('noise', self.seed))
 
     @property
     def scan_on(self):
@@ -70,16 +68,6 @@ class NoiseParams:
                                 check_stream_id(stream_id))
 
 
-def check_stream_id(stream_id):
-    if isinstance(stream_id, bool) or int(stream_id) != stream_id or not 0 <= int(stream_id) <= MAX_STREAM_ID:
-        raise ValueError(f'stream_id must be an integer in 0 .. {MAX_STREAM_ID}, got {stream_id!r}')
-    return int(stream_id)
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
 class Noise:
     """The noise of one env handle.  `stream_id` tells apart the handles of one run (a mix component's index), so that
     agent 0 of two handles draws different noise; the handle's world_offset tells apart the shards of a data-parallel
@@ -90,8 +78,7 @@ class Noise:
             raise TypeError('params must be a NoiseParams')
         self.env, self.params, self.stream_id = env, params, check_stream_id(stream_id)
         self._p = params.struct(self.stream_id)
-        d = torch.device(env.device)
-        self._dev = d if d.index is not None or d.type != 'cuda' else torch.device('cuda', torch.cuda.current_device())
+        self._dev = device_of(env)
         self.scan_draws = 0
         self.action_draws = 0
         self.executed = torch.zeros(env.N, 2, device=env.device) if params.action_on else None
@@ -104,17 +91,13 @@ class Noise:
         flags[:, 3] (was_reset) is set, and every row when `flags` is None, get the perturbed frame in all three
         slots.  Returns `stack`."""
         env = self.env
-        if tuple(stack.shape) != (env.N, 3, env.beam_mum) or stack.dtype != torch.float32 or \
-                not stack.is_contiguous() or stack.device != self._dev:
-            raise ValueError(f'stack must be a contiguous ({env.N}, 3, {env.beam_mum}) float32 tensor on {env.device}')
-        if flags is not None and (tuple(flags.shape) != (env.N, 4) or flags.dtype != torch.uint8 or
-                                  not flags.is_contiguous() or flags.device != self._dev):
-            raise ValueError(f'flags must be a contiguous ({env.N}, 4) uint8 tensor on {env.device}')
+        check_stack(env, self._dev, stack)
+        check_flags(env, self._dev, flags)
         draw = self.scan_draws
         self.scan_draws += 1
         if self.params.scan_on:
-            _lib.check(env.lib.rlca_noise_scan(C.byref(env.cfg), C.byref(self._p), draw & 0xFFFFFFFF, _ptr(flags),
-                                               _ptr(stack), env._stream()))
+            _lib.check(env.lib.rlca_noise_scan(C.byref(env.cfg), C.byref(self._p), draw & 0xFFFFFFFF, ptr(flags),
+                                               ptr(stack), env._stream()))
         return stack
 
     def action(self, scaled):
@@ -125,12 +108,9 @@ class Noise:
         self.action_draws += 1
         if not self.params.action_on:
             return scaled
-        a = scaled if (scaled.device == self._dev and scaled.dtype == torch.float32 and scaled.is_contiguous()) \
-            else scaled.to(device=env.device, dtype=torch.float32).contiguous()
-        if tuple(a.shape) != (env.N, 2):
-            raise ValueError(f'the command must have shape ({env.N}, 2)')
-        _lib.check(env.lib.rlca_noise_action(C.byref(env.cfg), C.byref(self._p), draw & 0xFFFFFFFF, _ptr(a),
-                                             _ptr(self.executed), env._stream()))
+        a = as_command(env, self._dev, scaled)
+        _lib.check(env.lib.rlca_noise_action(C.byref(env.cfg), C.byref(self._p), draw & 0xFFFFFFFF, ptr(a),
+                                             ptr(self.executed), env._stream()))
         return self.executed
 
 
@@ -140,9 +120,7 @@ def scan_host(cfg, params: NoiseParams, draw, stack, flags=None, stream_id=0):
     N = int(cfg.robots_per_world) * int(cfg.num_worlds)
     if stack.dtype != np.float32 or not stack.flags.c_contiguous or stack.shape != (N, 3, int(cfg.beams)):
         raise ValueError(f'stack must be a contiguous ({N}, 3, {int(cfg.beams)}) float32 array')
-    f = None if flags is None else np.ascontiguousarray(flags, np.uint8)
-    if f is not None and f.shape != (N, 4):
-        raise ValueError(f'flags must have shape ({N}, 4)')
+    f = host_flags(flags, N)
     vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
     _lib.check(_lib.load().rlca_noise_scan_host(C.byref(cfg), C.byref(params.struct(stream_id)), int(draw), vp(f),
                                                 vp(stack)))
@@ -178,14 +156,6 @@ def add_noise_arguments(ap):
                     help='seed of the noise draws (default: --seed)')
 
 
-def _action_sigmas(text):
-    parts = text.split(',')
-    if len(parts) not in (1, 2):
-        raise ValueError('--action-noise takes SIGMA or SIGMA_V,SIGMA_W')
-    vals = [float(p) for p in parts]
-    return (vals[0], vals[0]) if len(vals) == 1 else tuple(vals)
-
-
 def noise_from_arguments(ap, args):
     """NoiseParams of the noise flags, or None when none is given; ap.error for a bad value and for --noise-seed on its
     own.  The seed is --noise-seed, else --seed, else 0."""
@@ -194,10 +164,7 @@ def noise_from_arguments(ap, args):
         if args.noise_seed is not None:
             ap.error('--noise-seed applies with --scan-noise, --beam-dropout or --action-noise only')
         return None
-    try:
-        sv, sw = _action_sigmas(args.action_noise) if args.action_noise is not None else (0.0, 0.0)
-    except ValueError as e:
-        ap.error('--action-noise: %s' % e)
+    sv, sw = pair_argument(ap, args, '--action-noise')
     seed = args.noise_seed if args.noise_seed is not None else getattr(args, 'seed', 0)
     try:
         return NoiseParams(range_sigma=args.scan_noise if args.scan_noise is not None else 0.0,

@@ -24,6 +24,7 @@ from .latency import Latency
 from .localization import Localization
 from .noise import Noise
 from .orca import NonCooperative
+from .perturbation import Chain
 from .planner import Planner
 from .stage_world import RESULT_STRINGS
 
@@ -57,12 +58,8 @@ class _Component:
 
     def __init__(self, env, ro, a, b, noise=None, latency=None, dynamics=None, localization=None):
         self.env, self.a, self.b = env, a, b
-        self.noise = noise                              # noise.Noise of the env, or None
-        self.latency = latency                          # latency.Latency of the env, or None
-        self.dynamics = dynamics                        # dynamics.Dynamics of the env, or None
-        self.localization = localization                # localization.Localization of the env, or None
+        self.chain = Chain(env, noise, latency, dynamics, localization)     # attach_planners sets chain.planner
         self.masked = None                              # orca.NonCooperative or crowd.Crowd of the env, or None
-        self.planner = None                             # planner.Planner of the env (steering), or None
         self.ticked = False                             # a tick has run, so self.flags holds its flags
         self.name = env.sc.name
         self.relayout = env.sc.layout is not None
@@ -72,6 +69,13 @@ class _Component:
         self.rewards = ro.rewards[:, a:b]
         self.flags = ro.flags[:, a:b]
         self.eplog = ro.eplog[:, a:b]
+
+    # the chain's links, readable on the component; the chain holds the only reference
+    noise = property(lambda self: self.chain.noise)
+    latency = property(lambda self: self.chain.latency)
+    dynamics = property(lambda self: self.chain.dynamics)
+    localization = property(lambda self: self.chain.localization)
+    planner = property(lambda self: self.chain.planner)
 
     def check_aligned(self):
         for name, view in (('action', self.scaled), ('stack', self.stacks), ('gs', self.gs),
@@ -88,60 +92,35 @@ class _Component:
             e.random_layout()                           # the first layout, as evaluate() draws it
         obs = e.get_laser_observation()
         self.stacks[0] = obs[:, None, :]                # deque([obs, obs, obs]) (:60)
-        if self.latency is not None:
-            self.latency.scan(self.stacks[0])           # every row starts an episode: its rings hold the first scan
-        if self.noise is not None:
-            self.noise.scan(self.stacks[0])             # what a noisy robot's first scan reads, in all three slots
         self.gs[0] = e.gs
-        if self.localization is not None:
-            self.localization.observe(gs=self.gs[0], out=self.gs[0])    # every row starts an episode
-        if self.planner is not None:
-            self.planner.update(None, gs=self.gs[0])    # the first waypoints; every row starts an episode
+        self.chain.sense(self.stacks[0], None, gs=self.gs[0])      # every row starts an episode
 
     def tick(self, t):
-        """Tick t on the component's slices, after the policy has written ro.scaled.  With noise the robots execute
-        noise.action's command (ro.scaled, which PPO's actions were drawn with, is not written) and the stack the tick
-        and the re-layout wrote is perturbed as a noisy robot would read it.  With latency the command is delayed
-        first, with the flags of the tick before (at t = 0 slot H - 1 of the previous rollout, still intact; None on
-        the run's first tick), and the stack is delayed after the re-layout and before any noise.  With dynamics the
-        command, last of all, is limited in acceleration, with the same flags of the tick before.  With localization
-        the gs the tick and the re-layout wrote becomes, in place and last of all, the gs the robot believes, with the
-        flags of this tick.  With masked agents their rows of ro.scaled are overwritten first, before any latency; PPO
-        keeps the policy's sampled action in ro.actions.  With a planner the gs the tick and the re-layout wrote becomes,
-        in place and last of all, the waypoint gs, and a reward planner shapes the tick's reward and the returns of the
-        episodes it ended in place, with the flags as the re-layout left them."""
+        """Tick t on the component's slices, after the policy has written ro.scaled: masked agents overwrite their rows
+        of ro.scaled, the chain turns it into the executed command (PPO keeps the policy's sampled action in
+        ro.actions), and after the tick and the re-layout the chain perturbs, in place, the stack, gs, reward and eplog
+        slots the tick wrote (perturbation.Chain).  The flags of the tick before are at t = 0 slot H - 1 of the previous
+        rollout, still intact, and None on the run's first tick."""
         e = self.env
         if self.masked is not None:
             self.masked.apply(self.scaled)
-        cmd = self.scaled
         prev = self.flags[t - 1] if t > 0 else self.flags[-1] if self.ticked else None
-        if self.latency is not None:
-            cmd = self.latency.action(cmd, prev)
+        cmd = self.chain.command(self.scaled, prev)
         self.ticked = True
-        if self.noise is not None:
-            cmd = self.noise.action(cmd)
-        if self.dynamics is not None:
-            cmd = self.dynamics.action(cmd, prev)
         e.control_vel(cmd, live=e.live if self.relayout else None, stack_in=self.stacks[t],
                       stack_out=self.stacks[t + 1],
                       out={'reward': self.rewards[t], 'flags': self.flags[t], 'gs': self.gs[t + 1],
                            'eplog': self.eplog[t]})
         if self.relayout:
             e.relayout_finished(self.stacks[t + 1], out={'gs': self.gs[t + 1], 'flags': self.flags[t]})
-        if self.latency is not None:
-            self.latency.scan(self.stacks[t + 1], self.flags[t])
-        if self.noise is not None:
-            self.noise.scan(self.stacks[t + 1], self.flags[t])
-        if self.localization is not None:
-            self.localization.observe(self.flags[t], gs=self.gs[t + 1], out=self.gs[t + 1])
-        if self.planner is not None:
-            self.planner.update(self.flags[t], reward=self.rewards[t], eplog=self.eplog[t], gs=self.gs[t + 1])
+        self.chain.sense(self.stacks[t + 1], self.flags[t], gs=self.gs[t + 1], reward=self.rewards[t],
+                         eplog=self.eplog[t])
 
 
 def compose(envs, ro, noise=None, latency=None, dynamics=None, localization=None):
     """The components of `envs` on the rollout `ro`: env k owns the agent columns that follow env k - 1's.  With more
     than one env, ValueError for a slice the kernels cannot read at its alignment (mix.SLICE_ALIGN).  `noise`
-    (noise.NoiseParams) gives component k a noise.Noise with stream id k, `latency` (latency.LatencyParams) a
+    (noise.NoiseParams) gives component k's chain a noise.Noise with stream id k, `latency` (latency.LatencyParams) a
     latency.Latency with stream id k, `dynamics` (dynamics.DynamicsParams) a dynamics.Dynamics with stream id k and
     `localization` (localization.LocalizationParams) a localization.Localization with stream id k."""
     comps, a = [], 0
@@ -178,8 +157,8 @@ def attach_planners(comps, planner, localization=None, tables=None):
     if tables is not None and len(tables) != len(comps):
         raise ValueError('planner tables: %d given for %d components' % (len(tables), len(comps)))
     for k, c in enumerate(comps):
-        c.planner = Planner(c.env, steer=True, reward=planner == 'geodesic',
-                            tables=None if tables is None else tables[k])
+        c.chain.planner = Planner(c.env, steer=True, reward=planner == 'geodesic',
+                                  tables=None if tables is None else tables[k])
 
 
 def _status_shares(comps):
@@ -264,27 +243,22 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     `diagnostics` (DESIGN.md §9n) adds stats[k]['diagnostics'], the metrics of model.diagnostics.metrics plus
     'epochs_run' and 'logstd', and rank 0 writes one line per update to the diag.log logger; `target_kl` (finite and
     > 0, implies diagnostics) skips the remaining epochs of an update once an epoch's approx_kl_k3 exceeds it.
-    `noise` (noise.NoiseParams, DESIGN.md §9p) trains under sensor and actuation noise: component k gets a noise.Noise
-    with stream id k, its robots execute the perturbed command and every stack the policy reads is perturbed; the
-    env's world_offset makes the draws of each data-parallel rank differ.  None issues no noise launch.
-    `latency` (latency.LatencyParams, DESIGN.md §9q) trains under sensing and command latency: component k gets a
-    latency.Latency with stream id k, its robots execute the command of l ticks earlier and read the scan of d ticks
-    earlier, both before any noise; PPO still stores the issued action and its log-probability.  None launches nothing.
-    `dynamics` (dynamics.DynamicsParams, DESIGN.md §9r) trains under acceleration limits: component k gets a
-    dynamics.Dynamics with stream id k, applied to the command last, after any noise; PPO still stores the issued
-    action.  None launches nothing.
-    `localization` (localization.LocalizationParams, DESIGN.md §9s) trains under localization error: component k gets
-    a localization.Localization with stream id k, and every gs the policy reads (ro.gs, slot 0 and every slot a tick
-    wrote, after any re-layout) is the believed one, so PPO stores and re-evaluates what the policy read.  Rewards and
-    episode ends stay on the true state.  None launches nothing.
+    `noise` (noise.NoiseParams, DESIGN.md §9p), `latency` (latency.LatencyParams, §9q), `dynamics`
+    (dynamics.DynamicsParams, §9r) and `localization` (localization.LocalizationParams, §9s) train under sensor and
+    actuation noise, sensing and command latency, acceleration limits and localization error: component k gets each
+    as a link with stream id k of its perturbation.Chain, which fixes their order (§9y).  The robots execute the
+    perturbed command, and every stack and gs the policy reads (ro.stacks, ro.gs: slot 0 and every slot a tick wrote,
+    after any re-layout) is the perturbed one, so PPO stores and re-evaluates what the policy read; it still stores the
+    issued action and its log-probability.  Rewards and episode ends stay on the true state, and the env's
+    world_offset makes the draws of each data-parallel rank differ.  None launches nothing.
     `non_cooperative` ((k, speed or None), DESIGN.md §9h) or `crowd` ((k, crowd.CrowdParams, map flag), §9t) puts k
     masked agents into every world of every component (masked_agents); their rows of the action are overwritten before
-    any latency, and every row of their columns is left out of every PPO update (stage 1: filter_index; stage 2:
+    the chain, and every row of their columns is left out of every PPO update (stage 1: filter_index; stage 2:
     united with get_filter_index).  The stats then also hold 'by_role' {'cooperative', 'non_cooperative' or 'crowd'}.
-    `planner` ('geodesic' or 'straight', DESIGN.md §9x) gives component k a planner.Planner (attach_planners): every
-    gs the policy reads (ro.gs, slot 0 and every slot a tick wrote, after any re-layout) is the waypoint gs, so PPO
-    stores and re-evaluates what the policy read; 'geodesic' also shapes ro.rewards and the episodes' returns by
-    geodesic progress, 'straight' keeps the tick's reward.  The stats then also hold 'planner', the status shares of the
+    `planner` ('geodesic' or 'straight', DESIGN.md §9x) gives component k a planner.Planner (attach_planners), the
+    last link of its chain: every gs the policy reads is the waypoint gs, so PPO stores and re-evaluates what the
+    policy read; 'geodesic' also shapes ro.rewards and the episodes' returns by geodesic progress, 'straight' keeps
+    the tick's reward.  The stats then also hold 'planner', the status shares of the
     update's robot-ticks.  Refused with localization error and on maps the planner refuses.  None launches nothing.
     `planner_tables` (one planner.PlannerTables per env, in order) saves building the planning graphs again.
     Returns per-update stats (for tests / benchmarks); 'by_scenario' splits the episodes by component."""
