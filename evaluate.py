@@ -12,7 +12,8 @@ with random goals at least --random-min-travel L m away (defaults 8, 10, 1 and S
 does the same among static obstacles: world w lays out in arena w mod T of a generated map of --arena-count T walled
 arenas of --arena-side S m with --arena-obstacles LO,HI random boxes and discs each, drawn from --arena-seed (another
 seed gives held-out arenas), with --arena-robots, --arena-separation and --arena-min-travel (defaults 64, 10, 4,10, 0,
-8, 1.2 and S / 2; DESIGN.md §9v).  --hybrid switches
+8, 1.2 and S / 2; DESIGN.md §9v); --per-arena adds each arena's episodes and rates to --json and prints the ten arenas
+of lowest success (DESIGN.md §9z).  --hybrid switches
 the policy per robot by the nearest return of its newest scan: straight to the goal when it is beyond
 --hybrid-r-safe, the policy's action with v capped at --hybrid-v-safe when it is within --hybrid-r-risk, the policy's
 action otherwise, and prints the share of robot-ticks in each mode (DESIGN.md §9j).  --safety adds how closely the robots
@@ -88,7 +89,7 @@ from rl_collision_avoidance_b200.dwa import DWA_FLAGS, DwaController, add_argume
 from rl_collision_avoidance_b200.dynamics import DYNAMICS_FLAGS, Dynamics, add_dynamics_arguments, \
     dynamics_from_arguments
 from rl_collision_avoidance_b200.evaluation import AUTO_RESET, COLUMNS, PROGRESS_COLUMNS, PROGRESS_DEFAULTS, \
-    SAFETY_COLUMNS, evaluate, non_cooperative_mask
+    SAFETY_COLUMNS, evaluate, non_cooperative_mask, per_arena
 from rl_collision_avoidance_b200.latency import LATENCY_FLAGS, Latency, add_latency_arguments, \
     latency_from_arguments
 from rl_collision_avoidance_b200.localization import LOCALIZATION_FLAGS, Localization, add_localization_arguments, \
@@ -164,6 +165,9 @@ def main(argv=None):
     add_dynamics_arguments(ap)
     add_localization_arguments(ap)
     add_planner_arguments(ap)
+    ap.add_argument('--per-arena', action='store_true',
+                    help='arena scenario: metrics per arena (world w in arena w mod T) in --json, and the ten arenas '
+                         'of lowest success printed (DESIGN.md §9z)')
     ap.add_argument('--json', default=None, help='write totals, metrics and per-world partials here')
     args = ap.parse_args(argv)
     if args.policy is not None and not os.path.exists(args.policy):
@@ -177,6 +181,8 @@ def main(argv=None):
         ap.error('--circle-robots / --circle-radius apply to --scenario circle only')
     check_arena_arguments(ap, args)
     check_random_arguments(ap, args)
+    if args.per_arena and args.scenario != 'arena':
+        ap.error('--per-arena applies to --scenario arena only')
     if args.non_cooperative is None and args.non_cooperative_speed is not None:
         ap.error('--non-cooperative-speed applies with --non-cooperative only')
     v_max = COMMON['v_max']
@@ -362,6 +368,18 @@ def main(argv=None):
         if masked is not None:
             progress_line(out['progress_by_role']['cooperative'], 'cooperative  ')
             progress_line(out['progress_by_role'][role], label)
+    arenas = None
+    if args.per_arena:
+        arenas = per_arena(out['partials'], sc.layout, int(env.cfg.world_offset))
+        seen = [r for r in arenas if r['metrics']['episodes']]
+        low = sorted(seen, key=lambda r: (r['metrics']['success_rate'], r['arena']))[:10]
+        print('per arena (world w in arena w mod %d), lowest success of %d arenas with episodes:'
+              % (sc.layout.count, len(seen)))
+        for r in low:
+            ma = r['metrics']
+            print('  arena %3d  cells %5d  worlds %d  episodes %d  success %.4f  crash %.4f  time-out %.4f  '
+                  'unfinished %d' % (r['arena'], r['cells'], r['worlds'], ma['episodes'], ma['success_rate'],
+                                     ma['crash_rate'], ma['timeout_rate'], ma['unfinished']))
     if args.json:
         perturbations = (('noise', NOISE_FLAGS), ('latency', LATENCY_FLAGS), ('dynamics', DYNAMICS_FLAGS),
                          ('localization', LOCALIZATION_FLAGS))
@@ -392,6 +410,10 @@ def main(argv=None):
         if masked is not None:
             res['by_role'] = out['by_role']
             res['partials_split'] = out['partials_split'].tolist()
+        if arenas is not None:
+            res['per_arena'] = [{'arena': r['arena'], 'cells': r['cells'], 'worlds': r['worlds'],
+                                 **{k: r['metrics'][k] for k in ('episodes', 'success_rate', 'crash_rate',
+                                                                 'timeout_rate', 'unfinished')}} for r in arenas]
         if hy is not None:
             res['modes'] = out['modes']
             res['mode_counts'] = out['mode_counts'].tolist()

@@ -803,6 +803,59 @@ int rlca_layout_arena_respawn_host(const rlca_env_config *cfg, const rlca_layout
                                    uint8_t *live_host, int32_t *status_host);
 
 /* =====================================================================================
+ * Arena curriculum (csrc/rlca_layout.cu, DESIGN.md §9z): per-arena episode outcomes tallied on the device, and
+ * layouts that draw a world's arena in proportion to integer weights that favour arenas neither always nor never
+ * solved.
+ * ===================================================================================== */
+
+/* The state of a curriculum over T arenas.  Device pointers for the device entries, host pointers for the twins. */
+typedef struct rlca_arena_curriculum {
+    int32_t num_arenas;          /* T, 1 <= T < 2^20, equal to the tables' */
+    uint64_t *cdf;               /* T + 1: the exclusive prefix sum of the weights w_a; cdf[T] their total */
+    int32_t *world_arena;        /* num_worlds: the arena of each world's current layout */
+    int32_t *pending;            /* 2 T: episodes (a) and successes (T + a) ended in arena a since the last update */
+    float *E, *S;                /* T: decayed episodes and successes */
+} rlca_arena_curriculum;
+
+/* rlca_layout_arena with a weighted arena draw: world g (global index) lays out at episode 0 in the arena a with
+ * cdf[a] <= (m cdf[T]) >> 24 < cdf[a + 1], m = 2^24 u0 of pick 1's draw (agent g R, episode, draw 0, purpose 0xA0);
+ * equal weights give pick 1's arena.  Starts, goals, headings, records and status as rlca_layout_arena; a world laid
+ * out gets world_arena[w] = a, a world that fails keeps its world_arena.  RLCA_ERR_INVALID for what rlca_layout_arena
+ * rejects with pick 1, a NULL curriculum or buffer, curriculum T outside [1, 2^20) or different from the tables'. */
+int rlca_layout_arena_weighted(const rlca_env_config *cfg, const rlca_layout_params *params,
+                               const rlca_arena_tables *tables, const rlca_arena_curriculum *curriculum,
+                               const rlca_env_state *state, int32_t *status_dev, void *stream);
+/* The same from HOST buffers, tables and curriculum by the sequential loop; equal to the device's bit for bit.  Also
+ * RLCA_ERR_INVALID for what rlca_arena_tables_check rejects. */
+int rlca_layout_arena_weighted_host(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                    const rlca_arena_tables *tables_host, const rlca_arena_curriculum *curriculum_host,
+                                    float *pose_host, float *goal_host, float *acc_host, int32_t *status_host);
+/* After a tick (auto_reset 0), in place of rlca_layout_arena_respawn: first the tally, then the re-layout.  Tally: a
+ * row of world w whose tick flags have x != 0 and z != 0 ended an episode (a success when z == 1); rows with
+ * row_mask[i] != 0 are not counted (row_mask may be NULL: every row counts).  The world's counts go to
+ * pending[world_arena[w]] and pending[T + world_arena[w]], read before the re-layout.  Re-layout: as
+ * rlca_layout_arena_respawn at episode e = meta.y + 1 with the weighted draw of rlca_layout_arena_weighted at that
+ * episode; world_arena[w] changes only when the world is re-laid.  RLCA_ERR_INVALID for what
+ * rlca_layout_arena_weighted rejects, cfg->auto_reset != 0 or a NULL buffer other than row_mask. */
+int rlca_layout_arena_weighted_respawn(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                       const rlca_arena_tables *tables, const rlca_arena_curriculum *curriculum,
+                                       const uint8_t *row_mask_dev, const rlca_env_state *state, uint8_t *flags_dev,
+                                       uint8_t *live_dev, int32_t *status_dev, void *stream);
+int rlca_layout_arena_weighted_respawn_host(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                            const rlca_arena_tables *tables_host,
+                                            const rlca_arena_curriculum *curriculum_host,
+                                            const uint8_t *row_mask_host, float *pose_host, float *goal_host,
+                                            float *acc_host, int32_t *meta_host, uint8_t *flags_host,
+                                            uint8_t *live_host, int32_t *status_host);
+/* Once per PPO update, one CTA: for every arena a, in float32 with one rounding per operation,
+ *   E_a = decay E_a + e_a, S_a = decay S_a + s_a   (e_a, s_a = pending[a], pending[T + a]),
+ *   p = (S_a + 1) / (E_a + 2), q = uniform + (1 - uniform) 4 p (1 - p), w_a = max(1, floor(2^20 q)),
+ * then pending = 0 and cdf = the exclusive prefix sum of w in uint64.  world_arena is not read.  RLCA_ERR_INVALID for
+ * a NULL curriculum or buffer, T outside [1, 2^20), decay outside [0, 1) or uniform outside [0, 1] (NaN included). */
+int rlca_arena_curriculum_update(const rlca_arena_curriculum *curriculum, float decay, float uniform, void *stream);
+int rlca_arena_curriculum_update_host(const rlca_arena_curriculum *curriculum_host, float decay, float uniform);
+
+/* =====================================================================================
  * Safety metrics (csrc/rlca_safety.cu, DESIGN.md §9m): how closely robots pass and why they crash, per episode of the
  * evaluation tracker above.
  *

@@ -18,6 +18,9 @@ crowd agents (DESIGN.md §9t); either way their rows are left out of every PPO u
 --planner trains with the global planner (DESIGN.md §9x): the policy reads a line-of-sight waypoint on the geodesic path
 as its local goal and the reward pays geodesic progress; --planner-reward straight keeps the tick's straight-line
 reward.  Stage 1, stage 2 and the arenas, alone or mixed; not with localization error, random layouts or the circle.
+--arena-curriculum [--curriculum-decay L] [--curriculum-uniform E] draws the arena of each re-layout by an automatic
+curriculum (DESIGN.md §9z): per-arena success tallied on the device, arenas the policy neither always nor never solves
+drawn more often.  --scenario arena or an arena component of --mix.
 """
 import argparse
 import logging
@@ -29,6 +32,7 @@ import torch
 
 from rl_collision_avoidance_b200.crowd import add_crowd_arguments, crowd_from_arguments, \
     non_cooperative_from_arguments
+from rl_collision_avoidance_b200.curriculum import CurriculumParams, check_params
 from rl_collision_avoidance_b200.dynamics import add_dynamics_arguments, dynamics_from_arguments
 from rl_collision_avoidance_b200.latency import add_latency_arguments, latency_from_arguments
 from rl_collision_avoidance_b200.localization import add_localization_arguments, localization_from_arguments
@@ -148,6 +152,15 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
     ap.add_argument('--planner-reward', default=None, choices=('geodesic', 'straight'),
                     help='with --planner: geodesic (default) shapes the reward by geodesic progress, straight keeps '
                          "the tick's straight-line reward")
+    ap.add_argument('--arena-curriculum', action='store_true',
+                    help='draw the arena of every re-layout by an automatic curriculum (DESIGN.md §9z): arenas whose '
+                         'recent success rate is neither near 0 nor near 1 more often')
+    ap.add_argument('--curriculum-decay', type=float, default=None, metavar='L',
+                    help='with --arena-curriculum: weight of the per-arena counts before each update, in [0, 1) '
+                         '(default %g)' % CurriculumParams.decay)
+    ap.add_argument('--curriculum-uniform', type=float, default=None, metavar='E',
+                    help='with --arena-curriculum: share of every arena\'s score independent of its outcomes, in [0, 1] '
+                         '(default %g)' % CurriculumParams.uniform)
     args = ap.parse_args(argv)
     noise = noise_from_arguments(ap, args)
     latency = latency_from_arguments(ap, args)
@@ -190,6 +203,18 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
         arena_sc = arena_scenario_from_arguments(ap, args, pick=1)
         if mix is None:
             sc = arena_sc
+    curriculum = None
+    if args.arena_curriculum:
+        if args.scenario != 'arena' and not arena_in_mix:
+            ap.error('--arena-curriculum needs --scenario arena or an arena component of --mix')
+        try:
+            curriculum = check_params(CurriculumParams(
+                CurriculumParams.decay if args.curriculum_decay is None else args.curriculum_decay,
+                CurriculumParams.uniform if args.curriculum_uniform is None else args.curriculum_uniform))
+        except ValueError as e:
+            ap.error('--arena-curriculum: %s' % e)
+    elif args.curriculum_decay is not None or args.curriculum_uniform is not None:
+        ap.error('--curriculum-decay / --curriculum-uniform apply with --arena-curriculum only')
     planner = planner_tables = None
     if args.planner_reward is not None and not args.planner:
         ap.error('--planner-reward needs --planner')
@@ -266,6 +291,7 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
         logger.info('############Start Training###########')
         logger.info('#####################################')
     start_update = 0
+    curriculum_state = None
     if args.resume:
         policy.load_state_dict(torch.load(args.resume, map_location=device))
         extra = args.resume + '.trainer'
@@ -274,6 +300,8 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
             opt.load_state_dict(st['optimizer'])
             policy.sample_counter = int(st.get('sample_counter', 0))
             start_update = int(st.get('update', 0))              # checkpoint names continue instead of overwriting
+            if curriculum is not None:
+                curriculum_state = st.get('curriculum')
             if logger:
                 logger.info('resumed from %s (update %d, Adam step %d)' % (args.resume, st.get('update', -1), opt.step_count))
     hp = dict(HORIZON=HORIZON, GAMMA=GAMMA, LAMDA=LAMDA, BATCH_SIZE=batch_size, EPOCH=epoch, COEFF_ENTROPY=COEFF_ENTROPY,
@@ -284,7 +312,8 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
                     logger=logger, logger_cal=logger_cal, stage=stage, max_updates=args.updates, process_group=pg, rank=rank,
                     start_update=start_update, diagnostics=args.diagnostics, target_kl=args.target_kl, noise=noise,
                     latency=latency, dynamics=dynamics, localization=localization, non_cooperative=non_cooperative,
-                    crowd=crowd, planner=planner, planner_tables=planner_tables)
+                    crowd=crowd, planner=planner, planner_tables=planner_tables, curriculum=curriculum,
+                    curriculum_state=curriculum_state)
         if rank == 0 and stats:
             s = stats[-1]
             print('update %d: rollout %.3fs update %.3fs -> %.0f agent-steps/s per GPU; mean ep reward %.2f' %
@@ -294,6 +323,11 @@ def main(stage=1, world_cls=StageWorld, num_env=NUM_ENV, batch_size=BATCH_SIZE, 
             if 'planner' in s:
                 print('last update, planner: %s' % ', '.join('%s %.3f' % (k, v) for k, v in s['planner'].items()
                                                              if k != 'robot_ticks'))
+            if 'curriculum' in s:
+                cu = s['curriculum']
+                print('last update, curriculum: %d arenas, effective %.1f, draw share max %.4f min %.4f, %d episodes '
+                      'folded in' % (cu['arenas'], cu['effective_arenas'], cu['max_share'], cu['min_share'],
+                                     cu['episodes']))
             if 'by_role' in s:
                 for role, r in s['by_role'].items():
                     print('last update, %s: %d episodes, success %.3f, crash %.3f'

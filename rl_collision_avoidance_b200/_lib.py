@@ -73,6 +73,12 @@ class ArenaTables(C.Structure):
     _fields_ = [('num_arenas', C.c_int32), ('cell_off', C.c_void_p), ('cells', C.c_void_p)]
 
 
+class ArenaCurriculum(C.Structure):
+    """Mirror of rlca_arena_curriculum (include/rlca.h): device pointers, or host pointers for the host twins."""
+    _fields_ = [('num_arenas', C.c_int32), ('cdf', C.c_void_p), ('world_arena', C.c_void_p), ('pending', C.c_void_p),
+                ('E', C.c_void_p), ('S', C.c_void_p)]
+
+
 class HybridParams(C.Structure):
     """Mirror of rlca_hybrid_params (include/rlca.h)."""
     _fields_ = [('r_safe', C.c_float), ('r_risk', C.c_float), ('v_safe', C.c_float), ('heading_gain', C.c_float)]
@@ -299,6 +305,18 @@ SYMBOLS = {
                                             C.c_int32, C.POINTER(EnvState), _P, _P, _P, _P]),
     'rlca_layout_arena_respawn_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams),
                                                  C.POINTER(ArenaTables), C.c_int32, _P, _P, _P, _P, _P, _P, _P]),
+    'rlca_layout_arena_weighted': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams), C.POINTER(ArenaTables),
+                                             C.POINTER(ArenaCurriculum), C.POINTER(EnvState), _P, _P]),
+    'rlca_layout_arena_weighted_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams),
+                                                  C.POINTER(ArenaTables), C.POINTER(ArenaCurriculum), _P, _P, _P, _P]),
+    'rlca_layout_arena_weighted_respawn': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams),
+                                                     C.POINTER(ArenaTables), C.POINTER(ArenaCurriculum), _P,
+                                                     C.POINTER(EnvState), _P, _P, _P, _P]),
+    'rlca_layout_arena_weighted_respawn_host': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(LayoutParams),
+                                                          C.POINTER(ArenaTables), C.POINTER(ArenaCurriculum), _P, _P,
+                                                          _P, _P, _P, _P, _P, _P]),
+    'rlca_arena_curriculum_update': (C.c_int, [C.POINTER(ArenaCurriculum), C.c_float, C.c_float, _P]),
+    'rlca_arena_curriculum_update_host': (C.c_int, [C.POINTER(ArenaCurriculum), C.c_float, C.c_float]),
     'rlca_safety_track': (C.c_int, [C.POINTER(EnvConfig), C.POINTER(SafetyParams), C.POINTER(EnvState),
                                     C.POINTER(EnvState), C.POINTER(StepIO), C.POINTER(EvalState),
                                     C.POINTER(SafetyState), _P]),

@@ -1,5 +1,6 @@
 // rlca_layout.cu — random start / goal layouts for evaluation and training (sm_90a), C ABI in include/rlca.h,
-// DESIGN.md §9i and §9k, and the same sampler in the arenas of a generated obstacle map (§9v, at the end of the file).
+// DESIGN.md §9i and §9k, the same sampler in the arenas of a generated obstacle map (§9v), and the arena curriculum's
+// weighted arena draw, per-arena tally and weight update (§9z), at the end of the file.
 //
 // rlca_layout_random writes a layout into an env state in place, once before an episode: for world w (global index
 // cfg.world_offset + w) and robots r = 0 .. R-1 in order, the start is the first try k < max_reject whose draw,
@@ -24,6 +25,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
+
+#include <vector>
 
 #include "../../include/rlca.h"
 #include "rlca_common.cuh"
@@ -332,11 +335,16 @@ __host__ __device__ __forceinline__ int arena_of(const LayoutConsts &c, const Ar
     return (int)(((uint64_t)(u[0] * 16777216.0f) * (uint32_t)t.T) >> 24);
 }
 
-__host__ __device__ __forceinline__ ArenaDraw arena_draw(const LayoutConsts &c, const ArenaArgs &t, uint32_t world)
+// The draws of arena a.
+__host__ __device__ __forceinline__ ArenaDraw arena_cells_draw(const ArenaArgs &t, int a)
 {
-    const int a = arena_of(c, t, world);
     const int32_t off = t.cell_off[a];
     return ArenaDraw{ t.cells + off, (uint32_t)(t.cell_off[a + 1] - off), t.ocx, t.ocy, t.res };
+}
+
+__host__ __device__ __forceinline__ ArenaDraw arena_draw(const LayoutConsts &c, const ArenaArgs &t, uint32_t world)
+{
+    return arena_cells_draw(t, arena_of(c, t, world));
 }
 
 struct ArenaSampler {
@@ -466,6 +474,195 @@ int check_arena_cells(const rlca_env_config *cfg, const rlca_arena_tables *t, co
 ArenaArgs arena_args(const rlca_env_config *cfg, const rlca_arena_tables *t, int32_t pick)
 {
     return { t->cell_off, t->cells, t->num_arenas, pick, cfg->origin_cx, cfg->origin_cy, cfg->resolution };
+}
+
+// ---------------------------------------------------------------------------------------------- curriculum (§9z)
+// An arena drawn in proportion to integer weights w_a: pick 1's draw m = 2^24 u0 (agent g R, episode, draw 0, purpose
+// 0xA0) and the arena a with cdf[a] <= (m cdf[T]) >> 24 < cdf[a + 1], cdf the exclusive prefix sum of w.  Equal weights
+// W give floor(floor(m T W / 2^24) / W) = (m T) >> 24, pick 1's arena.  T < 2^20 and w <= 2^20 keep m cdf[T] < 2^64.
+#define CURRICULUM_THREADS 1024
+#define CURRICULUM_MAX_ARENAS (1 << 20)
+#define CURRICULUM_ONE 1048576.0f                    // 2^20: the weight of score 1
+
+__host__ __device__ __forceinline__ int weighted_arena(const LayoutConsts &c, const uint64_t *cdf, int T)
+{
+    float u[4];
+    dev_rand4(c.seed, c.agent0, c.episode, 0u, PURPOSE_ARENA, u);
+    const uint64_t target = ((uint64_t)(u[0] * 16777216.0f) * cdf[T]) >> 24;
+    int lo = 0, hi = T;                              // the largest lo < T with cdf[lo] <= target
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (cdf[mid] <= target) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// The arena sampler with the weighted draw; world_arena[world - world_offset] records the arena of a layout that
+// succeeded, and keeps the old arena when one fails.
+struct WeightedArenaSampler {
+    ArenaArgs t;
+    const uint64_t *cdf;
+    int32_t *world_arena;
+    int world_offset;
+    __device__ __forceinline__ bool operator()(const LayoutConsts &c, uint32_t world, LayoutSmem &s, int R,
+                                               int max_reject, int lane, int32_t *status) const
+    {
+        const int a = weighted_arena(c, cdf, t.T);
+        if (!warp_layout(arena_cells_draw(t, a), c, s, R, max_reject, lane, status)) return false;
+        if (lane == 0) world_arena[(int)world - world_offset] = a;
+        return true;
+    }
+};
+
+// The ended rows of world w in this tick's flags (x != 0 and z != 0; success z == 1), rows with row_mask != 0 left
+// out, added to pending[a] (episodes) and pending[T + a] (successes) of the world's arena a.  One integer atomic per
+// counter per world, so the sums do not depend on the order of the worlds.
+__device__ __forceinline__ void tally_world(int w, int lane, int R, int T, const uint8_t *__restrict__ flags,
+                                            const uint8_t *__restrict__ row_mask,
+                                            const int32_t *__restrict__ world_arena, int32_t *__restrict__ pending)
+{
+    const size_t i0 = (size_t)w * R;
+    int ended = 0, reached = 0;
+    for (int r = lane; r < 64; r += 32) {            // robots lane and lane + 32 (R <= 64), the loop warp-uniform
+        bool e = false, s = false;
+        if (r < R && !(row_mask && row_mask[i0 + r])) {
+            const uint8_t fx = flags[4 * (i0 + r)], fz = flags[4 * (i0 + r) + 2];
+            e = fx != 0 && fz != 0;
+            s = e && fz == 1;
+        }
+        ended += __popc(__ballot_sync(0xffffffffu, e));
+        reached += __popc(__ballot_sync(0xffffffffu, s));
+    }
+    if (lane == 0 && ended) {
+        const int a = world_arena[w];
+        if (a >= 0 && a < T) {
+            atomicAdd(pending + a, ended);
+            if (reached) atomicAdd(pending + T + a, reached);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(LAYOUT_THREADS)
+rlca_layout_arena_weighted_kernel(int num_worlds, int R, int max_reject, int pre_distance_zero, int world_offset,
+                                  uint64_t seed, float sep2, float travel2, ArenaArgs t,
+                                  const uint64_t *__restrict__ cdf, int32_t *__restrict__ world_arena,
+                                  float4 *__restrict__ pose, float4 *__restrict__ goal, float4 *__restrict__ acc,
+                                  int32_t *__restrict__ status)
+{
+    __shared__ LayoutSmem smem[LAYOUT_WARPS];
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int w = blockIdx.x * LAYOUT_WARPS + wib;
+    if (w >= num_worlds) return;                     // warp-uniform
+    LayoutSmem &s = smem[wib];
+    const LayoutConsts c = { seed, (uint32_t)(world_offset + w) * (uint32_t)R, 0.0f, sep2, travel2, 0u };
+    const WeightedArenaSampler sampler{ t, cdf, world_arena, world_offset };
+    if (!sampler(c, (uint32_t)(world_offset + w), s, R, max_reject, lane, status + w)) return;
+    for (int r = lane; r < R; r += 32) {
+        const size_t i = (size_t)w * R + r;
+        float4 p = pose[i], g = goal[i], a = acc[i];
+        layout_apply(pre_distance_zero, s.sx[r], s.sy[r], layout_heading(c, (uint32_t)r), s.gx[r], s.gy[r], p, g, a);
+        pose[i] = p; goal[i] = g; acc[i] = a;
+    }
+    if (lane == 0) status[w] = 0;
+}
+
+// After a tick (auto_reset 0): tally the tick's ended rows against each world's arena, then park and re-lay as
+// rlca_layout_arena_respawn_kernel does, with the weighted arena draw.  One warp per world.
+__global__ void __launch_bounds__(LAYOUT_THREADS)
+rlca_layout_arena_weighted_respawn_kernel(int num_worlds, int R, int max_reject, int pre_distance_zero,
+                                          int world_offset, uint64_t seed, float sep2, float travel2, ArenaArgs t,
+                                          const uint64_t *__restrict__ cdf, int32_t *__restrict__ world_arena,
+                                          int32_t *__restrict__ pending, const uint8_t *__restrict__ row_mask,
+                                          float4 *__restrict__ pose, float4 *__restrict__ goal,
+                                          float4 *__restrict__ acc, int4 *__restrict__ meta,
+                                          uint8_t *__restrict__ flags, uint8_t *__restrict__ live,
+                                          int32_t *__restrict__ status)
+{
+    __shared__ LayoutSmem smem[LAYOUT_WARPS];
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int w = blockIdx.x * LAYOUT_WARPS + wib;
+    if (w >= num_worlds) return;                     // warp-uniform
+    // lane 0 reads the world's arena here before its sampler writes a new one
+    tally_world(w, lane, R, t.T, flags, row_mask, world_arena, pending);
+    respawn_world(WeightedArenaSampler{ t, cdf, world_arena, world_offset }, smem[wib], w, lane, R, max_reject,
+                  pre_distance_zero, world_offset, seed, 0.0f, sep2, travel2, pose, goal, acc, meta, flags, live,
+                  status);
+}
+
+// Fold one update's counts into the decayed counts of arena a and return its weight, in float32 with one rounding
+// per operation: E = decay E + e, S = decay S + s, p = (S + 1) / (E + 2), q = uniform + (1 - uniform) 4 p (1 - p),
+// w = max(1, floor(2^20 q)).  q <= 1 whenever E, S >= 0; the clamp to 2^20 keeps the bound for any stored values.
+__host__ __device__ __forceinline__ uint32_t curriculum_fold(float &E, float &S, int32_t e, int32_t s, float decay,
+                                                             float uniform)
+{
+    E = decay * E + (float)e;
+    S = decay * S + (float)s;
+    const float p = (S + 1.0f) / (E + 2.0f);
+    const float q = uniform + (1.0f - uniform) * (4.0f * p * (1.0f - p));
+    const float v = q * CURRICULUM_ONE;
+    return v >= CURRICULUM_ONE ? (uint32_t)CURRICULUM_ONE : v >= 1.0f ? (uint32_t)v : 1u;
+}
+
+// One CTA: every arena's fold, pending zeroed, and the exclusive prefix sum of the weights into cdf (cdf[T] the
+// total), 1024 arenas per round with a carry.  Integer sums: the result does not depend on the thread order.
+__global__ void __launch_bounds__(CURRICULUM_THREADS)
+rlca_arena_curriculum_update_kernel(int T, float decay, float uniform, float *__restrict__ E, float *__restrict__ S,
+                                    int32_t *__restrict__ pending, unsigned long long *__restrict__ cdf)
+{
+    __shared__ unsigned long long warp_sum[CURRICULUM_THREADS / 32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    unsigned long long carry = 0;
+    for (int base = 0; base < T; base += CURRICULUM_THREADS) {
+        const int a = base + threadIdx.x;
+        unsigned long long w = 0;
+        if (a < T) {
+            float e = E[a], s = S[a];
+            w = curriculum_fold(e, s, pending[a], pending[T + a], decay, uniform);
+            E[a] = e; S[a] = s;
+            pending[a] = 0; pending[T + a] = 0;
+        }
+        unsigned long long x = w;                    // inclusive scan in the warp
+        for (int d = 1; d < 32; d <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, x, d);
+            if (lane >= d) x += y;
+        }
+        if (lane == 31) warp_sum[wid] = x;
+        __syncthreads();
+        if (wid == 0) {
+            unsigned long long v = warp_sum[lane];
+            for (int d = 1; d < 32; d <<= 1) {
+                const unsigned long long y = __shfl_up_sync(0xffffffffu, v, d);
+                if (lane >= d) v += y;
+            }
+            warp_sum[lane] = v;
+        }
+        __syncthreads();
+        if (a < T) cdf[a] = carry + (wid ? warp_sum[wid - 1] : 0ull) + x - w;
+        carry += warp_sum[CURRICULUM_THREADS / 32 - 1];
+        __syncthreads();                             // warp_sum is rewritten by the next round
+    }
+    if (threadIdx.x == 0) cdf[T] = carry;
+}
+
+int check_curriculum(const rlca_arena_curriculum *cur, const char *who)
+{
+    if (!cur || !cur->cdf || !cur->world_arena || !cur->pending || !cur->E || !cur->S)
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: curriculum or one of its buffers is NULL", who);
+    if (cur->num_arenas < 1 || cur->num_arenas >= CURRICULUM_MAX_ARENAS)
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: curriculum->num_arenas must be in [1, 2^20)", who);
+    return RLCA_OK;
+}
+
+// check_arena with pick 1 (the weighted draw replaces it), and a curriculum over the tables' arenas
+int check_weighted(const rlca_env_config *cfg, const rlca_layout_params *params, const rlca_arena_tables *tables,
+                   const rlca_arena_curriculum *cur, const char *who)
+{
+    int rc = check_arena(cfg, params, tables, 1, who);
+    if (!rc) rc = check_curriculum(cur, who);
+    if (rc) return rc;
+    if (cur->num_arenas != tables->num_arenas)
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: curriculum->num_arenas must equal tables->num_arenas", who);
+    return RLCA_OK;
 }
 
 }  // namespace
@@ -716,5 +913,159 @@ extern "C" int rlca_layout_arena_respawn_host(const rlca_env_config *cfg, const 
     host_respawn_worlds(cfg, params,
                         [&](const LayoutConsts &c, int w) { return arena_draw(c, t, (uint32_t)(cfg->world_offset + w)); },
                         pose_host, goal_host, acc_host, meta_host, flags_host, live_host, status_host);
+    return RLCA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- curriculum (§9z)
+extern "C" int rlca_layout_arena_weighted(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                          const rlca_arena_tables *tables, const rlca_arena_curriculum *curriculum,
+                                          const rlca_env_state *state, int32_t *status_dev, void *stream)
+{
+    int rc = check_weighted(cfg, params, tables, curriculum, "rlca_layout_arena_weighted");
+    if (rc) return rc;
+    if (!state || !state->pose_dev || !state->goal_dev || !state->acc_dev || !status_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_layout_arena_weighted: a state or status buffer is NULL");
+    const LayoutConsts c = layout_consts(cfg, params, 0, 0u);
+    const int ctas = (cfg->num_worlds + LAYOUT_WARPS - 1) / LAYOUT_WARPS;
+    rlca_layout_arena_weighted_kernel<<<ctas, LAYOUT_THREADS, 0, (cudaStream_t)stream>>>(
+        cfg->num_worlds, cfg->robots_per_world, cfg->max_reject, cfg->pre_distance_zero, cfg->world_offset, c.seed,
+        c.sep2, c.travel2, arena_args(cfg, tables, 1), curriculum->cdf, curriculum->world_arena,
+        reinterpret_cast<float4 *>(state->pose_dev), reinterpret_cast<float4 *>(state->goal_dev),
+        reinterpret_cast<float4 *>(state->acc_dev), status_dev);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_layout_arena_weighted_host(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                               const rlca_arena_tables *tables_host,
+                                               const rlca_arena_curriculum *curriculum_host, float *pose_host,
+                                               float *goal_host, float *acc_host, int32_t *status_host)
+{
+    int rc = check_weighted(cfg, params, tables_host, curriculum_host, "rlca_layout_arena_weighted_host");
+    if (!rc) rc = check_arena_cells(cfg, tables_host, "rlca_layout_arena_weighted_host");
+    if (rc) return rc;
+    if (!pose_host || !goal_host || !acc_host || !status_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "rlca_layout_arena_weighted_host: a buffer is NULL");
+    const ArenaArgs t = arena_args(cfg, tables_host, 1);
+    const rlca_arena_curriculum &cur = *curriculum_host;
+    std::vector<int> drawn(cfg->num_worlds, -1);
+    host_layout_worlds(cfg, params,
+                       [&](const LayoutConsts &c, int w) {
+                           drawn[w] = weighted_arena(c, cur.cdf, t.T);
+                           return arena_cells_draw(t, drawn[w]);
+                       },
+                       pose_host, goal_host, acc_host, status_host);
+    for (int w = 0; w < cfg->num_worlds; ++w)
+        if (status_host[w] == 0) cur.world_arena[w] = drawn[w];
+    return RLCA_OK;
+}
+
+extern "C" int rlca_layout_arena_weighted_respawn(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                                  const rlca_arena_tables *tables,
+                                                  const rlca_arena_curriculum *curriculum, const uint8_t *row_mask_dev,
+                                                  const rlca_env_state *state, uint8_t *flags_dev, uint8_t *live_dev,
+                                                  int32_t *status_dev, void *stream)
+{
+    const char *who = "rlca_layout_arena_weighted_respawn";
+    int rc = check_weighted(cfg, params, tables, curriculum, who);
+    if (rc) return rc;
+    if (cfg->auto_reset != 0) return rlca_set_err(RLCA_ERR_INVALID, "%s: cfg.auto_reset must be 0", who);
+    if (!state || !state->pose_dev || !state->goal_dev || !state->acc_dev || !state->meta_dev || !flags_dev ||
+        !live_dev || !status_dev)
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: a state, flags, live or status buffer is NULL", who);
+    const LayoutConsts c = layout_consts(cfg, params, 0, 0u);
+    const int ctas = (cfg->num_worlds + LAYOUT_WARPS - 1) / LAYOUT_WARPS;
+    rlca_layout_arena_weighted_respawn_kernel<<<ctas, LAYOUT_THREADS, 0, (cudaStream_t)stream>>>(
+        cfg->num_worlds, cfg->robots_per_world, cfg->max_reject, cfg->pre_distance_zero, cfg->world_offset, c.seed,
+        c.sep2, c.travel2, arena_args(cfg, tables, 1), curriculum->cdf, curriculum->world_arena, curriculum->pending,
+        row_mask_dev, reinterpret_cast<float4 *>(state->pose_dev), reinterpret_cast<float4 *>(state->goal_dev),
+        reinterpret_cast<float4 *>(state->acc_dev), reinterpret_cast<int4 *>(state->meta_dev), flags_dev, live_dev,
+        status_dev);
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_layout_arena_weighted_respawn_host(const rlca_env_config *cfg, const rlca_layout_params *params,
+                                                       const rlca_arena_tables *tables_host,
+                                                       const rlca_arena_curriculum *curriculum_host,
+                                                       const uint8_t *row_mask_host, float *pose_host,
+                                                       float *goal_host, float *acc_host, int32_t *meta_host,
+                                                       uint8_t *flags_host, uint8_t *live_host, int32_t *status_host)
+{
+    const char *who = "rlca_layout_arena_weighted_respawn_host";
+    int rc = check_weighted(cfg, params, tables_host, curriculum_host, who);
+    if (!rc) rc = check_arena_cells(cfg, tables_host, who);
+    if (rc) return rc;
+    if (cfg->auto_reset != 0) return rlca_set_err(RLCA_ERR_INVALID, "%s: cfg.auto_reset must be 0", who);
+    if (!pose_host || !goal_host || !acc_host || !meta_host || !flags_host || !live_host || !status_host)
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: a buffer is NULL", who);
+    const ArenaArgs t = arena_args(cfg, tables_host, 1);
+    const rlca_arena_curriculum &cur = *curriculum_host;
+    const int R = cfg->robots_per_world, T = t.T;
+    for (int w = 0; w < cfg->num_worlds; ++w) {                  // the tally, against the arenas before re-layout
+        int ended = 0, reached = 0;
+        for (int r = 0; r < R; ++r) {
+            const size_t i = (size_t)w * R + r;
+            if (row_mask_host && row_mask_host[i]) continue;
+            const uint8_t fx = flags_host[4 * i], fz = flags_host[4 * i + 2];
+            ended += fx != 0 && fz != 0;
+            reached += fx != 0 && fz == 1;
+        }
+        const int a = cur.world_arena[w];
+        if (ended && a >= 0 && a < T) {
+            cur.pending[a] += ended;
+            cur.pending[T + a] += reached;
+        }
+    }
+    std::vector<int> drawn(cfg->num_worlds, -1);
+    host_respawn_worlds(cfg, params,
+                        [&](const LayoutConsts &c, int w) {
+                            drawn[w] = weighted_arena(c, cur.cdf, T);
+                            return arena_cells_draw(t, drawn[w]);
+                        },
+                        pose_host, goal_host, acc_host, meta_host, flags_host, live_host, status_host);
+    for (int w = 0; w < cfg->num_worlds; ++w)
+        if (drawn[w] >= 0 && status_host[w] == 0) cur.world_arena[w] = drawn[w];
+    return RLCA_OK;
+}
+
+static int check_update(const rlca_arena_curriculum *cur, float decay, float uniform, const char *who)
+{
+    int rc = check_curriculum(cur, who);
+    if (rc) return rc;
+    if (!(decay >= 0.0f && decay < 1.0f)) return rlca_set_err(RLCA_ERR_INVALID, "%s: decay must be in [0, 1)", who);
+    if (!(uniform >= 0.0f && uniform <= 1.0f))
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: uniform must be in [0, 1]", who);
+    return RLCA_OK;
+}
+
+extern "C" int rlca_arena_curriculum_update(const rlca_arena_curriculum *curriculum, float decay, float uniform,
+                                            void *stream)
+{
+    int rc = check_update(curriculum, decay, uniform, "rlca_arena_curriculum_update");
+    if (rc) return rc;
+    rlca_arena_curriculum_update_kernel<<<1, CURRICULUM_THREADS, 0, (cudaStream_t)stream>>>(
+        curriculum->num_arenas, decay, uniform, curriculum->E, curriculum->S, curriculum->pending,
+        reinterpret_cast<unsigned long long *>(curriculum->cdf));
+    RLCA_CUDA_TRY(cudaGetLastError());
+    return RLCA_OK;
+}
+
+extern "C" int rlca_arena_curriculum_update_host(const rlca_arena_curriculum *curriculum_host, float decay,
+                                                 float uniform)
+{
+    int rc = check_update(curriculum_host, decay, uniform, "rlca_arena_curriculum_update_host");
+    if (rc) return rc;
+    const rlca_arena_curriculum &c = *curriculum_host;
+    const int T = c.num_arenas;
+    uint64_t total = 0;
+    for (int a = 0; a < T; ++a) {
+        const uint32_t w = curriculum_fold(c.E[a], c.S[a], c.pending[a], c.pending[T + a], decay, uniform);
+        c.pending[a] = 0;
+        c.pending[T + a] = 0;
+        c.cdf[a] = total;
+        total += w;
+    }
+    c.cdf[T] = total;
     return RLCA_OK;
 }

@@ -474,6 +474,22 @@ def metrics(tot):
     return out
 
 
+def per_arena(partials, layout, world_offset=0):
+    """evaluate()'s per-world partials (rows in world order from global world `world_offset`) grouped by arena with
+    pick 0's rule, world w in arena (world_offset + w) mod T (DESIGN.md §9z): one dict per arena a = 0 .. T-1 with
+    'arena', 'cells' (its placeable cells), 'worlds', 'totals' (totals of its rows) and 'metrics' (metrics of those)."""
+    p = np.asarray(partials, np.float64).reshape(-1, NPARTIALS)
+    T = int(layout.count)
+    arena = (int(world_offset) + np.arange(len(p))) % T
+    cells = np.diff(np.asarray(layout.tables.cell_off, np.int64))
+    out = []
+    for a in range(T):
+        tot = totals(p[arena == a])
+        out.append({'arena': a, 'cells': int(cells[a]), 'worlds': int((arena == a).sum()), 'totals': tot,
+                    'metrics': metrics(tot)})
+    return out
+
+
 def evaluate(env, policy, episodes, max_ticks, check_every=50, non_cooperative=None, hybrid=None, safety=None,
              progress=None, noise=None, latency=None, dynamics=None, localization=None, crowd=None, planner=None):
     """Drive every agent of `env` with the deterministic mean action of `policy` (generate_action_no_sampling, scans

@@ -86,6 +86,7 @@ class StageWorld:
         self._host = None
         self._host_ptrs = None
         self._ticked = False
+        self.curriculum = None                  # curriculum.ArenaCurriculum: weighted arena draws (DESIGN.md §9z)
         if self.sc.layout is not None:
             # training on random layouts (relayout_finished): the next tick's live mask and the per-world status
             self.live = torch.ones(N, dtype=torch.uint8, device=dev)
@@ -196,7 +197,7 @@ class StageWorld:
     def random_layout(self):
         """A random layout (DESIGN.md §9i) in every world of the current state: starts, goals and headings drawn on the
         device from the scenario's Layout (rlca_layout_random) or, on an arena scenario, in the world's arena
-        (rlca_layout_arena, §9v), then the scan and local goal from the new poses.  One
+        (rlca_layout_arena, §9v; rlca_layout_arena_weighted with an attached curriculum.ArenaCurriculum, §9z), then the scan and local goal from the new poses.  One
         synchronisation reads the per-world status; ValueError names the first world whose robots could not all be
         placed, and that world keeps its rows."""
         lay = self.sc.layout
@@ -205,7 +206,11 @@ class StageWorld:
         params = _lib.LayoutParams(lay.side, lay.separation, lay.min_travel)
         status = torch.empty(self.num_worlds, dtype=torch.int32, device=self.device)
         st = self._state_struct(self._cur)
-        if self._arena is not None:
+        if self.curriculum is not None:
+            _lib.check(self.lib.rlca_layout_arena_weighted(C.byref(self.cfg), C.byref(params), C.byref(self._arena),
+                                                           C.byref(self.curriculum.struct), C.byref(st), _ptr(status),
+                                                           self._stream()))
+        elif self._arena is not None:
             _lib.check(self.lib.rlca_layout_arena(C.byref(self.cfg), C.byref(params), C.byref(self._arena), lay.pick,
                                                   C.byref(st), _ptr(status), self._stream()))
         else:
@@ -230,7 +235,8 @@ class StageWorld:
     def relayout_finished(self, stack_out, out=None):
         """After a tick of a random scenario with auto_reset 0 (DESIGN.md §9k), on the env's stream with no
         synchronisation: park the robots whose episode ended (last command 0, `live` 0), give every world whose robots
-        have all ended a new layout (rlca_layout_respawn; rlca_layout_arena_respawn on arenas), scan the new state (rlca_env_observe into the env's own obs /
+        have all ended a new layout (rlca_layout_respawn; rlca_layout_arena_respawn on arenas; with an attached curriculum rlca_layout_arena_weighted_respawn, which
+        first tallies the tick's ended episodes per arena, §9z), scan the new state (rlca_env_observe into the env's own obs /
         gs), and make the re-laid robots' rows of stack_out (N, 3, beams) three copies of the new scan and their
         out['gs'] rows the new local goal and speed (rlca_stack_refresh).  `out` holds the 'flags' and 'gs' buffers the
         tick wrote (default the env's own); re-laid robots get flags[:, 3] (was_reset) = 1.  Pass `live` to the next
@@ -241,7 +247,12 @@ class StageWorld:
         flags, gs = o.get('flags', self.flags), o.get('gs', self.gs)
         st = self._state_struct(self._cur)
         stream = self._stream()
-        if self._arena is not None:
+        if self.curriculum is not None:
+            cur = self.curriculum
+            _lib.check(self.lib.rlca_layout_arena_weighted_respawn(
+                C.byref(self.cfg), C.byref(self._layout_params), C.byref(self._arena), C.byref(cur.struct),
+                _ptr(cur.row_mask), C.byref(st), _ptr(flags), _ptr(self.live), _ptr(self._relayout_status), stream))
+        elif self._arena is not None:
             _lib.check(self.lib.rlca_layout_arena_respawn(C.byref(self.cfg), C.byref(self._layout_params),
                                                           C.byref(self._arena), self.sc.layout.pick, C.byref(st),
                                                           _ptr(flags), _ptr(self.live), _ptr(self._relayout_status),

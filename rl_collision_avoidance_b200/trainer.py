@@ -18,6 +18,7 @@ from .mix import MIX_AUTO_RESET, MIX_SCENARIOS, SLICE_ALIGN, check_aligned
 from .model.ppo import generate_action, generate_train_data, ppo_update_stage1, ppo_update_stage2
 from .model.utils import get_filter_index
 from .crowd import Crowd
+from .curriculum import ArenaCurriculum
 from .dynamics import Dynamics
 from .evaluation import non_cooperative_mask
 from .latency import Latency
@@ -26,6 +27,7 @@ from .noise import Noise
 from .orca import NonCooperative
 from .perturbation import Chain
 from .planner import Planner
+from .scenarios import ArenaLayout
 from .stage_world import RESULT_STRINGS
 
 
@@ -60,6 +62,7 @@ class _Component:
         self.env, self.a, self.b = env, a, b
         self.chain = Chain(env, noise, latency, dynamics, localization)     # attach_planners sets chain.planner
         self.masked = None                              # orca.NonCooperative or crowd.Crowd of the env, or None
+        self.curriculum = None                          # curriculum.ArenaCurriculum of an arena env, or None
         self.ticked = False                             # a tick has run, so self.flags holds its flags
         self.name = env.sc.name
         self.relayout = env.sc.layout is not None
@@ -192,6 +195,25 @@ def masked_agents(comps, non_cooperative=None, crowd=None):
     return np.concatenate(masks) != 0
 
 
+def attach_curricula(comps, params, col_mask=None, state=None):
+    """Give every arena component an ArenaCurriculum with `params` (curriculum.CurriculumParams), the masked columns
+    of its slice of `col_mask` left out of its tallies, and return the curricula; `state` (a state_dict) restores
+    them.  None attaches nothing.  ValueError without an arena component."""
+    if params is None:
+        return []
+    out = []
+    for c in comps:
+        if isinstance(c.env.sc.layout, ArenaLayout):
+            c.curriculum = ArenaCurriculum(c.env, params, None if col_mask is None else col_mask[c.a:c.b])
+            if state is not None:
+                c.curriculum.load_state_dict(state)
+            out.append(c.curriculum)
+    if not out:
+        raise ValueError('an arena curriculum needs an arena scenario or an arena component, got %s'
+                         % ', '.join(c.name for c in comps))
+    return out
+
+
 def masked_rows(H, col_mask):
     """Every row t * N + i of a masked column i, sorted: stage 1's filter."""
     N = col_mask.shape[0]
@@ -229,7 +251,7 @@ def _check_mix(envs, stage):
 def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logger_cal=None, stage=1, max_updates=None,
         process_group=None, rank=0, save_every=20, generator=None, start_update=0, diagnostics=False, target_kl=None,
         noise=None, latency=None, dynamics=None, localization=None, non_cooperative=None, crowd=None, planner=None,
-        planner_tables=None):
+        planner_tables=None, curriculum=None, curriculum_state=None):
     """hp: dict with HORIZON, GAMMA, LAMDA, BATCH_SIZE, EPOCH, COEFF_ENTROPY, CLIP_VALUE, NUM_ENV, OBS_SIZE, ACT_SIZE,
     LASER_HIST, MAX_EPISODES.  `start_update` continues the checkpoint numbering of a resumed run.
     A random scenario (env.sc.layout, DESIGN.md §9k) trains with stage 2's update on per-world layouts: the env runs
@@ -261,6 +283,11 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     the tick's reward.  The stats then also hold 'planner', the status shares of the
     update's robot-ticks.  Refused with localization error and on maps the planner refuses.  None launches nothing.
     `planner_tables` (one planner.PlannerTables per env, in order) saves building the planning graphs again.
+    `curriculum` (curriculum.CurriculumParams, DESIGN.md §9z) gives the arena component an ArenaCurriculum
+    (attach_curricula) before its first layout: its re-layouts tally the episodes of its cooperative rows per arena and
+    draw arenas by the curriculum's weights, which every update refreshes (summed over the ranks under data
+    parallelism).  The stats then also hold 'curriculum' (ArenaCurriculum.stats), and the .trainer checkpoint its state
+    under 'curriculum'; `curriculum_state` (such a state) restores it.  None launches nothing.
     Returns per-update stats (for tests / benchmarks); 'by_scenario' splits the episodes by component."""
     envs = list(env) if isinstance(env, (list, tuple)) else [env]
     if not envs:
@@ -280,6 +307,7 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
     col_mask = masked_agents(comps, non_cooperative, crowd)
     role = 'crowd' if crowd is not None else 'non_cooperative'
     col_comp = np.repeat(np.arange(len(comps)), [e.N for e in envs])     # component of every agent column
+    curricula = attach_curricula(comps, curriculum, col_mask, curriculum_state)
     for c in comps:
         c.start()
     diag = None
@@ -310,6 +338,8 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
         for c in comps:
             if c.relayout:
                 c.env.check_relayout()
+        for cu in curricula:
+            cu.update(process_group)
         memory = (ro.stacks[:H], ro.gs[:H, :, 0:2], ro.gs[:H, :, 2:4], ro.actions, ro.logprobs, t_batch, ro.values,
                   ro.rewards, advs_batch)
         common = dict(policy=policy, optimizer=optimizer, batch_size=hp['BATCH_SIZE'], memory=memory, epoch=hp['EPOCH'],
@@ -357,8 +387,11 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
         if rank == 0 and policy_path and global_update % save_every == 0:
             name = '/Stage1_{}'.format(global_update) if stage == 1 else '/stage2_{}.pth'.format(global_update)
             torch.save(policy.state_dict(), policy_path + name)                      # ppo_stage1.py:122-126
-            torch.save({'optimizer': optimizer.state_dict(), 'update': global_update,
-                        'sample_counter': policy.sample_counter}, policy_path + name + '.trainer')
+            extra = {'optimizer': optimizer.state_dict(), 'update': global_update,
+                     'sample_counter': policy.sample_counter}
+            if curricula:
+                extra['curriculum'] = curricula[0].state_dict()
+            torch.save(extra, policy_path + name + '.trainer')
             if logger is not None:
                 logger.info('########################## model saved when update {} times#########'
                             '################'.format(global_update))
@@ -374,6 +407,8 @@ def run(env, policy, policy_path, action_bound, optimizer, hp, logger=None, logg
             stats[-1]['by_role'] = {'cooperative': _episode_stats(ep[~ep_masked]), role: _episode_stats(ep[ep_masked])}
         if planner is not None:
             stats[-1]['planner'] = _status_shares(comps)
+        if curricula:
+            stats[-1]['curriculum'] = curricula[0].stats()
         if diag is not None:
             stats[-1]['diagnostics'] = diag.metrics()
             if rank == 0:
