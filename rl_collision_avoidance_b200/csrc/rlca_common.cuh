@@ -1,4 +1,5 @@
-// rlca_common.cuh — error plumbing and contract math shared by the translation units of librlca.so.
+// rlca_common.cuh — error plumbing, argument checks, Philox purpose words and contract math shared by the translation
+// units of librlca.so.
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -20,6 +21,53 @@ inline int rlca_set_err(int code, const char *fmt, const char *a = "", const cha
         if (e__ != cudaSuccess)                                                                  \
             return rlca_set_err(RLCA_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e__)); \
     } while (0)
+
+// ------------------------------------------------------------------------------------------------ argument checks
+static inline bool finite_nonneg(float v) { return v >= 0.0f && v < INFINITY; }
+
+// 1 <= robots_per_world <= RLCA_MAX_ROBOTS_PER_WORLD and num_worlds >= 1
+static inline int rlca_check_robots(const rlca_env_config *cfg, const char *who)
+{
+    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: robots_per_world must be in 1..64 and num_worlds >= 1", who);
+    return RLCA_OK;
+}
+
+// worlds world_begin .. world_begin + world_count - 1 of the shard, at least one
+static inline int rlca_check_world_range(const rlca_env_config *cfg, int32_t world_begin, int32_t world_count,
+                                         const char *who)
+{
+    if (world_begin < 0 || world_count < 1 || world_begin > cfg->num_worlds - world_count)
+        return rlca_set_err(RLCA_ERR_INVALID, "%s: world range outside the shard", who);
+    return RLCA_OK;
+}
+
+// the key of a perturbation link's draws: global agents from world_offset * R, and a stream that fits above the
+// purpose byte of link_word
+static inline int rlca_check_link(const rlca_env_config *cfg, uint32_t stream_id, const char *who)
+{
+    if (cfg->world_offset < 0) return rlca_set_err(RLCA_ERR_INVALID, "%s: world_offset must be >= 0", who);
+    if (stream_id >= (1u << 24)) return rlca_set_err(RLCA_ERR_INVALID, "%s: stream_id must be below 2^24", who);
+    return RLCA_OK;
+}
+
+// float64 arithmetic without contraction, so that host, device and numpy round alike
+__host__ __device__ __forceinline__ double d_add(double a, double b)
+{
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+__host__ __device__ __forceinline__ double d_mul(double a, double b)
+{
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
 
 // angle wrap of the numerics contract: at most one step of 2 pi towards (-pi, pi]
 __host__ __device__ __forceinline__ float dev_normalize(float a)
@@ -55,9 +103,49 @@ __host__ __device__ __forceinline__ void dev_philox(uint32_t (&c)[4], uint32_t k
     }
 }
 
-// Four uniforms in [0, 1) (24 bits each) keyed by (seed, agent, episode, draw, purpose).  Purposes: 1 spawn and
-// heading, 2 goal (rlca_env.cu); 3 start, 4 goal, 5 heading of a random layout (rlca_layout.cu).  The action sampler
-// (sample_kernel, rlca_policy.cu) calls dev_philox directly with purpose word 0x5A17 and counter (row, call counter).
+// The purpose words of the project's Philox draws.  Every draw puts its purpose in counter word 3, and all draws may
+// share one seed (the perturbation seeds fall back to the env's), so the purpose is what keeps their streams apart: a
+// new draw takes a new name here.  The perturbation links put their stream above the purpose byte (link_word), so no
+// two words may share their low byte.
+constexpr uint32_t PURPOSE_SPAWN = 0x01u;            // the tick's spawn tries and heading (rlca_env.cu)
+constexpr uint32_t PURPOSE_GOAL = 0x02u;             // the tick's goal tries
+constexpr uint32_t PURPOSE_LAYOUT_START = 0x03u;     // a layout's start tries (rlca_layout.cu)
+constexpr uint32_t PURPOSE_LAYOUT_GOAL = 0x04u;      // a layout's goal tries
+constexpr uint32_t PURPOSE_LAYOUT_HEADING = 0x05u;   // a layout's headings
+constexpr uint32_t PURPOSE_ARENA = 0xA0u;            // an arena's pick, and ORed with the two above for its tries
+constexpr uint32_t PURPOSE_NOISE_RANGE = 0xE1u;      // lidar range noise (rlca_noise.cu)
+constexpr uint32_t PURPOSE_NOISE_DROPOUT = 0xE2u;    // beam dropout
+constexpr uint32_t PURPOSE_NOISE_ACTION = 0xE3u;     // velocity gain error
+constexpr uint32_t PURPOSE_SCAN_DELAY = 0xE4u;       // scan latency (rlca_latency.cu)
+constexpr uint32_t PURPOSE_CMD_DELAY = 0xE5u;        // command latency
+constexpr uint32_t PURPOSE_ACCEL = 0xE6u;            // acceleration limits (rlca_dynamics.cu)
+constexpr uint32_t PURPOSE_POSE_ERROR = 0xE7u;       // localization error (rlca_localization.cu)
+constexpr uint32_t PURPOSE_SAMPLER = 0x5A17u;        // the action sampler (sample_kernel, rlca_policy.cu)
+
+constexpr uint32_t rlca_purpose_words[] = {
+    PURPOSE_SPAWN, PURPOSE_GOAL, PURPOSE_LAYOUT_START, PURPOSE_LAYOUT_GOAL, PURPOSE_LAYOUT_HEADING, PURPOSE_ARENA,
+    PURPOSE_ARENA | PURPOSE_LAYOUT_START, PURPOSE_ARENA | PURPOSE_LAYOUT_GOAL, PURPOSE_NOISE_RANGE,
+    PURPOSE_NOISE_DROPOUT, PURPOSE_NOISE_ACTION, PURPOSE_SCAN_DELAY, PURPOSE_CMD_DELAY, PURPOSE_ACCEL,
+    PURPOSE_POSE_ERROR, PURPOSE_SAMPLER,
+};
+constexpr bool rlca_purpose_bytes_distinct()
+{
+    constexpr int n = sizeof(rlca_purpose_words) / sizeof(rlca_purpose_words[0]);
+    for (int i = 0; i < n; ++i)
+        for (int j = i + 1; j < n; ++j)
+            if ((rlca_purpose_words[i] & 0xFFu) == (rlca_purpose_words[j] & 0xFFu)) return false;
+    return true;
+}
+static_assert(rlca_purpose_bytes_distinct(), "two Philox purpose words share their low byte");
+
+// counter word 3 of a perturbation link's draw: the purpose byte and the link's stream above it
+__host__ __device__ __forceinline__ uint32_t link_word(uint32_t purpose, uint32_t stream)
+{
+    return purpose | (stream << 8);
+}
+
+// Four uniforms in [0, 1) (24 bits each) keyed by (seed, agent, episode, draw, purpose).  The action sampler calls
+// dev_philox directly with counter (row, call counter, PURPOSE_SAMPLER).
 __host__ __device__ __forceinline__ void dev_rand4(uint64_t seed, uint32_t agent, uint32_t episode, uint32_t draw,
                                                    uint32_t purpose, float (&u)[4])
 {

@@ -94,8 +94,7 @@ extern "C" int rlca_demo_append(const rlca_env_config *cfg, const rlca_env_state
                                 const rlca_demo_set *demo, void *stream)
 {
     if (!cfg || !state || !io || !demo) return rlca_set_err(RLCA_ERR_INVALID, "rlca_demo_append: NULL argument");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "cfg has no robots");
+    if (int rc = rlca_check_robots(cfg, "rlca_demo_append")) return rc;
     if (cfg->auto_reset < 0 || cfg->auto_reset > 2) return rlca_set_err(RLCA_ERR_INVALID, "cfg.auto_reset must be 0, 1 or 2");
     if (cfg->beams < 1 || (3 * cfg->beams) % 4 != 0)
         return rlca_set_err(RLCA_ERR_UNSUPPORTED, "rlca_demo_append: 3 * beams must be a multiple of 4");

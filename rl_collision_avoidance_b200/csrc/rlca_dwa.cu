@@ -222,7 +222,6 @@ __global__ void __launch_bounds__(DWA_THREADS)
 
 // ------------------------------------------------------------------------------------------------ entries
 static bool finite_pos(float v) { return v > 0.0f && v < INFINITY; }
-static bool finite_nonneg(float v) { return v >= 0.0f && v < INFINITY; }
 
 static int dwa_args(const rlca_env_config *cfg, const rlca_dwa_params *p, const void *cs, const void *stack,
                     const void *gs, const void *action, const void *status, DwaArgs &q)

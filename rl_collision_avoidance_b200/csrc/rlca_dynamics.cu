@@ -6,9 +6,9 @@
 // launch; the tick's kernels, its config and its outputs are untouched, and a run without limits issues none.
 //
 // The executed velocity and the limits are state across ticks, so this is a file of its own, as latency is.  Every
-// limit is a function of (seed, global agent, draw, 0xE6 | stream << 8) alone, and the rule is one subtraction, one
-// product and one addition per component, built without FMA contraction on either side, so the host twin (a serial
-// loop over the same code) equals the kernel bit for bit at any num_worlds, shard or launch shape.
+// limit is a function of (seed, global agent, draw, PURPOSE_ACCEL | stream << 8) alone, and the rule is one
+// subtraction, one product and one addition per component, built without FMA contraction on either side, so the host
+// twin (a serial loop over the same code) equals the kernel bit for bit at any num_worlds, shard or launch shape.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
@@ -17,7 +17,6 @@
 #include "rlca_common.cuh"
 
 #define DYNAMICS_THREADS 256
-#define PURPOSE_ACCEL 0xE6u
 
 struct DynamicsArgs {
     float lin_lo, lin_span, ang_lo, ang_span;   // limit = lo + span u; (0, 0) for a kind that is off
@@ -48,7 +47,7 @@ __host__ __device__ __forceinline__ float2 dynamics_agent(const DynamicsArgs &q,
 {
     float la, aa;
     if (fresh) {
-        uint32_t c[4] = {q.agent0 + (uint32_t)a, q.draw, 0u, PURPOSE_ACCEL | (q.stream << 8)};
+        uint32_t c[4] = {q.agent0 + (uint32_t)a, q.draw, 0u, link_word(PURPOSE_ACCEL, q.stream)};
         dev_philox(c, q.k0, q.k1);
         la = q.lin_lo + q.lin_span * ((float)(c[0] >> 8) * 5.9604644775390625e-08f);
         aa = q.ang_lo + q.ang_span * ((float)(c[1] >> 8) * 5.9604644775390625e-08f);
@@ -99,13 +98,11 @@ static int dynamics_args(const rlca_env_config *cfg, const rlca_dynamics_params 
     if (!st->vel || !st->lin_limit || !st->ang_limit)
         return rlca_set_err(RLCA_ERR_INVALID, "dynamics: state vel, lin_limit or ang_limit is NULL");
     if (!in || !out) return rlca_set_err(RLCA_ERR_INVALID, "dynamics: action_in or action_out is NULL");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "dynamics: robots_per_world must be in 1..64 and num_worlds >= 1");
-    if (cfg->world_offset < 0) return rlca_set_err(RLCA_ERR_INVALID, "dynamics: world_offset must be >= 0");
+    if (int rc = rlca_check_robots(cfg, "dynamics")) return rc;
+    if (int rc = rlca_check_link(cfg, p->stream_id, "dynamics")) return rc;
     if (!accel_range_ok(p->lin_lo, p->lin_hi) || !accel_range_ok(p->ang_lo, p->ang_hi))
         return rlca_set_err(RLCA_ERR_INVALID, "dynamics: every limit range must be (0, 0) or finite with "
                                               "0 < lo <= hi <= 100");
-    if (p->stream_id >= (1u << 24)) return rlca_set_err(RLCA_ERR_INVALID, "dynamics: stream_id must be below 2^24");
     q.lin_lo = p->lin_lo;
     q.lin_span = p->lin_hi - p->lin_lo;
     q.ang_lo = p->ang_lo;

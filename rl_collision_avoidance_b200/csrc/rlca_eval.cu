@@ -19,23 +19,6 @@
 
 #define EVAL_THREADS 128
 
-// float64 arithmetic without contraction, so that host and device (and numpy) round alike
-__host__ __device__ __forceinline__ double d_add(double a, double b)
-{
-#ifdef __CUDA_ARCH__
-    return __dadd_rn(a, b);
-#else
-    return a + b;
-#endif
-}
-__host__ __device__ __forceinline__ double d_mul(double a, double b)
-{
-#ifdef __CUDA_ARCH__
-    return __dmul_rn(a, b);
-#else
-    return a * b;
-#endif
-}
 __host__ __device__ __forceinline__ double d_hypot(double dx, double dy)
 {
     return sqrt(d_add(d_mul(dx, dx), d_mul(dy, dy)));      // sqrt is correctly rounded on both sides
@@ -150,17 +133,9 @@ __global__ void __launch_bounds__(EVAL_THREADS) eval_reduce_split_kernel(int R, 
 static int check_cfg(const rlca_env_config *cfg, int32_t episodes)
 {
     if (!cfg) return rlca_set_err(RLCA_ERR_INVALID, "cfg is NULL");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "cfg has no robots");
+    if (int rc = rlca_check_robots(cfg, "eval")) return rc;
     if (episodes < 1) return rlca_set_err(RLCA_ERR_INVALID, "episodes must be >= 1");
     if (!(cfg->dt > 0.0f) || !(cfg->v_max > 0.0f)) return rlca_set_err(RLCA_ERR_INVALID, "cfg needs dt > 0 and v_max > 0");
-    return RLCA_OK;
-}
-
-static int check_range(const rlca_env_config *cfg, int32_t world_begin, int32_t world_count)
-{
-    if (world_begin < 0 || world_count < 1 || world_begin > cfg->num_worlds - world_count)
-        return rlca_set_err(RLCA_ERR_INVALID, "world range outside the shard");
     return RLCA_OK;
 }
 
@@ -191,7 +166,7 @@ extern "C" int rlca_eval_reduce(const rlca_env_config *cfg, const rlca_eval_stat
 {
     int rc = check_cfg(cfg, ev ? ev->episodes : 0);
     if (rc) return rc;
-    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if ((rc = rlca_check_world_range(cfg, world_begin, world_count, "eval"))) return rc;
     if (!ev->count_dev || !ev->open_dev || !ev->records_dev || !partials_dev)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_eval_reduce: a buffer is NULL");
     eval_reduce_kernel<<<(world_count + EVAL_THREADS - 1) / EVAL_THREADS, EVAL_THREADS, 0, (cudaStream_t)stream>>>(
@@ -208,7 +183,7 @@ extern "C" int rlca_eval_reduce_host(const rlca_env_config *cfg, const float *re
 {
     int rc = check_cfg(cfg, episodes);
     if (rc) return rc;
-    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if ((rc = rlca_check_world_range(cfg, world_begin, world_count, "eval"))) return rc;
     if (!records_host || !count_host || !open_host || !partials_host)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_eval_reduce_host: a buffer is NULL");
     for (int i = 0; i < world_count; ++i)
@@ -223,7 +198,7 @@ extern "C" int rlca_eval_reduce_split(const rlca_env_config *cfg, const rlca_eva
 {
     int rc = check_cfg(cfg, ev ? ev->episodes : 0);
     if (rc) return rc;
-    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if ((rc = rlca_check_world_range(cfg, world_begin, world_count, "eval"))) return rc;
     if (!ev->count_dev || !ev->open_dev || !ev->records_dev || !mask_dev || !partials_dev)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_eval_reduce_split: a buffer is NULL");
     eval_reduce_split_kernel<<<(2 * world_count + EVAL_THREADS - 1) / EVAL_THREADS, EVAL_THREADS, 0,
@@ -242,7 +217,7 @@ extern "C" int rlca_eval_reduce_split_host(const rlca_env_config *cfg, const flo
 {
     int rc = check_cfg(cfg, episodes);
     if (rc) return rc;
-    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if ((rc = rlca_check_world_range(cfg, world_begin, world_count, "eval"))) return rc;
     if (!records_host || !count_host || !open_host || !mask_host || !partials_host)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_eval_reduce_split_host: a buffer is NULL");
     for (int i = 0; i < 2 * world_count; ++i)

@@ -17,8 +17,6 @@
 #include "rlca_common.cuh"
 
 #define LATENCY_THREADS 256
-#define PURPOSE_SCAN_DELAY 0xE4u
-#define PURPOSE_CMD_DELAY 0xE5u
 
 struct LatencyArgs {
     uint32_t k0, k1, stream, draw, agent0;  // agent0: global index of row 0, world_offset * R
@@ -32,7 +30,7 @@ struct LatencyArgs {
 // (agent, draw, 0, purpose | stream << 8)
 __host__ __device__ __forceinline__ uint8_t latency_delay(const LatencyArgs &q, uint32_t agent, uint32_t purpose)
 {
-    uint32_t c[4] = {agent, q.draw, 0u, purpose | (q.stream << 8)};
+    uint32_t c[4] = {agent, q.draw, 0u, link_word(purpose, q.stream)};
     dev_philox(c, q.k0, q.k1);
     return (uint8_t)(q.lo + (uint32_t)(((uint64_t)q.span * (uint64_t)c[0]) >> 32));
 }
@@ -128,13 +126,11 @@ static int latency_args(const rlca_env_config *cfg, const rlca_latency_params *p
                         bool scan, uint32_t draw, LatencyArgs &q)
 {
     if (!cfg || !p || !st) return rlca_set_err(RLCA_ERR_INVALID, "latency: cfg, params or state is NULL");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "latency: robots_per_world must be in 1..64 and num_worlds >= 1");
-    if (cfg->beams < 1 || cfg->world_offset < 0)
-        return rlca_set_err(RLCA_ERR_INVALID, "latency: beams must be >= 1 and world_offset >= 0");
+    if (int rc = rlca_check_robots(cfg, "latency")) return rc;
+    if (cfg->beams < 1) return rlca_set_err(RLCA_ERR_INVALID, "latency: beams must be >= 1");
+    if (int rc = rlca_check_link(cfg, p->stream_id, "latency")) return rc;
     if (!delay_range_ok(p->scan_lo, p->scan_hi) || !delay_range_ok(p->cmd_lo, p->cmd_hi))
         return rlca_set_err(RLCA_ERR_INVALID, "latency: every delay range must satisfy 0 <= lo <= hi <= 8 ticks");
-    if (p->stream_id >= (1u << 24)) return rlca_set_err(RLCA_ERR_INVALID, "latency: stream_id must be below 2^24");
     const int32_t lo = scan ? p->scan_lo : p->cmd_lo, hi = scan ? p->scan_hi : p->cmd_hi;
     if (hi > 0 && (scan ? (!st->scan_ring || !st->scan_delay) : (!st->cmd_ring || !st->cmd_delay)))
         return rlca_set_err(RLCA_ERR_INVALID, scan ? "latency: scan_ring or scan_delay is NULL"

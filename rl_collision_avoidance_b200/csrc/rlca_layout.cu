@@ -7,8 +7,8 @@
 // uniform in the square [-side/2, side/2]^2, is at least `separation` from the starts placed so far; the goal the
 // first try whose draw is at least `min_travel` from this start and `separation` from the goals placed so far; the
 // heading one draw u * 2 pi, wrapped as the env's spawn wraps it.  Draws use the env's Philox keys with agent =
-// global world * R + r, episode 0, draw k and purposes 3 (start), 4 (goal), 5 (heading), so a world's layout depends
-// only on (seed, global world, R, parameters, max_reject).
+// global world * R + r, episode 0, draw k and the layout purposes of rlca_common.cuh (start, goal, heading), so a
+// world's layout depends only on (seed, global world, R, parameters, max_reject).
 //
 // Distances are compared squared, and draws and tests use plain float32 + - x (this file is compiled with
 // -fmad=false on the device and -ffp-contract=off on the host), so rlca_layout_random_host gives the same bits.
@@ -43,7 +43,7 @@ struct LayoutConsts {
     uint32_t episode;        // Philox episode counter of the draws: 0 for rlca_layout_random, meta.y + 1 for a re-layout
 };
 
-// try k of robot r's start (purpose 3) or goal (purpose 4): uniform in the square, one rounding per coordinate
+// try k of robot r's start or goal: uniform in the square, one rounding per coordinate
 // ((u - 0.5) is exact for the 24-bit uniforms)
 __host__ __device__ __forceinline__ void layout_draw(const LayoutConsts &c, uint32_t r, uint32_t k, uint32_t purpose,
                                                      float &x, float &y)
@@ -57,7 +57,7 @@ __host__ __device__ __forceinline__ void layout_draw(const LayoutConsts &c, uint
 __host__ __device__ __forceinline__ float layout_heading(const LayoutConsts &c, uint32_t r)
 {
     float u[4];
-    dev_rand4(c.seed, c.agent0 + r, c.episode, 0u, 5u, u);
+    dev_rand4(c.seed, c.agent0 + r, c.episode, 0u, PURPOSE_LAYOUT_HEADING, u);
     return dev_normalize(u[0] * 6.28318548202514648438f);
 }
 
@@ -101,7 +101,7 @@ struct LayoutSmem {
     float gx[RLCA_MAX_ROBOTS_PER_WORLD], gy[RLCA_MAX_ROBOTS_PER_WORLD];
 };
 
-// The draws of the square (rlca_layout_random): try k of robot r at purpose 3 (start) or 4 (goal).
+// The draws of the square (rlca_layout_random): try k of robot r at the start or goal purpose.
 struct SquareDraw {
     __host__ __device__ __forceinline__ void operator()(const LayoutConsts &c, uint32_t r, uint32_t k, uint32_t purpose,
                                                         float &x, float &y) const
@@ -110,7 +110,7 @@ struct SquareDraw {
     }
 };
 
-// The first accepted try of robot r (purpose 3: start, 4: goal) by the whole warp; false when none of the budget is.
+// The first accepted try of robot r (start or goal purpose) by the whole warp; false when none of the budget is.
 template <class Draw>
 __device__ __forceinline__ bool warp_place(const Draw &draw, const LayoutConsts &c, const LayoutSmem &s, int r,
                                            uint32_t purpose, int max_reject, int lane, float &ox, float &oy)
@@ -121,7 +121,7 @@ __device__ __forceinline__ bool warp_place(const Draw &draw, const LayoutConsts 
         bool ok = false;
         if (k < max_reject) {
             draw(c, (uint32_t)r, (uint32_t)k, purpose, x, y);
-            ok = purpose == 3u ? start_ok(c, s.sx, s.sy, r, x, y) : goal_ok(c, s.gx, s.gy, r, s.sx[r], s.sy[r], x, y);
+            ok = purpose == PURPOSE_LAYOUT_START ? start_ok(c, s.sx, s.sy, r, x, y) : goal_ok(c, s.gx, s.gy, r, s.sx[r], s.sy[r], x, y);
         }
         const uint32_t mask = __ballot_sync(0xffffffffu, ok);
         if (mask) {
@@ -143,13 +143,13 @@ __device__ __forceinline__ bool warp_layout(const Draw &draw, const LayoutConsts
 {
     for (int r = 0; r < R; ++r) {
         float x, y, gx, gy;
-        if (!warp_place(draw, c, s, r, 3u, max_reject, lane, x, y)) {
+        if (!warp_place(draw, c, s, r, PURPOSE_LAYOUT_START, max_reject, lane, x, y)) {
             if (lane == 0) *status = 1 + r;
             return false;
         }
         if (lane == 0) { s.sx[r] = x; s.sy[r] = y; }
         __syncwarp();
-        if (!warp_place(draw, c, s, r, 4u, max_reject, lane, gx, gy)) {
+        if (!warp_place(draw, c, s, r, PURPOSE_LAYOUT_GOAL, max_reject, lane, gx, gy)) {
             if (lane == 0) *status = 1 + r;
             return false;
         }
@@ -167,12 +167,12 @@ inline int host_layout(const Draw &draw, const LayoutConsts &c, int R, int max_r
     for (int r = 0; r < R; ++r) {
         int k = 0;
         for (; k < max_reject; ++k) {
-            draw(c, (uint32_t)r, (uint32_t)k, 3u, sx[r], sy[r]);
+            draw(c, (uint32_t)r, (uint32_t)k, PURPOSE_LAYOUT_START, sx[r], sy[r]);
             if (start_ok(c, sx, sy, r, sx[r], sy[r])) break;
         }
         if (k == max_reject) return 1 + r;
         for (k = 0; k < max_reject; ++k) {
-            draw(c, (uint32_t)r, (uint32_t)k, 4u, gx[r], gy[r]);
+            draw(c, (uint32_t)r, (uint32_t)k, PURPOSE_LAYOUT_GOAL, gx[r], gy[r]);
             if (goal_ok(c, gx, gy, r, sx[r], sy[r], gx[r], gy[r])) break;
         }
         if (k == max_reject) return 1 + r;
@@ -193,13 +193,13 @@ rlca_layout_random_kernel(int num_worlds, int R, int max_reject, int pre_distanc
     const LayoutConsts c = { seed, (uint32_t)(world_offset + w) * (uint32_t)R, side, sep2, travel2, 0u };
     for (int r = 0; r < R; ++r) {
         float x, y, gx, gy;
-        if (!warp_place(SquareDraw(), c, s, r, 3u, max_reject, lane, x, y)) {
+        if (!warp_place(SquareDraw(), c, s, r, PURPOSE_LAYOUT_START, max_reject, lane, x, y)) {
             if (lane == 0) status[w] = 1 + r;
             return;
         }
         if (lane == 0) { s.sx[r] = x; s.sy[r] = y; }
         __syncwarp();
-        if (!warp_place(SquareDraw(), c, s, r, 4u, max_reject, lane, gx, gy)) {
+        if (!warp_place(SquareDraw(), c, s, r, PURPOSE_LAYOUT_GOAL, max_reject, lane, gx, gy)) {
             if (lane == 0) status[w] = 1 + r;
             return;
         }
@@ -298,10 +298,6 @@ rlca_layout_respawn_kernel(int num_worlds, int R, int max_reject, int pre_distan
 }
 
 // ---------------------------------------------------------------------------------------------- arenas (§9v)
-// The arena of a world with pick 1 is drawn at purpose 0xA0, try k of a start or goal at 0xA0 | 3 and 0xA0 | 4: bytes
-// no other draw of the project uses (the env 1 - 5, the noise chain 0xE1 - 0xE7, the sampler's word 0x5A17).
-#define PURPOSE_ARENA 0xA0u
-
 // Try k of robot r in one arena: a uniform cell of the arena's list, then a uniform point of that cell.
 struct ArenaDraw {
     const int32_t *cells;    // the arena's cells, cx | cy << 16
@@ -806,8 +802,7 @@ extern "C" int rlca_stack_refresh(const rlca_env_config *cfg, const uint8_t *fla
                                   const float *gs_src_dev, float *stack_dev, float *gs_dev, void *stream)
 {
     if (!cfg) return rlca_set_err(RLCA_ERR_INVALID, "rlca_stack_refresh: cfg is NULL");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "rlca_stack_refresh: cfg has no robots");
+    if (int rc = rlca_check_robots(cfg, "rlca_stack_refresh")) return rc;
     if (cfg->beams < 1 || (3 * cfg->beams) % 4 != 0)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_stack_refresh: 3 * beams must be a multiple of 4");
     if (!flags_dev || !obs_dev || !gs_src_dev || !stack_dev || !gs_dev)

@@ -8,10 +8,10 @@
 // its outputs are untouched, and a run without localization error issues none.
 //
 // The error and its standard deviations are state across ticks, so this is a file of its own, as latency and dynamics
-// are.  Every draw is a function of (seed, global agent, draw, group, 0xE7 | stream << 8) alone; the local goal is the
-// tick's own goal_speed and dev_sincosf, Box-Muller is noise's, and the file is built without FMA contraction on either
-// side, so the host twin (a serial loop over the same code) equals the kernel bit for bit at any num_worlds, shard or
-// launch shape.
+// are.  Every draw is a function of (seed, global agent, draw, group, PURPOSE_POSE_ERROR | stream << 8) alone; the
+// local goal is the tick's own goal_speed and dev_sincosf, Box-Muller is noise's, and the file is built without FMA
+// contraction on either side, so the host twin (a serial loop over the same code) equals the kernel bit for bit at any
+// num_worlds, shard or launch shape.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
@@ -20,7 +20,6 @@
 #include "rlca_common.cuh"
 
 #define LOCALIZATION_THREADS 256
-#define PURPOSE_POSE_ERROR 0xE7u
 
 struct LocalizationArgs {
     float xy_lo, xy_span, th_lo, th_span;       // sigma = lo + span u
@@ -43,7 +42,7 @@ __host__ __device__ __forceinline__ float4 localization_agent(const Localization
                                                               float4 pose, float4 goal, float4 gs, float4 *err,
                                                               float2 *sigma)
 {
-    const uint32_t agent = q.agent0 + (uint32_t)a, purpose = PURPOSE_POSE_ERROR | (q.stream << 8);
+    const uint32_t agent = q.agent0 + (uint32_t)a, purpose = link_word(PURPOSE_POSE_ERROR, q.stream);
     uint32_t c0[4] = {agent, q.draw, 0u, purpose}, c1[4] = {agent, q.draw, 1u, purpose};
     dev_philox(c0, q.k0, q.k1);
     dev_philox(c1, q.k0, q.k1);
@@ -90,8 +89,6 @@ __global__ void __launch_bounds__(LOCALIZATION_THREADS)
 }
 
 // ------------------------------------------------------------------------------------------------ entries
-static bool finite_nonneg(float v) { return v >= 0.0f && v < INFINITY; }
-
 static int localization_args(const rlca_env_config *cfg, const rlca_localization_params *p,
                              const rlca_localization_state *st, uint32_t draw, const rlca_env_state *env,
                              const float *gs_in, const float *gs_out, LocalizationArgs &q)
@@ -101,16 +98,14 @@ static int localization_args(const rlca_env_config *cfg, const rlca_localization
     if (!env->pose_dev || !env->goal_dev)
         return rlca_set_err(RLCA_ERR_INVALID, "localization: env state pose or goal is NULL");
     if (!gs_in || !gs_out) return rlca_set_err(RLCA_ERR_INVALID, "localization: gs_in or gs_out is NULL");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "localization: robots_per_world must be in 1..64 and num_worlds >= 1");
-    if (cfg->world_offset < 0) return rlca_set_err(RLCA_ERR_INVALID, "localization: world_offset must be >= 0");
+    if (int rc = rlca_check_robots(cfg, "localization")) return rc;
+    if (int rc = rlca_check_link(cfg, p->stream_id, "localization")) return rc;
     if (!finite_nonneg(p->xy_lo) || !finite_nonneg(p->xy_hi) || !(p->xy_lo <= p->xy_hi) ||
         !finite_nonneg(p->theta_lo) || !finite_nonneg(p->theta_hi) || !(p->theta_lo <= p->theta_hi))
         return rlca_set_err(RLCA_ERR_INVALID, "localization: every sigma range must be finite with 0 <= lo <= hi");
     if (!finite_nonneg(p->v_sigma) || !finite_nonneg(p->w_sigma))
         return rlca_set_err(RLCA_ERR_INVALID, "localization: v_sigma and w_sigma must be finite and >= 0");
     if (!(p->tau >= 0.0f)) return rlca_set_err(RLCA_ERR_INVALID, "localization: tau must be >= 0 or +inf");
-    if (p->stream_id >= (1u << 24)) return rlca_set_err(RLCA_ERR_INVALID, "localization: stream_id must be below 2^24");
     // rho = exp(-dt / tau) and kappa = sqrt(1 - rho^2), once here in double: the kernel and the twin share the floats
     double rho = 0.0, kappa = 1.0;
     if (p->tau == INFINITY) {

@@ -17,9 +17,6 @@
 #include "rlca_common.cuh"
 
 #define NOISE_THREADS 256
-#define PURPOSE_RANGE 0xE1u
-#define PURPOSE_DROPOUT 0xE2u
-#define PURPOSE_ACTION 0xE3u
 
 struct NoiseArgs {
     float range_sigma, dropout, v_sigma, w_sigma;
@@ -37,7 +34,7 @@ __host__ __device__ __forceinline__ void noise_words(const NoiseArgs &q, uint32_
     c[0] = agent;
     c[1] = q.draw;
     c[2] = group;
-    c[3] = purpose | (q.stream << 8);
+    c[3] = link_word(purpose, q.stream);
     dev_philox(c, q.k0, q.k1);
 }
 
@@ -47,14 +44,14 @@ __host__ __device__ __forceinline__ void group_draws(const NoiseArgs &q, uint32_
 {
     uint32_t c[4];
     if (q.range_sigma > 0.0f) {
-        noise_words(q, agent, g, PURPOSE_RANGE, c);
+        noise_words(q, agent, g, PURPOSE_NOISE_RANGE, c);
         box_muller(c[0], c[1], z[0], z[1]);
         box_muller(c[2], c[3], z[2], z[3]);
     } else {
         z[0] = z[1] = z[2] = z[3] = 0.0f;
     }
     if (q.dropout > 0.0f) {
-        noise_words(q, agent, g, PURPOSE_DROPOUT, c);
+        noise_words(q, agent, g, PURPOSE_NOISE_DROPOUT, c);
 #pragma unroll
         for (int j = 0; j < 4; ++j) u[j] = (float)(c[j] >> 8) * 5.9604644775390625e-08f;
     } else {
@@ -87,7 +84,7 @@ __host__ __device__ __forceinline__ void noise_command(const NoiseArgs &q, uint3
     w = clip(w, q.w_min, q.w_max);
     if (q.v_sigma > 0.0f || q.w_sigma > 0.0f) {
         uint32_t c[4];
-        noise_words(q, agent, 0u, PURPOSE_ACTION, c);
+        noise_words(q, agent, 0u, PURPOSE_NOISE_ACTION, c);
         float z1, z2;
         box_muller(c[0], c[1], z1, z2);
         v = clip(v * fmaxf(fmaf(q.v_sigma, z1, 1.0f), 0.0f), q.v_min, q.v_max);
@@ -157,20 +154,16 @@ __global__ void __launch_bounds__(NOISE_THREADS) rlca_noise_action_kernel(NoiseA
 }
 
 // ------------------------------------------------------------------------------------------------ entries
-static bool finite_nonneg(float v) { return v >= 0.0f && v < INFINITY; }
-
 static int noise_args(const rlca_env_config *cfg, const rlca_noise_params *p, uint32_t draw, NoiseArgs &q)
 {
     if (!cfg || !p) return rlca_set_err(RLCA_ERR_INVALID, "noise: cfg or params is NULL");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "noise: robots_per_world must be in 1..64 and num_worlds >= 1");
-    if (cfg->beams < 1 || cfg->world_offset < 0)
-        return rlca_set_err(RLCA_ERR_INVALID, "noise: beams must be >= 1 and world_offset >= 0");
+    if (int rc = rlca_check_robots(cfg, "noise")) return rc;
+    if (cfg->beams < 1) return rlca_set_err(RLCA_ERR_INVALID, "noise: beams must be >= 1");
+    if (int rc = rlca_check_link(cfg, p->stream_id, "noise")) return rc;
     if (!finite_nonneg(p->range_sigma) || !finite_nonneg(p->v_gain_sigma) || !finite_nonneg(p->w_gain_sigma))
         return rlca_set_err(RLCA_ERR_INVALID, "noise: range_sigma, v_gain_sigma and w_gain_sigma must be finite and >= 0");
     if (!(p->dropout >= 0.0f && p->dropout <= 1.0f))
         return rlca_set_err(RLCA_ERR_INVALID, "noise: dropout must be in [0, 1]");
-    if (p->stream_id >= (1u << 24)) return rlca_set_err(RLCA_ERR_INVALID, "noise: stream_id must be below 2^24");
     q.range_sigma = p->range_sigma;
     q.dropout = p->dropout;
     q.v_sigma = p->v_gain_sigma;

@@ -707,8 +707,7 @@ static int check_args(const rlca_env_config *cfg, float radius, float neighbour_
                       float heading_gain, OrcaParams &q)
 {
     if (!cfg) return rlca_set_err(RLCA_ERR_INVALID, "cfg is NULL");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "cfg has no robots");
+    if (int rc = rlca_check_robots(cfg, "orca")) return rc;
     if (!(cfg->dt > 0.0f) || !(cfg->v_max > 0.0f)) return rlca_set_err(RLCA_ERR_INVALID, "cfg needs dt > 0 and v_max > 0");
     const float ps[4] = {radius, neighbour_dist, time_horizon, heading_gain};
     for (float p : ps)

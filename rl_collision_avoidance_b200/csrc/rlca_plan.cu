@@ -520,23 +520,6 @@ __global__ void __launch_bounds__(TRACK_THREADS) rlca_plan_track_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------ reduction
-__host__ __device__ __forceinline__ double d_add(double a, double b)
-{
-#ifdef __CUDA_ARCH__
-    return __dadd_rn(a, b);
-#else
-    return a + b;
-#endif
-}
-__host__ __device__ __forceinline__ double d_mul(double a, double b)
-{
-#ifdef __CUDA_ARCH__
-    return __dmul_rn(a, b);
-#else
-    return a * b;
-#endif
-}
-
 // Partials of world w, layout RLCA_PLAN_* of include/rlca.h; with a mask only the agents whose (mask != 0) equals want
 __host__ __device__ inline void plan_reduce_world(int R, int episodes, double goal_radius, const float *geo,
                                                   const float4 *erec, const int32_t *count, int w, const uint8_t *mask,
@@ -585,8 +568,7 @@ static int plan_args(const char *who, const rlca_env_config *cfg, const rlca_pla
                      PlanMap &m)
 {
     if (!cfg || !t || !ps) return rlca_set_err(RLCA_ERR_INVALID, "%s: cfg, tables or plan state is NULL", who);
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "%s: robots_per_world must be in 1..64 and num_worlds >= 1", who);
+    if (int rc = rlca_check_robots(cfg, who)) return rc;
     if (cfg->grid_w < 1 || cfg->grid_h < 1 || !(cfg->ppm > 0.0f) || !(cfg->resolution > 0.0f))
         return rlca_set_err(RLCA_ERR_INVALID, "%s: the config has no map", who);
     if (t->num_components < 1 || t->max_area < 1 || t->max_area > RLCA_PLAN_MAX_CELLS || !t->label || !t->rects)
@@ -870,12 +852,9 @@ static int reduce_args(const char *who, const rlca_env_config *cfg, int32_t epis
                        int32_t world_count)
 {
     if (!cfg) return rlca_set_err(RLCA_ERR_INVALID, "%s: cfg is NULL", who);
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "%s: robots_per_world must be in 1..64 and num_worlds >= 1", who);
+    if (int rc = rlca_check_robots(cfg, who)) return rc;
     if (episodes < 1) return rlca_set_err(RLCA_ERR_INVALID, "%s: episodes must be >= 1", who);
-    if (world_begin < 0 || world_count < 1 || world_begin > cfg->num_worlds - world_count)
-        return rlca_set_err(RLCA_ERR_INVALID, "%s: world range outside the shard", who);
-    return RLCA_OK;
+    return rlca_check_world_range(cfg, world_begin, world_count, who);
 }
 
 static int plan_reduce_launch(const char *who, const rlca_env_config *cfg, const rlca_plan_state *ps,

@@ -789,7 +789,7 @@ __global__ void sample_kernel(const float *__restrict__ logstd, const float *__r
     float a0 = m0, a1 = m1;
     if (deterministic == 2) { a0 = action[2 * i]; a1 = action[2 * i + 1]; }   // evaluate a given action
     if (!deterministic) {
-        uint32_t c[4] = {(uint32_t)i, (uint32_t)counter, (uint32_t)(counter >> 32), 0x5A17u};
+        uint32_t c[4] = {(uint32_t)i, (uint32_t)counter, (uint32_t)(counter >> 32), PURPOSE_SAMPLER};
         dev_philox(c, (uint32_t)seed, (uint32_t)(seed >> 32));
         // Box-Muller on two 24-bit uniforms in (0,1]
         const float u1 = ((float)(c[0] >> 8) + 1.0f) * 5.9604644775390625e-08f;

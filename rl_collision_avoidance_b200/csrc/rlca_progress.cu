@@ -124,24 +124,6 @@ __global__ void __launch_bounds__(PROGRESS_THREADS) rlca_progress_track_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------ reduction
-// float64 arithmetic without contraction, so that host, device and numpy round alike
-__host__ __device__ __forceinline__ double d_add(double a, double b)
-{
-#ifdef __CUDA_ARCH__
-    return __dadd_rn(a, b);
-#else
-    return a + b;
-#endif
-}
-__host__ __device__ __forceinline__ double d_mul(double a, double b)
-{
-#ifdef __CUDA_ARCH__
-    return __dmul_rn(a, b);
-#else
-    return a * b;
-#endif
-}
-
 // the seven columns of one group (time-outs at base 0, unfinished episodes at base 7) for one episode.  The cause
 // columns add 1 or 0 (exact either way), so that every index is a constant and the partials stay in registers.
 __host__ __device__ __forceinline__ void tally(double *s, int base, int cause, float closest, bool folded)
@@ -211,14 +193,11 @@ __global__ void __launch_bounds__(REDUCE_THREADS) rlca_progress_reduce_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------ entries
-static bool finite_nonneg(float v) { return v >= 0.0f && v < INFINITY; }
-
 static int progress_args(const rlca_env_config *cfg, const rlca_progress_params *p, int32_t episodes,
                          ProgressParams &q)
 {
     if (!cfg || !p) return rlca_set_err(RLCA_ERR_INVALID, "progress: cfg or params is NULL");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "progress: robots_per_world must be in 1..64 and num_worlds >= 1");
+    if (int rc = rlca_check_robots(cfg, "progress")) return rc;
     if (episodes < 1) return rlca_set_err(RLCA_ERR_INVALID, "progress: episodes must be >= 1");
     if (p->window < 1) return rlca_set_err(RLCA_ERR_INVALID, "progress: window must be >= 1");
     if (!finite_nonneg(p->progress_dist) || !finite_nonneg(p->still_dist) || !finite_nonneg(p->block_dist))
@@ -230,13 +209,6 @@ static int progress_args(const rlca_env_config *cfg, const rlca_progress_params 
     q.window = p->window;
     q.R = cfg->robots_per_world;
     q.episodes = episodes;
-    return RLCA_OK;
-}
-
-static int check_range(const rlca_env_config *cfg, int32_t world_begin, int32_t world_count)
-{
-    if (world_begin < 0 || world_count < 1 || world_begin > cfg->num_worlds - world_count)
-        return rlca_set_err(RLCA_ERR_INVALID, "progress: world range outside the shard");
     return RLCA_OK;
 }
 
@@ -311,7 +283,7 @@ extern "C" int rlca_progress_reduce(const rlca_env_config *cfg, const rlca_progr
     ProgressParams q;
     int rc = progress_args(cfg, params, ps ? ps->episodes : 0, q);
     if (rc) return rc;
-    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if ((rc = rlca_check_world_range(cfg, world_begin, world_count, "progress"))) return rc;
     if (!ev) return rlca_set_err(RLCA_ERR_INVALID, "rlca_progress_reduce: eval state is NULL");
     if (ev->episodes != ps->episodes)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_progress_reduce: the tracker holds a different number of episodes");
@@ -339,7 +311,7 @@ extern "C" int rlca_progress_reduce_host(const rlca_env_config *cfg, const rlca_
     ProgressParams q;
     int rc = progress_args(cfg, params, episodes, q);
     if (rc) return rc;
-    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if ((rc = rlca_check_world_range(cfg, world_begin, world_count, "progress"))) return rc;
     if (!progress_records_host || !causes_host || !running_host || !counters_host || !eval_records_host ||
         !count_host || !open_host || !partials_host)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_progress_reduce_host: a buffer is NULL");

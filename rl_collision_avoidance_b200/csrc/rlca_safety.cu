@@ -266,24 +266,6 @@ __global__ void __launch_bounds__(SAFETY_THREADS) rlca_safety_track_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------ reduction
-// float64 arithmetic without contraction, so that host, device and numpy round alike
-__host__ __device__ __forceinline__ double d_add(double a, double b)
-{
-#ifdef __CUDA_ARCH__
-    return __dadd_rn(a, b);
-#else
-    return a + b;
-#endif
-}
-__host__ __device__ __forceinline__ double d_mul(double a, double b)
-{
-#ifdef __CUDA_ARCH__
-    return __dmul_rn(a, b);
-#else
-    return a * b;
-#endif
-}
-
 // Partials of world w, layout RLCA_SAFETY_* of include/rlca.h.  `split`: only the agents whose (mask != 0) equals
 // `want` count.  erec are the tracker's records (result code in .x), srec this file's.
 __host__ __device__ inline void safety_reduce_world(int R, int episodes, const float4 *srec, const float4 *erec,
@@ -345,8 +327,7 @@ __global__ void __launch_bounds__(REDUCE_THREADS) rlca_safety_reduce_kernel(int 
 static int safety_args(const rlca_env_config *cfg, const rlca_safety_params *p, int32_t episodes, SafetyParams &q)
 {
     if (!cfg || !p) return rlca_set_err(RLCA_ERR_INVALID, "safety: cfg or params is NULL");
-    if (cfg->robots_per_world < 1 || cfg->robots_per_world > RLCA_MAX_ROBOTS_PER_WORLD || cfg->num_worlds < 1)
-        return rlca_set_err(RLCA_ERR_INVALID, "safety: robots_per_world must be in 1..64 and num_worlds >= 1");
+    if (int rc = rlca_check_robots(cfg, "safety")) return rc;
     if (cfg->beams < 1) return rlca_set_err(RLCA_ERR_INVALID, "safety: cfg has no beams");
     if (episodes < 1) return rlca_set_err(RLCA_ERR_INVALID, "safety: episodes must be >= 1");
     if (!(p->near_dist >= 0.0f && p->near_dist < INFINITY))
@@ -365,13 +346,6 @@ static int safety_args(const rlca_env_config *cfg, const rlca_safety_params *p, 
     q.R = cfg->robots_per_world;
     q.beams = cfg->beams;
     q.episodes = episodes;
-    return RLCA_OK;
-}
-
-static int check_range(const rlca_env_config *cfg, int32_t world_begin, int32_t world_count)
-{
-    if (world_begin < 0 || world_count < 1 || world_begin > cfg->num_worlds - world_count)
-        return rlca_set_err(RLCA_ERR_INVALID, "safety: world range outside the shard");
     return RLCA_OK;
 }
 
@@ -500,7 +474,7 @@ extern "C" int rlca_safety_reduce(const rlca_env_config *cfg, const rlca_safety_
     SafetyParams q;
     int rc = safety_args(cfg, &p, ss ? ss->episodes : 0, q);
     if (rc) return rc;
-    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if ((rc = rlca_check_world_range(cfg, world_begin, world_count, "safety"))) return rc;
     if (!ev) return rlca_set_err(RLCA_ERR_INVALID, "rlca_safety_reduce: eval state is NULL");
     if (ev->episodes != ss->episodes)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_safety_reduce: the tracker holds a different number of episodes");
@@ -525,7 +499,7 @@ extern "C" int rlca_safety_reduce_host(const rlca_env_config *cfg, const float *
     SafetyParams q;
     int rc = safety_args(cfg, &p, episodes, q);
     if (rc) return rc;
-    if ((rc = check_range(cfg, world_begin, world_count))) return rc;
+    if ((rc = rlca_check_world_range(cfg, world_begin, world_count, "safety"))) return rc;
     if (!safety_records_host || !eval_records_host || !count_host || !partials_host)
         return rlca_set_err(RLCA_ERR_INVALID, "rlca_safety_reduce_host: a buffer is NULL");
     const int rows = role_mask_host ? 2 : 1;
